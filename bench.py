@@ -81,7 +81,7 @@ def measured_peak():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback: HBM3 bandwidth of the H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -293,6 +293,57 @@ def cpu_sample_text(name, n_workers, per_worker, wall, worker_s, bases):
             % (n_workers, per_worker, wall, bases / max(worker_s, 1e-9), extra))
 
 
+DUMP_BYTES = 64 << 20
+# piece fields in the dump: not op_off / ev_off, which locate a piece's script in the ops buffer -- retried unaligned reads
+# take their slot from a pool with an atomic, so those offsets differ from run to run while every output byte does not
+PIECE_FIELDS = ("n_ops", "kind", "chrom", "pos", "ref_len", "out_len", "out_rel", "l_new", "ref_req", "read_slot", "ev_n_ops",
+                "polya_len")
+
+
+def dump_outputs(out_dir, pipe, jobs, fastq, metagenome):
+    """--dump-outputs: the batches of the last timed step (``jobs``) as a caller of ns_fetch receives them -- read and
+    piece records, bases, qualities -- for a fixed, seeded sample of reads that fits DUMP_BYTES, written as
+    ``<aligned|unaligned>_{read_index,reads,pieces,seq,qual}.npy`` (float64 records, float32 bytes)."""
+    from nanosim_b200 import _lib as L
+
+    held = {(getattr(e, "_kind", None), getattr(e, "_first", None)): e for e in pipe.engines}
+    batches = [held[(kind, first)].fetch() if (kind, first) in held else None for kind, first, _ in jobs]
+    for i, (kind, first, n) in enumerate(jobs):
+        if batches[i] is None:
+            # one context ran both jobs of the step.  Outside metagenome mode a batch is a pure function of the seed and
+            # its read ids, so it is simulated again.  Metagenome batches also depend on the context's species quotas;
+            # main() refuses --depth 1 there, and with static assignment over >= 2 contexts both jobs stay held.
+            if metagenome:
+                raise RuntimeError("--dump-outputs: the last metagenome batch is no longer held by its context")
+            eng = pipe.engines[0]
+            eng.simulate(kind, first, n)
+            batches[i] = eng.fetch()
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0)
+    budget = DUMP_BYTES // len(jobs) - 4096          # per batch; 4096 covers the .npy headers
+    for (kind, _, _), b in zip(jobs, batches):
+        label = "aligned" if kind == L.NS_KIND_ALIGNED else "unaligned"
+        order = rng.permutation(len(b.reads))
+        r = b.reads[order]
+        cost = r["seq_len"].astype(np.int64) * (8 if fastq else 4) + 8 * (len(L.READ_DTYPE.names) + 1) \
+            + r["n_pieces"].astype(np.int64) * 8 * len(PIECE_FIELDS)
+        take = np.sort(order[:np.searchsorted(np.cumsum(cost), budget, side="right")])
+        reads = b.reads[take]
+        lens = reads["seq_len"].astype(np.int64)
+        starts = np.repeat(reads["seq_off"].astype(np.int64) - (np.cumsum(lens) - lens), lens)
+        bidx = starts + np.arange(int(lens.sum()))
+        npc = reads["n_pieces"].astype(np.int64)
+        pidx = np.repeat(reads["piece_first"].astype(np.int64) - (np.cumsum(npc) - npc), npc) + np.arange(int(npc.sum()))
+        out = {"read_index": take.astype(np.float64),
+               "reads": np.stack([reads[f].astype(np.float64) for f in L.READ_DTYPE.names], axis=1),
+               "pieces": np.stack([b.pieces[pidx][f].astype(np.float64) for f in PIECE_FIELDS], axis=1),
+               "seq": b.seq[bidx].astype(np.float32)}
+        if fastq:
+            out["qual"] = b.qual[bidx].astype(np.float32)
+        for name, a in out.items():
+            np.save(os.path.join(out_dir, "%s_%s.npy" % (label, name)), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -308,7 +359,15 @@ def main():
     ap.add_argument("--cpu_reads", type=int, default=0, help="reads PER WORKER in a CPU-baseline step (0 = auto)")
     ap.add_argument("--cpu_procs", type=int, default=0, help="CPU-baseline worker processes (0 = all host cores)")
     ap.add_argument("--no_cpu_baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (rank 0) to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs dumps the outputs of the CUDA path (--impl b200)")
+    if args.dump_outputs and WORKLOADS[args.workload]["mode"] == "metagenome" and args.depth < 2:
+        ap.error("--dump-outputs in metagenome mode needs --depth >= 2 (one context would run both batches of the last step)")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -434,7 +493,7 @@ def main():
 
     # ---- kernel-only arm: outputs stay in HBM.  `depth` contexts (ns_clone) share the reference; the latency-bound tails
     #      of one batch's plan / unaligned kernels overlap the emit kernel of another.  Every step simulates new read ids;
-    #      a batch's working set (GBs written + a reference sampled at random) is far larger than the 126 MB L2 (config 1,
+    #      a batch's working set (GBs written + a reference sampled at random) is far larger than the 50 MB L2 (config 1,
     #      a 5 Mb reference and 9 MB of output per step, is the exception: the reference's own tiny case).
     pipe = BatchPipeline(eng, depth=args.depth, fetch=False)
     clocks = ClockSampler(local)
@@ -448,6 +507,8 @@ def main():
     barrier()
     wall = time.perf_counter() - t0
     clocks.window(t0, t0 + wall, "kernel-only arm")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pipe, jobs_for([total_steps - 1]), W["fastq"], W["mode"] == "metagenome")
     pipe.close()
     if args.timeline and rank == 0:
         with open(args.timeline, "w") as f:       # phases are back to back on a context's stream: begin + cumulative durations

@@ -1,5 +1,5 @@
 /*
- * nanosim_b200 -- C ABI of the B200-native per-read simulation path of NanoSim.
+ * nanosim_b200 -- C ABI of the H100-native (sm_90a) per-read simulation path of NanoSim.
  *
  * The reference (bcgsc/NanoSim, pure Python) has no FFI: the seam this library replaces is the Python call
  *

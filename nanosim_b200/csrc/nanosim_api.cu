@@ -84,7 +84,7 @@ struct NsContext {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     std::string err;
-    int sm_count = 148;
+    int sm_count = 0;               // ns_create: cudaDeviceProp::multiProcessorCount
 
     bool borrowed = false;          // ns_clone: reference + model buffers belong to the parent
     bool have_ref = false, have_model = false, have_cfg = false;
@@ -128,12 +128,10 @@ struct NsContext {
 };
 
 // Wait for everything queued on the context's stream.  cudaStreamSynchronize spins: a host thread per overlapped context then
-// burns a core for the whole 20-100 ms of a big batch.  The boxes of this pool grant their GPU processes a CPU quota (16 cores
-// for 1 GPU, 24 for 2, 96 logical for 8), and per-GPU end-to-end throughput fell with the number of GPU processes (39 / 30 /
-// 16 Gbases/s) although no PCIe link was saturated and the expansion of the 2-bit bases takes 19 ms of a 100 ms fetch: four
-// spinning threads per process are the largest CPU consumer left.  With several GPU processes on the host (torchrun's
-// LOCAL_WORLD_SIZE > 1, or NANOSIM_B200_BLOCKING_SYNC=1) long waits therefore sleep on a cudaEventBlockingSync event; a single
-// process, and every short wait, spins as before.  (Written after the round's GPU minutes were spent: not measured.)
+// burns a core for the whole of a big batch.  GPU processes that share a host under a CPU quota also need that CPU time for
+// the expansion of the 2-bit bases in ns_fetch, so with several GPU processes on the host (torchrun's LOCAL_WORLD_SIZE > 1,
+// or NANOSIM_B200_BLOCKING_SYNC=1) long waits sleep on a cudaEventBlockingSync event; a single process, and every short
+// wait, spins as before.  Not measured on H100.
 static bool blocking_sync_wanted() {
     static const bool want = [] {
         if (const char* e = getenv("NANOSIM_B200_BLOCKING_SYNC")) return atoi(e) != 0;
@@ -1251,9 +1249,9 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     pa.batch_reversed = batch_reversed;
     pa.abort = d_abort;
     const unsigned plan_tb = 128;
-    // 2 resident blocks per SM: measured faster than 4 (the register limit) both alone (6.3-6.8 vs 8.2-8.6 ms on the config-2
-    // batch) and next to another context's emit kernel, which then still finds room on every SM
-    // (transcripts are short -- 1-2 kb reads, no long tail, two passes: there the register limit of 4 blocks is better)
+    // 2 resident blocks per SM rather than 4 (the register limit): the kernel is bound by the latency of its table lookups,
+    // and another context's emit kernel still finds room on every SM (transcripts are short -- 1-2 kb reads, no long tail,
+    // two passes: there the register limit of 4 blocks is used).  DESIGN.md §10 has the H100 comparison.
     static const int plan_per_sm_env = env_int("NANOSIM_B200_PLAN_BLOCKS_PER_SM", 0);
     const int plan_per_sm = plan_per_sm_env > 0 ? plan_per_sm_env : (ctx->dcfg.transcriptome ? 4 : 2);
     unsigned plan_blocks = std::min<unsigned>((n + plan_tb - 1) / plan_tb, (unsigned)ctx->sm_count * (unsigned)std::max(1, plan_per_sm));
@@ -1577,8 +1575,8 @@ void unpack_bases(const uint8_t* packed, uint8_t* seq, uint64_t seq_bytes, bool 
     for (uint64_t k = whole * 8; k < seq_bytes; ++k) seq[k] = (uint8_t)abc[(packed[k >> 2] >> (2 * (k & 3))) & 3u];
 }
 
-// CPUs this process can really use: the affinity mask, capped by the container's cgroup CPU quota (cpu.max) -- the boxes of
-// this pool show 128 logical CPUs and grant 16-24 cores of CPU time
+// CPUs this process can really use: the affinity mask, capped by the container's cgroup CPU quota (cpu.max) -- a container
+// can show many more logical CPUs than its quota grants
 unsigned effective_cpus() {
     unsigned n = std::thread::hardware_concurrency();
     cpu_set_t set;

@@ -440,7 +440,7 @@ __device__ __forceinline__ uint32_t uread_one(const UreadArgs& a, uint2 key, uin
 }
 
 #ifndef UREAD_MIN_BLOCKS
-#define UREAD_MIN_BLOCKS 3          // 80 registers: 24 warps per SM hide the shuffle chains better than 16 (-7 % measured)
+#define UREAD_MIN_BLOCKS 3          // 80 registers: 24 warps per SM to hide the shuffle chains (not re-measured on H100)
 #endif
 template <bool REPLAY>
 __global__ void __launch_bounds__(UREAD_WARPS * 32, UREAD_MIN_BLOCKS) uread_kernel(const __grid_constant__ UreadArgs a) {

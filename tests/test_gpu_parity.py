@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: ``pytest -m gpu``).  Everything goes through the C ABI.
+"""GPU parity tests (run on an H100: ``pytest -m gpu``).  Everything goes through the C ABI.
 
  * bit-exact: every edit script re-applied on the host reproduces the device's bases (mutate_read semantics);
    same seed -> same bytes; results independent of the batch split;

@@ -122,28 +122,76 @@ def test_compiled_model_roundtrip(tmp_path, compiled_models):
         assert np.array_equal(cm.kde[k][0], cm2.kde[k][0]) and cm.kde[k][1] == cm2.kde[k][1]
 
 
-REF_MODELS = "/root/reference/pre-trained_models"
+def _new_obj(cls):
+    return cls.__new__(cls)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_MODELS), reason="the reference's pre-trained models are only present in the build container")
-@pytest.mark.parametrize("tarball,prefix,shipped", [
-    ("human_NA12878_DNA_FAB49712_guppy.tar.gz", "human_NA12878_DNA_FAB49712_guppy/training", "guppy_fab49712_plusq.npz"),
-    ("human_NA12878_DNA_FAB49712_guppy_flipflop.tar.gz", "human_NA12878_DNA_FAB49712_guppy_flipflop/training", None),
-    ("human_giab_hg002_sub1M_kitv14_dorado.tar.gz", "human_giab_hg002_sub1M_kitv14_dorado/hg002_nanosim_sub1M", None),
-])
-def test_reference_model_directories_load_and_tabulate(tmp_path, tarball, prefix, shipped):
-    """`-c <model_dir>/<prefix>` on the reference's own model archives: text tables + sklearn KDE pickles -> device tables;
-    the shipped .npz is a lossless copy of the directory it was compiled from (plus the quality table of config 2)."""
-    import tarfile
+class _EuclideanDistance:
+    pickled_as = ("sklearn.neighbors._dist_metrics", "EuclideanDistance")
+
+    def __reduce__(self):
+        return _new_obj, (_EuclideanDistance,), (2.0, np.zeros(0), np.zeros((0, 0)))
+
+
+class _KDTree:
+    """The KDTree inside a scikit-learn 0.22/0.23 KernelDensity pickles as newObj(KDTree) + BinaryTree.__getstate__: (data,
+    idx_array, node_data, node_bounds, leaf_size, n_levels, n_nodes, n_trims, n_leaves, n_splits, n_calls, dist_metric)."""
+    pickled_as = ("sklearn.neighbors._kd_tree", "KDTree")
+
+    def __init__(self, data):
+        self.data = data
+
+    def __reduce__(self):
+        node = np.zeros(1, dtype=[("idx_start", "<i8"), ("idx_end", "<i8"), ("is_leaf", "<i8"), ("radius", "<f8")])
+        bounds = np.stack([self.data.min(0), self.data.max(0)])[:, None, :]
+        state = (self.data, np.arange(len(self.data), dtype=np.int64), node, bounds, 40, 1, 1, 0, 1, 0, 0,
+                 _EuclideanDistance())
+        return _new_obj, (_KDTree,), state
+
+
+class _KernelDensity:
+    pickled_as = ("sklearn.neighbors._kde", "KernelDensity")
+
+    def __init__(self, data, bandwidth):
+        self.__dict__.update(algorithm="auto", atol=0, bandwidth=bandwidth, breadth_first=True, kernel="gaussian",
+                             leaf_size=40, metric="euclidean", metric_params=None, rtol=0, tree_=_KDTree(data))
+
+
+_new_obj.pickled_as = ("sklearn.neighbors._kd_tree", "newObj")
+
+
+def _dump_kde(path, data, bandwidth):
+    """A ``<prefix>_<kde>.pkl`` as the reference's training writes it (joblib.dump of a KernelDensity), without sklearn."""
+    import pickle
+    from joblib.numpy_pickle import NumpyPickler
+
+    class _Pickler(NumpyPickler):
+        def save_global(self, obj, name=None):
+            if not hasattr(obj, "pickled_as"):
+                return super().save_global(obj, name)
+            self.write(pickle.GLOBAL + ("%s\n%s\n" % obj.pickled_as).encode())
+            self.memoize(obj)
+
+    with open(path, "wb") as f:
+        _Pickler(f, protocol=2).dump(_KernelDensity(data, bandwidth))
+
+
+@pytest.mark.parametrize("tag,prefix", [("guppy", "training"), ("dorado", "hg002_nanosim_sub1M")])   # the archives' prefixes
+def test_reference_model_directories_load_and_tabulate(tmp_path, tag, prefix):
+    """`-c <model_dir>/<prefix>` on a model directory in the reference's format -- text tables + KernelDensity pickles --
+    written from a shipped .npz: it loads back to exactly that model and tabulates into device tables."""
+    from conftest import MODEL_FILES
     from nanosim_b200.model import CompiledModel, DeviceTables, load_model
-    with tarfile.open(os.path.join(REF_MODELS, tarball)) as tf:
-        tf.extractall(str(tmp_path), filter="data")
-    cm = load_model(os.path.join(str(tmp_path), prefix))
+    ours = CompiledModel.load(os.path.join(DATA, MODEL_FILES[tag]))
+    prefix = os.path.join(str(tmp_path), prefix)
+    for k, v in ours.text.items():
+        with open(prefix + "_" + k, "w") as f:
+            f.write(v)
+    for k, (data, bw) in ours.kde.items():
+        _dump_kde(prefix + "_" + k + ".pkl", data, bw)
+    cm = load_model(prefix)
     t = DeviceTables(cm, fastq=False, chimeric="chimeric_info" in cm.text)
     assert len(t.alias_prob) > 1000 and len(cm.kde) >= 5
-    if shipped:
-        ours = CompiledModel.load(os.path.join(DATA, shipped))
-        for k, v in cm.text.items():
-            assert ours.text[k] == v, k
-        for k, (data, bw) in cm.kde.items():
-            assert np.array_equal(ours.kde[k][0], data) and ours.kde[k][1] == bw, k
+    assert cm.text == ours.text and sorted(cm.kde) == sorted(ours.kde)
+    for k, (data, bw) in cm.kde.items():
+        assert np.array_equal(ours.kde[k][0], data) and ours.kde[k][1] == bw, k
