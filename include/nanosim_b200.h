@@ -205,7 +205,8 @@ typedef struct {
     uint64_t total_bases;     /* sum of seq_len */
     uint32_t n_reads;
     uint32_t n_pieces;
-    uint32_t n_launches;      /* kernels launched for this batch (ours + the two CUB scan kernels per scan) */
+    uint32_t n_launches;      /* launches for this batch (and ns_reemit on it): one per kernel of this library, one per CUB
+                               * scan, one per CUB sort; memsets and copies are not counted */
     /* CUDA-event durations on the library's stream: set-up (segment counts, buffer growth), plan pass 1 (rejection
      * loops + counts), scans + host round trip of the totals, plan pass 2 (edit scripts), emit, and the whole batch */
     float ms_setup, ms_plan, ms_scan, ms_script, ms_emit, ms_total;

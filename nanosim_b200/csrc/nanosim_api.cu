@@ -19,6 +19,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 #include <string>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <vector>
@@ -39,9 +40,16 @@
 
 namespace {
 
+// Device memory, page-locked host memory and events belong to exactly one owner, which frees them: none of them is copied.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() {
+        if (p) cudaFree(p);
+    }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -68,12 +76,60 @@ struct DevBuf {
         cap = want;
         return e;
     }
-    void release() {
-        if (p) cudaFree(p);
+    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+struct PinnedBuf {
+    void* p = nullptr;
+    size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() {
+        if (p) cudaFreeHost(p);
+    }
+    cudaError_t ensure(size_t bytes, unsigned flags) {
+        if (bytes <= cap) return cudaSuccess;
+        if (p) cudaFreeHost(p);
         p = nullptr;
         cap = 0;
+        size_t want = bytes + bytes / 8 + 4096;
+        cudaError_t e = cudaHostAlloc(&p, want, flags);
+        if (e == cudaSuccess) cap = want;
+        return e;
     }
     template <class T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() {
+        if (e) cudaEventDestroy(e);
+    }
+    operator cudaEvent_t() const { return e; }
+};
+
+// Reference and model tables in HBM.  A context and its clones (ns_clone) hold one copy; only the context that created
+// it sets them.
+struct Tables {
+    bool have_ref = false, have_model = false, have_expr = false;
+    DevBuf ref_bases, ref_off, ref_packed, ref_pk_off, ref_exc, ref_species, ref_circular, ref_sp_off;
+    DevBuf kde[5], alias, qlut, kde2d_x, kde2d_y, expr_alias, expr_chrom, chrom_polya;
+    std::vector<uint64_t> h_chrom_off;
+    std::vector<uint32_t> h_sp_off;
+    DevRef dref{};                  // without the transcript-length table: that one is per context (NsContext::trx)
+    DevModel dmodel{};
+    NsModel hmodel{};
+};
+
+// transcript lengths ascending + their record indices (ns_configure, transcriptome mode); a clone that configures another
+// record count builds its own
+struct TrxTable {
+    DevBuf buf;
+    uint32_t n = 0;
 };
 
 }  // namespace
@@ -82,40 +138,30 @@ struct NsContext {
     int device = 0;
     uint64_t seed = 0;
     cudaStream_t stream = nullptr;
-    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    Event ev[6];
     std::string err;
     int sm_count = 0;               // ns_create: cudaDeviceProp::multiProcessorCount
 
-    bool borrowed = false;          // ns_clone: reference + model buffers belong to the parent
-    bool have_ref = false, have_model = false, have_cfg = false;
-    DevBuf ref_bases, ref_off, ref_packed, ref_pk_off, ref_exc;
-    DevBuf trx_sorted;              // transcript lengths ascending + their records (ns_configure, transcriptome mode)
-    bool trx_sorted_owned = false;  // false on a clone that still uses its parent's table
-    DevRef dref{};
-    std::vector<uint64_t> h_chrom_off;
-
-    DevBuf kde[5], alias, qlut, ref_species, ref_circular, ref_sp_off, kde2d_x, kde2d_y, expr_alias, expr_chrom, chrom_polya;
-    bool have_expr = false;
-    std::vector<uint32_t> h_sp_off;
-    std::vector<double> abun, abun_inflated, species_bases;     // metagenome: dict_abun, dict_abun_inflated, running totals
-    DevBuf sp_bases_dev;
-    DevModel dmodel{};
-    NsModel hmodel{};
+    std::shared_ptr<Tables> tables = std::make_shared<Tables>();
+    bool clone = false;             // ns_clone: the tables are the parent's, and only the parent sets them
+    bool have_cfg = false;
     NsRunConfig hcfg{};
     DevCfg dcfg{};
+    std::shared_ptr<const TrxTable> trx;
+    std::vector<double> abun, abun_inflated, species_bases;     // metagenome: dict_abun, dict_abun_inflated, running totals
+    DevBuf sp_bases_dev;
 
     // batch state
     DevBuf split_base, split_extra, split_ckpt, hp_keys;     // long pieces -> extra emit work items (emit_kernel.cuh:split_kernel)
     DevBuf reads, pieces, ops, seq, qual, nseg, npieces, piece_first, scan_in, scan_out, scan_tmp, counter, totals,
         stats, sort_keys, sort_vals, sort_tmp, hp_off;
-    uint64_t* h_totals = nullptr;   // pinned + mapped
+    PinnedBuf h_totals;             // mapped
     uint64_t* h_totals_dev = nullptr;
     // ns_fetch sends bases over PCIe as 2 bits each: device pack buffer, pinned staging, event after its copy
     DevBuf pack_dev;
-    uint8_t* pack_host = nullptr;
-    size_t pack_host_cap = 0;
-    cudaEvent_t ev_pack = nullptr;
-    cudaEvent_t ev_block = nullptr;     // cudaEventBlockingSync: long waits sleep instead of spinning (wait_stream)
+    PinnedBuf pack_host;
+    Event ev_pack;
+    Event ev_block;                 // cudaEventBlockingSync: long waits sleep instead of spinning (wait_stream)
     // Batches of one job have near-identical sizes: once a batch of a kind has run with host-sized buffers, the next ones
     // are submitted in one go (no host round trip between the first and the last kernel) against those capacities; a
     // kernel checks them on the device and a batch that does not fit is simply run again the sized way.
@@ -125,6 +171,10 @@ struct NsContext {
     int last_kind = 0;
     uint64_t last_first_id = 0;
     bool have_batch = false;
+
+    ~NsContext() {
+        if (stream) cudaStreamDestroy(stream);
+    }
 };
 
 // Wait for everything queued on the context's stream.  cudaStreamSynchronize spins: a host thread per overlapped context then
@@ -143,7 +193,7 @@ static bool blocking_sync_wanted() {
 static cudaError_t wait_stream(NsContext* ctx, bool long_wait) {
     if (!long_wait || !blocking_sync_wanted()) return cudaStreamSynchronize(ctx->stream);
     cudaError_t e = cudaSuccess;
-    if (!ctx->ev_block) e = cudaEventCreateWithFlags(&ctx->ev_block, cudaEventBlockingSync | cudaEventDisableTiming);
+    if (!ctx->ev_block) e = cudaEventCreateWithFlags(&ctx->ev_block.e, cudaEventBlockingSync | cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_block, ctx->stream);
     if (e == cudaSuccess) e = cudaEventSynchronize(ctx->ev_block);
     return e;
@@ -188,9 +238,9 @@ __global__ void gather_flagged_ops(const NsPieceMeta* pieces, const NsReadMeta* 
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = (reads[pieces[i].read_slot].flags & 1u) ? pieces[i].n_ops : 0u;
 }
-__global__ void scatter_flagged_off(NsPieceMeta* pieces, const NsReadMeta* reads, uint32_t n, const uint64_t* off, uint64_t base) {
+__global__ void scatter_flagged_off(NsPieceMeta* pieces, const NsReadMeta* reads, uint32_t n, const uint64_t* off, const uint64_t* base) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && (reads[pieces[i].read_slot].flags & 1u)) pieces[i].op_off = base + off[i];
+    if (i < n && (reads[pieces[i].read_slot].flags & 1u)) pieces[i].op_off = *base + off[i];
 }
 __global__ void copy_ev_fields(NsPieceMeta* pieces, uint32_t n) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -275,10 +325,6 @@ __global__ void capacity_stage_b(uint64_t* totals, uint64_t ops_cap, uint64_t se
     if (threadIdx.x || blockIdx.x) return;
     if (totals[NS_T_PRIMARY] + totals[1] + 4 > ops_cap) totals[NS_T_ABORT] |= 2u;
     if (totals[2] + 16 > seq_cap) totals[NS_T_ABORT] |= 4u;
-}
-__global__ void scatter_flagged_off_dev(NsPieceMeta* pieces, const NsReadMeta* reads, uint32_t n, const uint64_t* off, const uint64_t* base) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && (reads[pieces[i].read_slot].flags & 1u)) pieces[i].op_off = *base + off[i];
 }
 __global__ void gather_read_bytes(const NsReadMeta* reads, uint32_t n, uint64_t* out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -465,6 +511,131 @@ void build_qlut(const uint32_t cdf32[NS_N_QUAL_STATES][NS_QUAL_SLOTS], std::vect
     }
 }
 
+// The steps of a batch.  Every kernel, CUB scan and CUB sort of a batch is counted in NsBatchInfo.n_launches here.
+template <class... P, class... A>
+cudaError_t launch(NsContext* ctx, void (*kernel)(P...), unsigned grid, unsigned block, size_t smem, A... args) {
+    kernel<<<grid, block, smem, ctx->stream>>>(args...);
+    ++ctx->last.n_launches;
+    return cudaGetLastError();
+}
+
+// out = exclusive prefix sum of in[0, n); totals[slot] = the sum of all n
+int scan_total(NsContext* ctx, const uint64_t* in, uint64_t* out, uint32_t n, int slot) {
+    size_t tmp = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, in, out, (int)n, ctx->stream));
+    CK(ctx->scan_tmp.ensure(tmp));
+    CK(cub::DeviceScan::ExclusiveSum(ctx->scan_tmp.p, tmp, in, out, (int)n, ctx->stream));
+    ++ctx->last.n_launches;
+    CK(launch(ctx, last_total, 1, 32, 0, in, out, n, ctx->totals.as<uint64_t>(), slot));
+    return NS_OK;
+}
+
+// a 16-byte aligned sequence slot per read: reads[i].seq_off, totals[2] = sequence bytes, totals[3] = bases
+int read_layout(NsContext* ctx, uint32_t n) {
+    const unsigned gb = (n + 255) / 256;
+    NsReadMeta* reads = ctx->reads.as<NsReadMeta>();
+    uint64_t* totals = ctx->totals.as<uint64_t>();
+    CK(launch(ctx, gather_read_bytes, gb, 256, 0, reads, n, ctx->scan_in.as<uint64_t>()));
+    if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n, 2)) return rc;
+    CK(launch(ctx, scatter_read_off, gb, 256, 0, reads, n, ctx->scan_out.as<uint64_t>()));
+    CK(cudaMemsetAsync(totals + 3, 0, sizeof(uint64_t), ctx->stream));
+    CK(launch(ctx, sum_bases, std::min(gb, 1024u), 256, 0, reads, n, (unsigned long long*)(totals + 3)));
+    return NS_OK;
+}
+
+int sort_pairs_descending(NsContext* ctx, const uint32_t* keys_in, uint32_t* keys_out, const uint32_t* vals_in, uint32_t* vals_out,
+                          uint32_t n) {
+    size_t tmp = 0;
+    CK(cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, keys_in, keys_out, vals_in, vals_out, (int)n, 0, 32, ctx->stream));
+    CK(ctx->sort_tmp.ensure(tmp));
+    CK(cub::DeviceRadixSort::SortPairsDescending(ctx->sort_tmp.p, tmp, keys_in, keys_out, vals_in, vals_out, (int)n, 0, 32, ctx->stream));
+    ++ctx->last.n_launches;
+    return NS_OK;
+}
+
+// the host reads the batch totals (h_totals) after this
+int publish_totals_and_wait(NsContext* ctx, bool long_wait = false) {
+    CK(launch(ctx, publish_totals, 1, 32, 0, ctx->totals.as<uint64_t>(), ctx->h_totals_dev));
+    CK(wait_stream(ctx, long_wait));
+    return NS_OK;
+}
+
+// the reference as the kernels see it: the shared tables plus this context's transcript-length table
+DevRef dev_ref(const NsContext* ctx) {
+    DevRef r = ctx->tables->dref;
+    if (ctx->trx) {
+        r.trx_len_sorted = ctx->trx->buf.as<uint32_t>();
+        r.trx_len_idx = r.trx_len_sorted + ctx->trx->n;
+        r.n_trx_sorted = ctx->trx->n;
+    }
+    return r;
+}
+
+// emit_kernel over `n_pieces` pieces of the context's current batch (all of them, or the ones `order` lists)
+int launch_emit(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_pieces, const uint32_t* order,
+                const uint32_t* abort_flag = nullptr, bool split = true, cudaEvent_t emit_begin = nullptr) {
+    cudaStream_t st = ctx->stream;
+    EmitArgs ea;
+    ea.ref = dev_ref(ctx);
+    ea.cfg = ctx->dcfg;
+    ea.kind = (uint32_t)kind;
+    ea.first_id = first_read_id;
+    ea.reads = ctx->reads.as<NsReadMeta>();
+    ea.pieces = ctx->pieces.as<NsPieceMeta>();
+    ea.ops = ctx->ops.as<uint32_t>();
+    ea.n_pieces = n_pieces;
+    ea.seq = ctx->seq.as<uint8_t>();
+    ea.qual = ctx->qual.as<uint8_t>();
+    ea.qlut = ctx->tables->qlut.as<uint32_t>();
+    ea.force_exact = (ctx->hcfg.flags & NS_FLAG_EMIT_EXACT) ? 1u : 0u;
+    ea.abort = abort_flag;
+    ea.counter = ctx->counter.as<uint32_t>();
+    ea.order = order;
+    CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
+    {   // long pieces become several work items.  Capacity: every extra item stands for EMIT_SPLIT - 16 or more output bytes
+        // of its piece, and a batch's output fits the sequence buffer (checked on the device for sync-free batches).
+        const uint32_t cap_extra = (uint32_t)std::min<size_t>(ctx->seq.cap / (EMIT_SPLIT - 16u) + 64u, 0x7fffffffu);
+        ea.split_base = nullptr;
+        ea.extra = nullptr;
+        ea.ckpt = nullptr;
+        ea.n_extra = ctx->counter.as<uint32_t>() + 4;
+        ea.cap_extra = cap_extra;
+        if (split && n_pieces && !(ctx->hcfg.flags & NS_FLAG_EMIT_WHOLE)) {     // (`order` lists pieces below n_pieces whenever split is asked for)
+            CK(ctx->split_base.ensure((size_t)n_pieces * sizeof(uint32_t)));
+            CK(ctx->split_extra.ensure((size_t)cap_extra * sizeof(uint2)));
+            CK(ctx->split_ckpt.ensure((size_t)cap_extra * sizeof(uint4)));
+            CK(cudaMemsetAsync(ctx->split_extra.p, 0xff, (size_t)cap_extra * sizeof(uint2), st));
+            SplitArgs sa;
+            sa.reads = ea.reads;
+            sa.pieces = ea.pieces;
+            sa.ops = ea.ops;
+            sa.n_pieces = n_pieces;
+            sa.split_base = ctx->split_base.as<uint32_t>();
+            sa.extra = ctx->split_extra.as<uint2>();
+            sa.ckpt = ctx->split_ckpt.as<uint4>();
+            sa.n_extra = ctx->counter.as<uint32_t>() + 4;
+            sa.cap_extra = cap_extra;
+            sa.abort = abort_flag;
+            const unsigned sblocks = std::min<unsigned>((n_pieces + 7u) / 8u, (unsigned)ctx->sm_count * 8u);
+            CK(launch(ctx, split_kernel, sblocks, 256, 0, sa));
+            if (emit_begin) CK(cudaEventRecord(emit_begin, st));     // the emit phase of the batch timings starts after the split
+            ea.split_base = sa.split_base;
+            ea.extra = sa.extra;
+            ea.ckpt = sa.ckpt;
+        }
+    }
+    // FASTQ: the quality tables go to shared memory as well
+    void (*kernel)(EmitArgs) = ctx->hcfg.fastq ? emit_kernel<true> : emit_kernel<false>;
+    const size_t smem = (size_t)EMIT_WARPS * EMIT_RING * sizeof(uint4) + 512 + EMIT_WINDOW_SMEM +
+                        (ctx->hcfg.fastq ? (size_t)NS_N_QUAL_STATES * QLUT_SIZE * 4 : 0);
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 1;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, EMIT_WARPS * 32, smem));
+    const unsigned blocks = std::min<unsigned>((n_pieces + EMIT_WARPS - 1) / EMIT_WARPS, (unsigned)(ctx->sm_count * std::max(per_sm, 1)));
+    CK(launch(ctx, kernel, blocks, EMIT_WARPS * 32, smem, ea));
+    return NS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -477,9 +648,9 @@ int ns_create(int device, uint64_t seed, NsContext** out) {
     ctx->seed = seed;
     cudaError_t e = cudaSetDevice(device);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
-    for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = cudaEventCreate(&ctx->ev[i]);
-    if (e == cudaSuccess) e = cudaHostAlloc((void**)&ctx->h_totals, 16 * sizeof(uint64_t), cudaHostAllocMapped);
-    if (e == cudaSuccess) e = cudaHostGetDevicePointer((void**)&ctx->h_totals_dev, ctx->h_totals, 0);
+    for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = cudaEventCreate(&ctx->ev[i].e);
+    if (e == cudaSuccess) e = ctx->h_totals.ensure(16 * sizeof(uint64_t), cudaHostAllocMapped);
+    if (e == cudaSuccess) e = cudaHostGetDevicePointer((void**)&ctx->h_totals_dev, ctx->h_totals.p, 0);
     if (e == cudaSuccess && device >= 0 && device < 64 && !g_base[device]) {
         e = cudaEventCreate(&g_base[device]);
         if (e == cudaSuccess) e = cudaEventRecord(g_base[device], ctx->stream);
@@ -503,29 +674,6 @@ int ns_destroy(NsContext* ctx) {
     if (!ctx) return NS_EINVAL;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    DevBuf* bufs[] = {&ctx->ref_bases, &ctx->ref_off, &ctx->ref_packed, &ctx->ref_pk_off, &ctx->ref_exc, &ctx->alias, &ctx->qlut, &ctx->reads, &ctx->pieces,
-                      &ctx->ops, &ctx->seq, &ctx->qual, &ctx->nseg, &ctx->npieces, &ctx->piece_first, &ctx->scan_in,
-                      &ctx->scan_out, &ctx->scan_tmp, &ctx->counter, &ctx->totals, &ctx->stats, &ctx->sort_keys, &ctx->sort_vals,
-                      &ctx->sort_tmp, &ctx->hp_off, &ctx->ref_species, &ctx->ref_circular, &ctx->ref_sp_off, &ctx->sp_bases_dev, &ctx->kde2d_x, &ctx->kde2d_y,
-                      &ctx->expr_alias, &ctx->expr_chrom, &ctx->chrom_polya, &ctx->split_base, &ctx->split_extra, &ctx->split_ckpt, &ctx->hp_keys};
-    if (ctx->borrowed) {            // shared with the parent: drop the pointers without freeing
-        DevBuf* shared[] = {&ctx->ref_bases, &ctx->ref_off, &ctx->ref_packed, &ctx->ref_pk_off, &ctx->ref_exc, &ctx->alias, &ctx->qlut, &ctx->ref_species,
-                            &ctx->ref_circular, &ctx->ref_sp_off, &ctx->kde2d_x, &ctx->kde2d_y, &ctx->expr_alias,
-                            &ctx->expr_chrom, &ctx->chrom_polya};
-        for (DevBuf* b : shared) { b->p = nullptr; b->cap = 0; }
-        for (auto& k : ctx->kde) { k.p = nullptr; k.cap = 0; }
-    }
-    if (ctx->trx_sorted_owned) ctx->trx_sorted.release();
-    for (DevBuf* b : bufs) b->release();
-    for (auto& k : ctx->kde) k.release();
-    if (ctx->h_totals) cudaFreeHost(ctx->h_totals);
-    if (ctx->pack_host) cudaFreeHost(ctx->pack_host);
-    ctx->pack_dev.release();
-    if (ctx->ev_pack) cudaEventDestroy(ctx->ev_pack);
-    if (ctx->ev_block) cudaEventDestroy(ctx->ev_block);
-    for (auto& e : ctx->ev)
-        if (e) cudaEventDestroy(e);
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
     return NS_OK;
 }
@@ -537,38 +685,15 @@ int ns_clone(NsContext* parent, NsContext** out) {
     NsContext* c = nullptr;
     int rc = ns_create(parent->device, parent->seed, &c);
     if (rc != NS_OK) return rc;
-    c->borrowed = true;
-    c->have_ref = parent->have_ref;
-    c->have_model = parent->have_model;
+    c->tables = parent->tables;
+    c->clone = true;
     c->have_cfg = parent->have_cfg;
-    c->ref_bases = parent->ref_bases;      // plain pointer copies; ns_destroy() of a clone does not free them
-    c->ref_off = parent->ref_off;
-    c->ref_packed = parent->ref_packed;
-    c->ref_pk_off = parent->ref_pk_off;
-    c->ref_exc = parent->ref_exc;
-    c->trx_sorted = parent->trx_sorted;        // shared; trx_sorted_owned stays false
-    c->alias = parent->alias;
-    c->qlut = parent->qlut;
-    c->ref_species = parent->ref_species;
-    c->ref_circular = parent->ref_circular;
-    c->ref_sp_off = parent->ref_sp_off;
-    c->kde2d_x = parent->kde2d_x;
-    c->kde2d_y = parent->kde2d_y;
-    c->expr_alias = parent->expr_alias;
-    c->expr_chrom = parent->expr_chrom;
-    c->chrom_polya = parent->chrom_polya;
-    c->have_expr = parent->have_expr;
-    c->h_sp_off = parent->h_sp_off;
+    c->hcfg = parent->hcfg;
+    c->dcfg = parent->dcfg;
+    c->trx = parent->trx;
     c->abun = parent->abun;
     c->abun_inflated = parent->abun_inflated;
     c->species_bases.assign(parent->abun.size(), 0.0);      // every clone is its own worker (own running totals)
-    for (int i = 0; i < 5; ++i) c->kde[i] = parent->kde[i];
-    c->dref = parent->dref;
-    c->h_chrom_off = parent->h_chrom_off;
-    c->dmodel = parent->dmodel;
-    c->hmodel = parent->hmodel;
-    c->hcfg = parent->hcfg;
-    c->dcfg = parent->dcfg;
     *out = c;
     return NS_OK;
 }
@@ -576,69 +701,68 @@ int ns_clone(NsContext* parent, NsContext** out) {
 int ns_set_reference(NsContext* ctx, const NsReference* ref) {
     if (!ctx || !ref || !ref->bases || !ref->chrom_off || ref->n_chrom == 0)
         return fail(ctx, NS_EINVAL, "ns_set_reference: null argument or empty reference");
-    if (ctx->borrowed) return fail(ctx, NS_ESTATE, "ns_set_reference: a cloned context shares its parent's reference");
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "ns_set_reference: a cloned context shares its parent's reference");
     CK(cudaSetDevice(ctx->device));
-    ctx->h_chrom_off.resize(ref->n_chrom + 1);
-    CK(cudaMemcpy(ctx->h_chrom_off.data(), ref->chrom_off, (ref->n_chrom + 1) * sizeof(uint64_t), cudaMemcpyDefault));
-    if (ctx->h_chrom_off[0] != 0 || ctx->h_chrom_off[ref->n_chrom] != ref->n_bases)
+    Tables& tab = *ctx->tables;
+    tab.h_chrom_off.resize(ref->n_chrom + 1);
+    CK(cudaMemcpy(tab.h_chrom_off.data(), ref->chrom_off, (ref->n_chrom + 1) * sizeof(uint64_t), cudaMemcpyDefault));
+    if (tab.h_chrom_off[0] != 0 || tab.h_chrom_off[ref->n_chrom] != ref->n_bases)
         return fail(ctx, NS_EINVAL, "ns_set_reference: chrom_off must start at 0 and end at n_bases");
     for (uint32_t i = 0; i < ref->n_chrom; ++i) {
-        uint64_t len = ctx->h_chrom_off[i + 1] - ctx->h_chrom_off[i];
-        if (ctx->h_chrom_off[i + 1] < ctx->h_chrom_off[i] || len > 0xffffffffull)
+        uint64_t len = tab.h_chrom_off[i + 1] - tab.h_chrom_off[i];
+        if (tab.h_chrom_off[i + 1] < tab.h_chrom_off[i] || len > 0xffffffffull)
             return fail(ctx, NS_EINVAL, "ns_set_reference: chromosome %u has an invalid length", i);
     }
-    CK(upload(ctx->ref_bases, ref->bases, ref->n_bases, ctx->stream));
-    CK(upload(ctx->ref_off, ctx->h_chrom_off.data(), (ref->n_chrom + 1) * sizeof(uint64_t), ctx->stream));
+    CK(upload(tab.ref_bases, ref->bases, ref->n_bases, ctx->stream));
+    CK(upload(tab.ref_off, tab.h_chrom_off.data(), (ref->n_chrom + 1) * sizeof(uint64_t), ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->dref.bases = ctx->ref_bases.as<uint8_t>();
-    ctx->dref.chrom_off = ctx->ref_off.as<uint64_t>();
+    tab.dref.bases = tab.ref_bases.as<uint8_t>();
+    tab.dref.chrom_off = tab.ref_off.as<uint64_t>();
     {   // 2-bit copy + exception counts for the emit kernel's fast path
         std::vector<uint64_t> pk(ref->n_chrom + 1);
         uint64_t words = 1;                                             // guard word in front
         for (uint32_t i = 0; i < ref->n_chrom; ++i) {
             pk[i] = words;
-            words += (ctx->h_chrom_off[i + 1] - ctx->h_chrom_off[i] + 15) / 16;
+            words += (tab.h_chrom_off[i + 1] - tab.h_chrom_off[i] + 15) / 16;
         }
         pk[ref->n_chrom] = words;
         const uint64_t n_blocks = ((words + 2) >> REF_EXC_BLOCK_SHIFT) + 2;
-        CK(ctx->ref_packed.ensure((size_t)(words + 2 + 64) * 4));      // + slack: a 64-word window copy may start at the last word
-        CK(ctx->ref_exc.ensure((size_t)(2 * n_blocks + 2) * 4 + 16));
-        CK(upload(ctx->ref_pk_off, pk.data(), pk.size() * sizeof(uint64_t), ctx->stream));
-        CK(cudaMemsetAsync(ctx->ref_packed.p, 0, (size_t)(words + 2 + 64) * 4, ctx->stream));
-        CK(cudaMemsetAsync(ctx->ref_exc.p, 0, (size_t)(2 * n_blocks + 2) * 4 + 16, ctx->stream));
-        uint32_t* cnt = ctx->ref_exc.as<uint32_t>() + n_blocks + 1;     // counts behind the prefix array
-        unsigned long long* other = (unsigned long long*)(ctx->ref_exc.as<uint32_t>() + ((2 * n_blocks + 2 + 1) & ~1ull));
+        CK(tab.ref_packed.ensure((size_t)(words + 2 + 64) * 4));      // + slack: a 64-word window copy may start at the last word
+        CK(tab.ref_exc.ensure((size_t)(2 * n_blocks + 2) * 4 + 16));
+        CK(upload(tab.ref_pk_off, pk.data(), pk.size() * sizeof(uint64_t), ctx->stream));
+        CK(cudaMemsetAsync(tab.ref_packed.p, 0, (size_t)(words + 2 + 64) * 4, ctx->stream));
+        CK(cudaMemsetAsync(tab.ref_exc.p, 0, (size_t)(2 * n_blocks + 2) * 4 + 16, ctx->stream));
+        uint32_t* cnt = tab.ref_exc.as<uint32_t>() + n_blocks + 1;     // counts behind the prefix array
+        unsigned long long* other = (unsigned long long*)(tab.ref_exc.as<uint32_t>() + ((2 * n_blocks + 2 + 1) & ~1ull));
         pack_reference_kernel<<<(unsigned)((words + 255) / 256), 256, 0, ctx->stream>>>(
-            ctx->ref_bases.as<uint8_t>(), ctx->ref_off.as<uint64_t>(), ctx->ref_pk_off.as<uint64_t>(), ref->n_chrom,
-            ctx->ref_packed.as<uint32_t>(), words, cnt, other);
+            tab.ref_bases.as<uint8_t>(), tab.ref_off.as<uint64_t>(), tab.ref_pk_off.as<uint64_t>(), ref->n_chrom,
+            tab.ref_packed.as<uint32_t>(), words, cnt, other);
         CK(cudaGetLastError());
         size_t tmp = 0;
-        CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, cnt, ctx->ref_exc.as<uint32_t>(), (int)(n_blocks + 1), ctx->stream));
+        CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, cnt, tab.ref_exc.as<uint32_t>(), (int)(n_blocks + 1), ctx->stream));
         CK(ctx->scan_tmp.ensure(tmp));
-        CK(cub::DeviceScan::ExclusiveSum(ctx->scan_tmp.p, tmp, cnt, ctx->ref_exc.as<uint32_t>(), (int)(n_blocks + 1), ctx->stream));
+        CK(cub::DeviceScan::ExclusiveSum(ctx->scan_tmp.p, tmp, cnt, tab.ref_exc.as<uint32_t>(), (int)(n_blocks + 1), ctx->stream));
         unsigned long long h_other = 0;
         CK(cudaMemcpyAsync(&h_other, other, sizeof h_other, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        ctx->dref.packed = ctx->ref_packed.as<uint32_t>();
-        ctx->dref.pk_words = words + 2;
-        ctx->dref.pk_off = ctx->ref_pk_off.as<uint64_t>();
-        ctx->dref.exc_pre = ctx->ref_exc.as<uint32_t>();
-        ctx->dref.all_iupac = h_other == 0 ? 1u : 0u;
+        tab.dref.packed = tab.ref_packed.as<uint32_t>();
+        tab.dref.pk_words = words + 2;
+        tab.dref.pk_off = tab.ref_pk_off.as<uint64_t>();
+        tab.dref.exc_pre = tab.ref_exc.as<uint32_t>();
+        tab.dref.all_iupac = h_other == 0 ? 1u : 0u;
     }
-    ctx->dref.genome_len = ref->n_bases;
-    ctx->dref.n_chrom = ref->n_chrom;
-    ctx->dref.n_species = 0;
-    ctx->dref.chrom_species = nullptr;
-    ctx->dref.chrom_circular = nullptr;
-    ctx->dref.species_chrom_off = nullptr;
-    ctx->dref.expr_alias = nullptr;
-    ctx->dref.expr_chrom = nullptr;
-    ctx->dref.n_expressed = 0;
-    ctx->dref.chrom_has_polya = nullptr;
-    ctx->dref.trx_len_sorted = nullptr;
-    ctx->dref.trx_len_idx = nullptr;
-    ctx->dref.n_trx_sorted = 0;
-    ctx->have_expr = false;
+    tab.dref.genome_len = ref->n_bases;
+    tab.dref.n_chrom = ref->n_chrom;
+    tab.dref.n_species = 0;
+    tab.dref.chrom_species = nullptr;
+    tab.dref.chrom_circular = nullptr;
+    tab.dref.species_chrom_off = nullptr;
+    tab.dref.expr_alias = nullptr;
+    tab.dref.expr_chrom = nullptr;
+    tab.dref.n_expressed = 0;
+    tab.dref.chrom_has_polya = nullptr;
+    ctx->trx.reset();
+    tab.have_expr = false;
     if (ref->n_species > 0) {
         if (!ref->chrom_species || !ref->chrom_circular)
             return fail(ctx, NS_EINVAL, "ns_set_reference: n_species > 0 needs chrom_species and chrom_circular");
@@ -646,26 +770,26 @@ int ns_set_reference(NsContext* ctx, const NsReference* ref) {
         std::vector<uint8_t> circ(ref->n_chrom);
         CK(cudaMemcpy(sp.data(), ref->chrom_species, sp.size() * 4, cudaMemcpyDefault));
         CK(cudaMemcpy(circ.data(), ref->chrom_circular, circ.size(), cudaMemcpyDefault));
-        ctx->h_sp_off.assign(ref->n_species + 1, 0);
+        tab.h_sp_off.assign(ref->n_species + 1, 0);
         for (uint32_t i = 0; i < ref->n_chrom; ++i) {
             if (sp[i] >= ref->n_species || (i > 0 && sp[i] < sp[i - 1]))
                 return fail(ctx, NS_EINVAL, "ns_set_reference: chromosomes must be grouped by species in species order");
-            ctx->h_sp_off[sp[i] + 1] = i + 1;
+            tab.h_sp_off[sp[i] + 1] = i + 1;
         }
         for (uint32_t k = 1; k <= ref->n_species; ++k) {
-            if (ctx->h_sp_off[k] == 0) ctx->h_sp_off[k] = ctx->h_sp_off[k - 1];
-            if (ctx->h_sp_off[k] == ctx->h_sp_off[k - 1]) return fail(ctx, NS_EINVAL, "ns_set_reference: species %u has no chromosome", k - 1);
+            if (tab.h_sp_off[k] == 0) tab.h_sp_off[k] = tab.h_sp_off[k - 1];
+            if (tab.h_sp_off[k] == tab.h_sp_off[k - 1]) return fail(ctx, NS_EINVAL, "ns_set_reference: species %u has no chromosome", k - 1);
         }
-        CK(upload(ctx->ref_species, sp.data(), sp.size() * 4, ctx->stream));
-        CK(upload(ctx->ref_circular, circ.data(), circ.size(), ctx->stream));
-        CK(upload(ctx->ref_sp_off, ctx->h_sp_off.data(), ctx->h_sp_off.size() * 4, ctx->stream));
+        CK(upload(tab.ref_species, sp.data(), sp.size() * 4, ctx->stream));
+        CK(upload(tab.ref_circular, circ.data(), circ.size(), ctx->stream));
+        CK(upload(tab.ref_sp_off, tab.h_sp_off.data(), tab.h_sp_off.size() * 4, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        ctx->dref.n_species = ref->n_species;
-        ctx->dref.chrom_species = ctx->ref_species.as<uint32_t>();
-        ctx->dref.chrom_circular = ctx->ref_circular.as<uint8_t>();
-        ctx->dref.species_chrom_off = ctx->ref_sp_off.as<uint32_t>();
+        tab.dref.n_species = ref->n_species;
+        tab.dref.chrom_species = tab.ref_species.as<uint32_t>();
+        tab.dref.chrom_circular = tab.ref_circular.as<uint8_t>();
+        tab.dref.species_chrom_off = tab.ref_sp_off.as<uint32_t>();
     }
-    ctx->have_ref = true;
+    tab.have_ref = true;
     ctx->have_batch = false;
     ctx->opt_ok[0] = ctx->opt_ok[1] = false;
     return NS_OK;
@@ -673,20 +797,21 @@ int ns_set_reference(NsContext* ctx, const NsReference* ref) {
 
 int ns_set_model(NsContext* ctx, const NsModel* m) {
     if (!ctx || !m) return fail(ctx, NS_EINVAL, "ns_set_model: null argument");
-    if (ctx->borrowed) return fail(ctx, NS_ESTATE, "ns_set_model: a cloned context shares its parent's model");
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "ns_set_model: a cloned context shares its parent's model");
     if (m->n_match_bins == 0 || m->n_match_bins > NS_MAX_BINS || m->n_tables != 4 + m->n_match_bins)
         return fail(ctx, NS_EINVAL, "ns_set_model: need 1..%d match bins and 4+bins alias tables", NS_MAX_BINS);
     if (!m->alias_prob || !m->alias_idx || !m->alias_desc || !m->match_bin_lo || !m->match_bin_hi)
         return fail(ctx, NS_EINVAL, "ns_set_model: null table pointer");
     CK(cudaSetDevice(ctx->device));
-    ctx->hmodel = *m;
-    DevModel& d = ctx->dmodel;
+    Tables& tab = *ctx->tables;
+    tab.hmodel = *m;
+    DevModel& d = tab.dmodel;
     const NsKde* src[5] = {&m->kde_aligned, &m->kde_ht, &m->kde_ht_ratio, &m->kde_unaligned, &m->kde_gap};
     DevKde* dst[5] = {&d.aligned, &d.ht, &d.ratio, &d.unaligned, &d.gap};
     for (int i = 0; i < 5; ++i) {
         if (src[i]->n && !src[i]->data) return fail(ctx, NS_EINVAL, "ns_set_model: KDE %d has n>0 but no data", i);
-        CK(upload(ctx->kde[i], src[i]->data, (size_t)src[i]->n * sizeof(float), ctx->stream));
-        dst[i]->data = ctx->kde[i].as<float>();
+        CK(upload(tab.kde[i], src[i]->data, (size_t)src[i]->n * sizeof(float), ctx->stream));
+        dst[i]->data = tab.kde[i].as<float>();
         dst[i]->n = src[i]->n;
         dst[i]->bw = src[i]->bandwidth;
     }
@@ -701,10 +826,10 @@ int ns_set_model(NsContext* ctx, const NsModel* m) {
         CK(cudaMemcpy(hx.data(), m->kde2d_x, hx.size() * sizeof(float), cudaMemcpyDefault));
         for (uint32_t i = 1; i < m->n_kde2d; ++i)
             if (hx[i] < hx[i - 1]) return fail(ctx, NS_EINVAL, "ns_set_model: kde2d_x must be sorted ascending");
-        CK(upload(ctx->kde2d_x, m->kde2d_x, (size_t)m->n_kde2d * sizeof(float), ctx->stream));
-        CK(upload(ctx->kde2d_y, m->kde2d_y, (size_t)m->n_kde2d * sizeof(float), ctx->stream));
-        d.kde2d_x = ctx->kde2d_x.as<float>();
-        d.kde2d_y = ctx->kde2d_y.as<float>();
+        CK(upload(tab.kde2d_x, m->kde2d_x, (size_t)m->n_kde2d * sizeof(float), ctx->stream));
+        CK(upload(tab.kde2d_y, m->kde2d_y, (size_t)m->n_kde2d * sizeof(float), ctx->stream));
+        d.kde2d_x = tab.kde2d_x.as<float>();
+        d.kde2d_y = tab.kde2d_y.as<float>();
         d.n_kde2d = m->n_kde2d;
         d.kde2d_bw = m->kde2d_bandwidth;
     }
@@ -715,8 +840,8 @@ int ns_set_model(NsContext* ctx, const NsModel* m) {
     CK(cudaMemcpy(desc.data(), m->alias_desc, desc.size() * 4, cudaMemcpyDefault));
     std::vector<uint2> inter(m->alias_len);
     for (uint32_t i = 0; i < m->alias_len; ++i) inter[i] = make_uint2(hp[i], hi[i]);
-    CK(upload(ctx->alias, inter.data(), inter.size() * sizeof(uint2), ctx->stream));
-    d.alias = ctx->alias.as<uint2>();
+    CK(upload(tab.alias, inter.data(), inter.size() * sizeof(uint2), ctx->stream));
+    d.alias = tab.alias.as<uint2>();
     for (uint32_t t = 0; t < m->n_tables; ++t) {
         d.tab_off[t] = desc[2 * t];
         d.tab_n[t] = desc[2 * t + 1];
@@ -736,9 +861,9 @@ int ns_set_model(NsContext* ctx, const NsModel* m) {
     d.seg_p = m->segment_mean > 1.0f ? 1.0 / (double)m->segment_mean : 1.0;
     std::vector<uint32_t> lut;
     build_qlut(m->qual_cdf, lut);
-    CK(upload(ctx->qlut, lut.data(), lut.size() * 4, ctx->stream));
+    CK(upload(tab.qlut, lut.data(), lut.size() * 4, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->have_model = true;
+    tab.have_model = true;
     ctx->have_batch = false;
     ctx->opt_ok[0] = ctx->opt_ok[1] = false;
     return NS_OK;
@@ -746,11 +871,12 @@ int ns_set_model(NsContext* ctx, const NsModel* m) {
 
 int ns_configure(NsContext* ctx, const NsRunConfig* cfg) {
     if (!ctx || !cfg) return fail(ctx, NS_EINVAL, "ns_configure: null argument");
+    const Tables& tab = *ctx->tables;
     if (cfg->mode > 2) return fail(ctx, NS_EINVAL, "ns_configure: mode must be 0 (genome), 1 (metagenome) or 2 (transcriptome)");
     if (cfg->mode == 2 && cfg->chimeric) return fail(ctx, NS_EINVAL, "ns_configure: transcriptome reads are not chimeric");
-    if (cfg->mode == 2 && ctx->have_model && ctx->dmodel.n_kde2d == 0)
+    if (cfg->mode == 2 && tab.have_model && tab.dmodel.n_kde2d == 0)
         return fail(ctx, NS_ESTATE, "ns_configure: transcriptome mode needs _aligned_region_2d.pkl in the model");
-    if (cfg->mode == 1 && ctx->have_ref && ctx->dref.n_species == 0)
+    if (cfg->mode == 1 && tab.have_ref && tab.dref.n_species == 0)
         return fail(ctx, NS_ESTATE, "ns_configure: metagenome mode needs a reference with species information");
     if (cfg->mode == 1 && cfg->kmer_bias != 0) return fail(ctx, NS_EINVAL, "ns_configure: -hp/-k is not offered in metagenome mode");
     if (cfg->max_len < cfg->min_len) return fail(ctx, NS_EINVAL, "Maximum read length must be longer than Minimum read length!");
@@ -759,7 +885,7 @@ int ns_configure(NsContext* ctx, const NsRunConfig* cfg) {
         return fail(ctx, NS_EINVAL, "Please provide both mean and standard deviation of read length!");
     if (cfg->median_len != 0.0 && cfg->chimeric) return fail(ctx, NS_EINVAL, "Lognormal distributed reads cannot be chimeric!");
     if (cfg->median_len < 0.0 || cfg->sd_len < 0.0) return fail(ctx, NS_EINVAL, "ns_configure: negative -med/-sd");
-    if (cfg->kmer_bias != 0 && ctx->have_model && !ctx->hmodel.has_hp)
+    if (cfg->kmer_bias != 0 && tab.have_model && !tab.hmodel.has_hp)
         return fail(ctx, NS_ESTATE, "ns_configure: -hp/-k needs _hp_lengths_model_parameters.tsv in the model");
     if (cfg->kmer_bias == 1) return fail(ctx, NS_EINVAL, "ns_configure: -k must be >= 2 (every base is a run of length 1)");
     ctx->hcfg = *cfg;
@@ -773,34 +899,29 @@ int ns_configure(NsContext* ctx, const NsRunConfig* cfg) {
     ctx->dcfg.uracil = (cfg->flags & NS_FLAG_URACIL) ? 1u : 0u;
     ctx->dcfg.kde2d_n = cfg->kde2d_sample ? cfg->kde2d_sample : 1u;
     ctx->dcfg.trx_records = cfg->trx_records;
-    if (cfg->mode == 2 && ctx->have_ref) {
+    if (cfg->mode == 2 && tab.have_ref) {
         // records sorted by length for the unaligned reads' transcript draw (plan_kernel.cuh:draw_position_trx)
-        const uint32_t nrec = cfg->trx_records ? std::min(cfg->trx_records, ctx->dref.n_chrom) : ctx->dref.n_chrom;
-        if (ctx->dref.n_trx_sorted != nrec || !ctx->dref.trx_len_sorted) {
+        const uint32_t nrec = cfg->trx_records ? std::min(cfg->trx_records, tab.dref.n_chrom) : tab.dref.n_chrom;
+        if (!ctx->trx || ctx->trx->n != nrec) {
             std::vector<uint32_t> idx(nrec), both(2 * (size_t)nrec);
             for (uint32_t i = 0; i < nrec; ++i) idx[i] = i;
-            const std::vector<uint64_t>& off = ctx->h_chrom_off;
+            const std::vector<uint64_t>& off = tab.h_chrom_off;
             std::stable_sort(idx.begin(), idx.end(), [&](uint32_t x, uint32_t y) { return off[x + 1] - off[x] < off[y + 1] - off[y]; });
             for (uint32_t i = 0; i < nrec; ++i) {
                 both[i] = (uint32_t)(off[idx[i] + 1] - off[idx[i]]);
                 both[nrec + i] = idx[i];
             }
             CK(cudaSetDevice(ctx->device));
-            if (!ctx->trx_sorted_owned) {          // a clone must not grow (= free) its parent's buffer
-                ctx->trx_sorted.p = nullptr;
-                ctx->trx_sorted.cap = 0;
-            }
-            CK(upload(ctx->trx_sorted, both.data(), both.size() * 4, ctx->stream));
+            auto trx = std::make_shared<TrxTable>();
+            CK(upload(trx->buf, both.data(), both.size() * 4, ctx->stream));
             CK(cudaStreamSynchronize(ctx->stream));
-            ctx->trx_sorted_owned = true;
-            ctx->dref.trx_len_sorted = ctx->trx_sorted.as<uint32_t>();
-            ctx->dref.trx_len_idx = ctx->trx_sorted.as<uint32_t>() + nrec;
-            ctx->dref.n_trx_sorted = nrec;
+            trx->n = nrec;
+            ctx->trx = std::move(trx);
         }
     }
     ctx->dcfg.polya_scale = cfg->polya_scale;
     ctx->dcfg.min_len = cfg->min_len;
-    ctx->dcfg.max_len = cfg->max_len;
+    ctx->dcfg.max_len = std::min(cfg->max_len, 0x0fffffffu);
     ctx->dcfg.seed = ctx->seed;
     ctx->dcfg.median_len = cfg->median_len;
     ctx->dcfg.sd_len = cfg->sd_len;
@@ -812,8 +933,9 @@ int ns_configure(NsContext* ctx, const NsRunConfig* cfg) {
 
 int ns_set_abundance(NsContext* ctx, const double* abun, const double* abun_inflated, uint32_t n_species) {
     if (!ctx || !abun || n_species == 0) return fail(ctx, NS_EINVAL, "ns_set_abundance: null argument");
-    if (!ctx->have_ref || ctx->dref.n_species != n_species)
-        return fail(ctx, NS_ESTATE, "ns_set_abundance: the reference has %u species, got %u", ctx ? ctx->dref.n_species : 0, n_species);
+    const Tables& tab = *ctx->tables;
+    if (!tab.have_ref || tab.dref.n_species != n_species)
+        return fail(ctx, NS_ESTATE, "ns_set_abundance: the reference has %u species, got %u", tab.dref.n_species, n_species);
     ctx->abun.assign(abun, abun + n_species);
     if (abun_inflated) ctx->abun_inflated.assign(abun_inflated, abun_inflated + n_species);
     else ctx->abun_inflated.assign(n_species, 0.0);
@@ -824,8 +946,9 @@ int ns_set_abundance(NsContext* ctx, const double* abun, const double* abun_infl
 int ns_set_expression(NsContext* ctx, const NsExpression* ex) {
     if (!ctx || !ex || !ex->alias_prob || !ex->alias_idx || !ex->expr_chrom || ex->n_expressed == 0)
         return fail(ctx, NS_EINVAL, "ns_set_expression: null argument or no expressed transcript");
-    if (!ctx->have_ref) return fail(ctx, NS_ESTATE, "ns_set_expression: set the reference transcriptome first");
-    if (ctx->borrowed) return fail(ctx, NS_ESTATE, "ns_set_expression: a cloned context shares its parent's tables");
+    Tables& tab = *ctx->tables;
+    if (!tab.have_ref) return fail(ctx, NS_ESTATE, "ns_set_expression: set the reference transcriptome first");
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "ns_set_expression: a cloned context shares its parent's tables");
     CK(cudaSetDevice(ctx->device));
     const uint32_t n = ex->n_expressed;
     std::vector<uint32_t> hp(n), hi(n), hc(n);
@@ -834,21 +957,21 @@ int ns_set_expression(NsContext* ctx, const NsExpression* ex) {
     CK(cudaMemcpy(hc.data(), ex->expr_chrom, n * 4, cudaMemcpyDefault));
     std::vector<uint2> inter(n);
     for (uint32_t i = 0; i < n; ++i) {
-        if (hi[i] >= n || hc[i] >= ctx->dref.n_chrom) return fail(ctx, NS_EINVAL, "ns_set_expression: index out of range at %u", i);
+        if (hi[i] >= n || hc[i] >= tab.dref.n_chrom) return fail(ctx, NS_EINVAL, "ns_set_expression: index out of range at %u", i);
         inter[i] = make_uint2(hp[i], hi[i]);
     }
-    CK(upload(ctx->expr_alias, inter.data(), inter.size() * sizeof(uint2), ctx->stream));
-    CK(upload(ctx->expr_chrom, hc.data(), hc.size() * 4, ctx->stream));
-    ctx->dref.expr_alias = ctx->expr_alias.as<uint2>();
-    ctx->dref.expr_chrom = ctx->expr_chrom.as<uint32_t>();
-    ctx->dref.n_expressed = n;
-    ctx->dref.chrom_has_polya = nullptr;
+    CK(upload(tab.expr_alias, inter.data(), inter.size() * sizeof(uint2), ctx->stream));
+    CK(upload(tab.expr_chrom, hc.data(), hc.size() * 4, ctx->stream));
+    tab.dref.expr_alias = tab.expr_alias.as<uint2>();
+    tab.dref.expr_chrom = tab.expr_chrom.as<uint32_t>();
+    tab.dref.n_expressed = n;
+    tab.dref.chrom_has_polya = nullptr;
     if (ex->chrom_has_polya) {
-        CK(upload(ctx->chrom_polya, ex->chrom_has_polya, ctx->dref.n_chrom, ctx->stream));
-        ctx->dref.chrom_has_polya = ctx->chrom_polya.as<uint8_t>();
+        CK(upload(tab.chrom_polya, ex->chrom_has_polya, tab.dref.n_chrom, ctx->stream));
+        tab.dref.chrom_has_polya = tab.chrom_polya.as<uint8_t>();
     }
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->have_expr = true;
+    tab.have_expr = true;
     ctx->have_batch = false;
     return NS_OK;
 }
@@ -976,94 +1099,7 @@ __global__ void species_bases_kernel(const NsPieceMeta* pieces, uint32_t n, cons
 }
 }  // namespace
 
-static int exclusive_scan_u64(NsContext* ctx, const uint64_t* in, uint64_t* out, uint32_t n) {
-    size_t tmp = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, in, out, (int)n, ctx->stream));
-    CK(ctx->scan_tmp.ensure(tmp));
-    CK(cub::DeviceScan::ExclusiveSum(ctx->scan_tmp.p, tmp, in, out, (int)n, ctx->stream));
-    return NS_OK;
-}
-
 namespace {
-// Launch geometry: NANOSIM_B200_EMIT_BLOCKS_PER_SM / NANOSIM_B200_PLAN_BLOCKS_PER_SM cap the persistent grids (0 / unset =
-// as many blocks as fit), so that kernels of overlapped contexts can share an SM instead of queueing.
-// emit_kernel over `n_pieces` pieces of the context's current batch (all of them, or the ones `order` lists)
-int launch_emit(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_pieces, const uint32_t* order,
-                const uint32_t* abort_flag = nullptr, bool split = true, cudaEvent_t emit_begin = nullptr) {
-    cudaStream_t st = ctx->stream;
-    EmitArgs ea;
-    ea.ref = ctx->dref;
-    ea.cfg = ctx->dcfg;
-    ea.kind = (uint32_t)kind;
-    ea.first_id = first_read_id;
-    ea.reads = ctx->reads.as<NsReadMeta>();
-    ea.pieces = ctx->pieces.as<NsPieceMeta>();
-    ea.ops = ctx->ops.as<uint32_t>();
-    ea.n_pieces = n_pieces;
-    ea.seq = ctx->seq.as<uint8_t>();
-    ea.qual = ctx->qual.as<uint8_t>();
-    ea.qlut = ctx->qlut.as<uint32_t>();
-    ea.force_exact = (ctx->hcfg.flags & NS_FLAG_EMIT_EXACT) ? 1u : 0u;
-    ea.abort = abort_flag;
-    ea.counter = ctx->counter.as<uint32_t>();
-    ea.order = order;
-    CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
-    {   // long pieces become several work items.  Capacity: every extra item stands for EMIT_SPLIT - 16 or more output bytes
-        // of its piece, and a batch's output fits the sequence buffer (checked on the device for sync-free batches).
-        static const int no_split = env_int("NANOSIM_B200_NO_SPLIT", 0);
-        const uint32_t cap_extra = (uint32_t)std::min<size_t>(ctx->seq.cap / (EMIT_SPLIT - 16u) + 64u, 0x7fffffffu);
-        ea.split_base = nullptr;
-        ea.extra = nullptr;
-        ea.ckpt = nullptr;
-        ea.n_extra = ctx->counter.as<uint32_t>() + 4;
-        ea.cap_extra = cap_extra;
-        if (split && !no_split && n_pieces && !(ctx->hcfg.flags & NS_FLAG_EMIT_WHOLE)) {     // (`order` lists pieces below n_pieces whenever split is asked for)
-            CK(ctx->split_base.ensure((size_t)n_pieces * sizeof(uint32_t)));
-            CK(ctx->split_extra.ensure((size_t)cap_extra * sizeof(uint2)));
-            CK(ctx->split_ckpt.ensure((size_t)cap_extra * sizeof(uint4)));
-            CK(cudaMemsetAsync(ctx->split_extra.p, 0xff, (size_t)cap_extra * sizeof(uint2), st));
-            SplitArgs sa;
-            sa.reads = ea.reads;
-            sa.pieces = ea.pieces;
-            sa.ops = ea.ops;
-            sa.n_pieces = n_pieces;
-            sa.split_base = ctx->split_base.as<uint32_t>();
-            sa.extra = ctx->split_extra.as<uint2>();
-            sa.ckpt = ctx->split_ckpt.as<uint4>();
-            sa.n_extra = ctx->counter.as<uint32_t>() + 4;
-            sa.cap_extra = cap_extra;
-            sa.abort = abort_flag;
-            const unsigned sblocks = std::min<unsigned>((n_pieces + 7u) / 8u, (unsigned)ctx->sm_count * 8u);
-            split_kernel<<<sblocks, 256, 0, st>>>(sa);
-            if (emit_begin) CK(cudaEventRecord(emit_begin, st));     // the emit phase of the batch timings starts after the split
-            ea.split_base = sa.split_base;
-            ea.extra = sa.extra;
-            ea.ckpt = sa.ckpt;
-        }
-    }
-    const size_t ring_bytes = (size_t)EMIT_WARPS * EMIT_RING * sizeof(uint4) + 512 + EMIT_WINDOW_SMEM;
-    if (ctx->hcfg.fastq) {
-        size_t smem = ring_bytes + (size_t)NS_N_QUAL_STATES * QLUT_SIZE * 4;
-        CK(cudaFuncSetAttribute(emit_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 1;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, emit_kernel<true>, EMIT_WARPS * 32, smem));
-        static const int cap_sm = env_int("NANOSIM_B200_EMIT_BLOCKS_PER_SM", 0);
-        if (cap_sm > 0) per_sm = std::min(per_sm, cap_sm);
-        unsigned blocks = std::min<unsigned>((n_pieces + EMIT_WARPS - 1) / EMIT_WARPS, (unsigned)(ctx->sm_count * std::max(per_sm, 1)));
-        emit_kernel<true><<<blocks, EMIT_WARPS * 32, smem, st>>>(ea);
-    } else {
-        size_t smem = ring_bytes;
-        int per_sm = 1;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, emit_kernel<false>, EMIT_WARPS * 32, smem));
-        static const int cap_sm = env_int("NANOSIM_B200_EMIT_BLOCKS_PER_SM", 0);
-        if (cap_sm > 0) per_sm = std::min(per_sm, cap_sm);
-        unsigned blocks = std::min<unsigned>((n_pieces + EMIT_WARPS - 1) / EMIT_WARPS, (unsigned)(ctx->sm_count * std::max(per_sm, 1)));
-        emit_kernel<false><<<blocks, EMIT_WARPS * 32, smem, st>>>(ea);
-    }
-    CK(cudaGetLastError());
-    return NS_OK;
-}
-
 __global__ void hp_piece_keys(const NsPieceMeta* pieces, uint32_t n, uint32_t* keys, uint32_t* vals) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -1087,18 +1123,18 @@ __global__ void iota_from(uint32_t* v, uint32_t n, uint32_t first) {
 
 int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_reads, NsBatchInfo* info) {
     if (!ctx) return NS_EINVAL;
-    if (!ctx->have_ref || !ctx->have_model || !ctx->have_cfg)
+    const Tables& tab = *ctx->tables;
+    if (!tab.have_ref || !tab.have_model || !ctx->have_cfg)
         return fail(ctx, NS_ESTATE, "ns_simulate: reference, model and run configuration must be set first");
     if (kind != NS_KIND_ALIGNED && kind != NS_KIND_UNALIGNED) return fail(ctx, NS_EINVAL, "ns_simulate: bad kind %d", kind);
-    if (kind == NS_KIND_UNALIGNED && ctx->dmodel.unaligned.n == 0 && ctx->hcfg.median_len == 0.0)
+    if (kind == NS_KIND_UNALIGNED && tab.dmodel.unaligned.n == 0 && ctx->hcfg.median_len == 0.0)
         return fail(ctx, NS_ESTATE, "ns_simulate: model has no unaligned-length KDE");
-    if (kind == NS_KIND_ALIGNED && ctx->hcfg.chimeric && ctx->dmodel.gap.n == 0)
+    if (kind == NS_KIND_ALIGNED && ctx->hcfg.chimeric && tab.dmodel.gap.n == 0)
         return fail(ctx, NS_ESTATE, "ns_simulate: chimeric simulation needs the gap-length KDE");
-    if (ctx->dcfg.transcriptome && kind == NS_KIND_ALIGNED && !ctx->have_expr)
+    if (ctx->dcfg.transcriptome && kind == NS_KIND_ALIGNED && !tab.have_expr)
         return fail(ctx, NS_ESTATE, "ns_simulate: transcriptome mode needs ns_set_expression");
-    if (ctx->hcfg.fastq && !ctx->hmodel.has_qual)
+    if (ctx->hcfg.fastq && !tab.hmodel.has_qual)
         return fail(ctx, NS_ESTATE, "ns_simulate: --fastq needs base-quality parameters in the model");
-    if (ctx->hcfg.max_len > 0x0fffffffu) ctx->dcfg.max_len = 0x0fffffffu;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     ctx->have_batch = false;
@@ -1110,8 +1146,16 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         return NS_OK;
     }
     const uint32_t n = n_reads;
-    uint32_t launches = 0;
+    const bool chim = (kind == NS_KIND_ALIGNED) && ctx->hcfg.chimeric;
+    const bool species = ctx->dcfg.metagenome && kind == NS_KIND_ALIGNED;
+    const bool hp = ctx->hcfg.kmer_bias > 0 && kind == NS_KIND_ALIGNED;
     const bool fast_unaligned = kind == NS_KIND_UNALIGNED && !(ctx->hcfg.flags & NS_FLAG_UNALIGNED_SCRIPTS);
+    // One submission, no host round trip (DESIGN §3): a kind of batch without a chimeric piece count, species assignment,
+    // homopolymer pass or scripted unaligned reads in the way, of which a batch at least this large has run sized.
+    const bool may_sync_free = !chim && !species && !hp && (kind == NS_KIND_ALIGNED || fast_unaligned);
+    const bool sync_free = may_sync_free && ctx->opt_ok[kind] && n <= ctx->opt_n[kind] && ctx->ops.cap > 64 && ctx->seq.cap > 64 &&
+                           (!ctx->hcfg.fastq || ctx->qual.cap >= ctx->seq.cap);
+    const DevRef dref = dev_ref(ctx);
     const unsigned tb = 256, gb = (n + tb - 1) / tb;
     CK(ctx->reads.ensure((size_t)n * sizeof(NsReadMeta)));
     CK(ctx->counter.ensure(64));
@@ -1120,18 +1164,15 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     CK(ctx->scan_out.ensure((size_t)n * (2 * NS_MAX_SEGMENTS) * sizeof(uint64_t)));
     CK(cudaMemsetAsync(ctx->totals.p, 0, 16 * sizeof(uint64_t), st));
     CK(cudaEventRecord(ctx->ev[0], st));
-
-    // ---- pieces per read
-    const bool chim = (kind == NS_KIND_ALIGNED) && ctx->hcfg.chimeric;
-    // one submission, no host round trip: same kind of batch as one already sized, no chimeric piece count, species
-    // assignment, homopolymer pass or scripted unaligned reads in the way
-    static const bool no_opt = getenv("NANOSIM_B200_SYNC_BATCHES") != nullptr;
-    const bool optimistic = !no_opt && ctx->opt_ok[kind] && n <= ctx->opt_n[kind] && !chim && !(ctx->dcfg.metagenome && kind == NS_KIND_ALIGNED) &&
-                            !(ctx->hcfg.kmer_bias > 0 && kind == NS_KIND_ALIGNED) && (kind == NS_KIND_ALIGNED || fast_unaligned) &&
-                            ctx->ops.cap > 64 && ctx->seq.cap > 64 && (!ctx->hcfg.fastq || ctx->qual.cap >= ctx->seq.cap);
     const uint64_t ops_cap = ctx->ops.cap / sizeof(uint32_t), seq_cap = ctx->seq.cap;
     uint64_t* d_totals = ctx->totals.as<uint64_t>();
-    const uint32_t* d_abort = optimistic ? (const uint32_t*)(d_totals + NS_T_ABORT) : nullptr;
+    const uint64_t* h_totals = ctx->h_totals.as<uint64_t>();      // as of the last publish_totals_and_wait
+    auto script_ops = [h_totals] { return h_totals[NS_T_PRIMARY] + h_totals[1] + h_totals[6]; };
+    uint64_t* scan_in = ctx->scan_in.as<uint64_t>();
+    uint64_t* scan_out = ctx->scan_out.as<uint64_t>();
+    const uint32_t* d_abort = sync_free ? (const uint32_t*)(d_totals + NS_T_ABORT) : nullptr;
+
+    // ---- pieces per read
     uint32_t n_pieces = n;
     const uint32_t* d_nseg = nullptr;
     const uint32_t* d_pfirst = nullptr;
@@ -1139,23 +1180,21 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         CK(ctx->nseg.ensure((size_t)n * 4));
         CK(ctx->npieces.ensure((size_t)n * 4));
         CK(ctx->piece_first.ensure((size_t)n * 4));
-        segments_kernel<<<gb, tb, 0, st>>>(ctx->dmodel, ctx->dcfg, (uint32_t)kind, first_read_id, n, ctx->nseg.as<uint32_t>(),
-                                           ctx->npieces.as<uint32_t>());
-        widen_u32<<<gb, tb, 0, st>>>(ctx->npieces.as<uint32_t>(), n, ctx->scan_in.as<uint64_t>());
-        int rc = exclusive_scan_u64(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n);
-        if (rc) return rc;
-        narrow_u64<<<gb, tb, 0, st>>>(ctx->scan_out.as<uint64_t>(), n, ctx->piece_first.as<uint32_t>());
-        last_total<<<1, 32, 0, st>>>(ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n, ctx->totals.as<uint64_t>(), 0);
-        launches += 6;
-        publish_totals<<<1, 32, 0, st>>>(ctx->totals.as<uint64_t>(), ctx->h_totals_dev);
-        CK(cudaStreamSynchronize(st));
-        n_pieces = (uint32_t)ctx->h_totals[0];
+        CK(launch(ctx, segments_kernel, gb, tb, 0, tab.dmodel, ctx->dcfg, (uint32_t)kind, first_read_id, n, ctx->nseg.as<uint32_t>(),
+                  ctx->npieces.as<uint32_t>()));
+        CK(launch(ctx, widen_u32, gb, tb, 0, ctx->npieces.as<uint32_t>(), n, scan_in));
+        if (int rc = scan_total(ctx, scan_in, scan_out, n, 0)) return rc;
+        CK(launch(ctx, narrow_u64, gb, tb, 0, scan_out, n, ctx->piece_first.as<uint32_t>()));
+        if (int rc = publish_totals_and_wait(ctx)) return rc;
+        n_pieces = (uint32_t)h_totals[0];
         d_nseg = ctx->nseg.as<uint32_t>();
         d_pfirst = ctx->piece_first.as<uint32_t>();
     }
     CK(ctx->pieces.ensure((size_t)(n_pieces + 1) * sizeof(NsPieceMeta)));
     CK(cudaMemsetAsync(ctx->pieces.p, 0, (size_t)(n_pieces + 1) * sizeof(NsPieceMeta), st));
     const unsigned gp = (n_pieces + tb - 1) / tb;
+    NsReadMeta* reads = ctx->reads.as<NsReadMeta>();
+    NsPieceMeta* pieces = ctx->pieces.as<NsPieceMeta>();
 
     // ---- generation-0 lengths -> op-slot capacities (scan) and processing order (longest reads first)
     CK(ctx->sort_keys.ensure((size_t)n * 8));
@@ -1165,38 +1204,24 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     uint32_t* vals_in = ctx->sort_vals.as<uint32_t>();
     uint32_t* vals_out = vals_in + n;
     const bool exact_only = (kind == NS_KIND_UNALIGNED) && !fast_unaligned;
-    lengths_kernel<<<gb, tb, 0, st>>>(ctx->dmodel, ctx->dcfg, (uint32_t)kind, first_read_id, n, d_nseg, d_pfirst,
-                                      ctx->pieces.as<NsPieceMeta>(), 1.0f / std::max(1.0f, ctx->hmodel.mean_ref_per_event),
-                                      std::min(8.0f, std::max(1.0f, ctx->hmodel.ref_per_event_cv)),
-                                      exact_only ? 1u : 0u, ctx->scan_in.as<uint64_t>(), keys_in, vals_in);
-    CK(cudaGetLastError());
-    {
-        int rc = exclusive_scan_u64(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n_pieces);
-        if (rc) return rc;
-    }
-    scatter_piece_off<<<gp, tb, 0, st>>>(ctx->pieces.as<NsPieceMeta>(), n_pieces, ctx->scan_out.as<uint64_t>());
-    last_total<<<1, 32, 0, st>>>(ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n_pieces, ctx->totals.as<uint64_t>(), 4);
-    set_sentinel_off<<<1, 32, 0, st>>>(ctx->pieces.as<NsPieceMeta>(), n_pieces, ctx->totals.as<uint64_t>() + 4);
-    {
-        size_t tmp = 0;
-        CK(cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, keys_in, keys_out, vals_in, vals_out, (int)n, 0, 32, st));
-        CK(ctx->sort_tmp.ensure(tmp));
-        CK(cub::DeviceRadixSort::SortPairsDescending(ctx->sort_tmp.p, tmp, keys_in, keys_out, vals_in, vals_out, (int)n, 0, 32, st));
-    }
+    CK(launch(ctx, lengths_kernel, gb, tb, 0, tab.dmodel, ctx->dcfg, (uint32_t)kind, first_read_id, n, d_nseg, d_pfirst, pieces,
+              1.0f / std::max(1.0f, tab.hmodel.mean_ref_per_event), std::min(8.0f, std::max(1.0f, tab.hmodel.ref_per_event_cv)),
+              exact_only ? 1u : 0u, scan_in, keys_in, vals_in));
+    if (int rc = scan_total(ctx, scan_in, scan_out, n_pieces, 4)) return rc;
+    CK(launch(ctx, scatter_piece_off, gp, tb, 0, pieces, n_pieces, scan_out));
+    CK(launch(ctx, set_sentinel_off, 1, 32, 0, pieces, n_pieces, d_totals + 4));
+    if (int rc = sort_pairs_descending(ctx, keys_in, keys_out, vals_in, vals_out, n)) return rc;
     // primary script area = the capped slots (+ a bump pool for re-drawn unaligned reads, uread_kernel.cuh)
-    uint64_t primary_ops = 0;
-    capacity_stage_a<<<1, 32, 0, st>>>(d_totals, fast_unaligned ? 1u : 0u, optimistic ? ops_cap : ~0ull);
-    if (!optimistic) {
-        publish_totals<<<1, 32, 0, st>>>(d_totals, ctx->h_totals_dev);
-        CK(cudaStreamSynchronize(st));
-        primary_ops = ctx->h_totals[NS_T_PRIMARY];
-        CK(ctx->ops.ensure((size_t)(primary_ops + 4) * sizeof(uint32_t)));
+    CK(launch(ctx, capacity_stage_a, 1, 32, 0, d_totals, fast_unaligned ? 1u : 0u, sync_free ? ops_cap : ~0ull));
+    if (!sync_free) {
+        if (int rc = publish_totals_and_wait(ctx)) return rc;
+        CK(ctx->ops.ensure((size_t)(h_totals[NS_T_PRIMARY] + 4) * sizeof(uint32_t)));
     }
     uint32_t batch_reversed = 0;
-    if (ctx->dcfg.metagenome && kind == NS_KIND_ALIGNED) {
+    if (species) {
         // ---- assign_species (:758-811): sequential greedy quota fill over this batch's segments, on the host.  Down: the
         //      drawn segment lengths and the reads' order by length (4 B each); up: one species per segment.
-        if (ctx->abun.size() != ctx->dref.n_species) return fail(ctx, NS_ESTATE, "ns_simulate: call ns_set_abundance first");
+        if (ctx->abun.size() != tab.dref.n_species) return fail(ctx, NS_ESTATE, "ns_simulate: call ns_set_abundance first");
         std::vector<uint32_t> hseg(n, 1u), hfirst(n), by_len(n);
         uint32_t n_segs = n;
         if (chim) {
@@ -1214,51 +1239,50 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         uint32_t* d_sfirst = ctx->hp_off.as<uint32_t>();
         uint32_t* d_segval = d_sfirst + n;
         if (chim) CK(cudaMemcpyAsync(d_sfirst, hfirst.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        gather_segment_req<<<gb, tb, 0, st>>>(ctx->pieces.as<NsPieceMeta>(), d_pfirst, d_nseg, n, chim ? d_sfirst : nullptr, d_segval);
+        CK(launch(ctx, gather_segment_req, gb, tb, 0, pieces, d_pfirst, d_nseg, n, chim ? d_sfirst : nullptr, d_segval));
         std::vector<uint32_t> seg_len(n_segs), seg_species(n_segs, 0u);
         CK(cudaMemcpyAsync(seg_len.data(), d_segval, (size_t)n_segs * 4, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(by_len.data(), vals_out, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         HostRng hr{ctx->seed * 0x9E3779B97F4A7C15ull ^ (first_read_id + 0x1234567ull)};
-        batch_reversed = hr.uniform() > (double)ctx->dmodel.strandness ? 1u : 0u;      // once per batch (:860)
+        batch_reversed = hr.uniform() > (double)tab.dmodel.strandness ? 1u : 0u;      // once per batch (:860)
         assign_species_host(hseg, hfirst, seg_len, by_len, seg_species, ctx->abun, ctx->abun_inflated, ctx->species_bases, hr);
         CK(cudaMemcpyAsync(d_segval, seg_species.data(), (size_t)n_segs * 4, cudaMemcpyHostToDevice, st));
-        scatter_segment_species<<<gb, tb, 0, st>>>(ctx->pieces.as<NsPieceMeta>(), d_pfirst, d_nseg, n, chim ? d_sfirst : nullptr, d_segval);
-        CK(cudaGetLastError());
+        CK(launch(ctx, scatter_segment_species, gb, tb, 0, pieces, d_pfirst, d_nseg, n, chim ? d_sfirst : nullptr, d_segval));
         CK(cudaStreamSynchronize(st));                                    // seg_species must outlive the copy
     }
     CK(cudaEventRecord(ctx->ev[1], st));
-    launches += 10;
 
     // ---- plan: rejection loops, positions, edit scripts (single pass)
     PlanArgs pa;
-    pa.m = ctx->dmodel;
-    pa.ref = ctx->dref;
+    pa.m = tab.dmodel;
+    pa.ref = dref;
     pa.cfg = ctx->dcfg;
     pa.kind = (uint32_t)kind;
     pa.first_id = first_read_id;
     pa.n_reads = n;
     pa.n_seg = d_nseg;
     pa.piece_first = d_pfirst;
-    pa.reads = ctx->reads.as<NsReadMeta>();
-    pa.pieces = ctx->pieces.as<NsPieceMeta>();
+    pa.reads = reads;
+    pa.pieces = pieces;
     pa.ops = ctx->ops.as<uint32_t>();
     pa.order = vals_out;
     pa.counter = ctx->counter.as<uint32_t>();
-    pa.n_flagged = (uint32_t*)(ctx->totals.as<uint64_t>() + 5);
+    pa.n_flagged = (uint32_t*)(d_totals + 5);
     pa.batch_reversed = batch_reversed;
     pa.abort = d_abort;
     const unsigned plan_tb = 128;
     // 2 resident blocks per SM rather than 4 (the register limit): the kernel is bound by the latency of its table lookups,
     // and another context's emit kernel still finds room on every SM (transcripts are short -- 1-2 kb reads, no long tail,
-    // two passes: there the register limit of 4 blocks is used).  DESIGN.md §10 has the H100 comparison.
+    // two passes: there the register limit of 4 blocks is used).  NANOSIM_B200_PLAN_BLOCKS_PER_SM overrides the cap.
+    // DESIGN.md §10 has the H100 comparison.
     static const int plan_per_sm_env = env_int("NANOSIM_B200_PLAN_BLOCKS_PER_SM", 0);
     const int plan_per_sm = plan_per_sm_env > 0 ? plan_per_sm_env : (ctx->dcfg.transcriptome ? 4 : 2);
     unsigned plan_blocks = std::min<unsigned>((n + plan_tb - 1) / plan_tb, (unsigned)ctx->sm_count * (unsigned)std::max(1, plan_per_sm));
     // unaligned reads without NS_FLAG_UNALIGNED_SCRIPTS: warp-per-read evaluation (uread_kernel.cuh), same outputs
     UreadArgs ua;
-    ua.m = ctx->dmodel;
-    ua.ref = ctx->dref;
+    ua.m = tab.dmodel;
+    ua.ref = dref;
     ua.cfg = ctx->dcfg;
     ua.first_id = first_read_id;
     ua.n_reads = n;
@@ -1268,16 +1292,15 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     ua.order = vals_out;
     ua.counter = pa.counter;
     ua.n_flagged = pa.n_flagged;
-    ua.pool_cursor = (unsigned long long*)(ctx->totals.as<uint64_t>() + 7);
+    ua.pool_cursor = (unsigned long long*)(d_totals + 7);
     ua.pool = d_totals + NS_T_POOL;             // {base, size} of the bump pool, written by capacity_stage_a
     ua.abort = d_abort;
-    static const int cta_min = env_int("NANOSIM_B200_UREAD_CTA_MIN", (int)UREAD_CTA_MIN_LEN);
-    ua.cta_min_len = (ctx->hcfg.flags & NS_FLAG_EMIT_WHOLE) ? 0u : (uint32_t)std::max(cta_min, 0);
+    ua.cta_min_len = (ctx->hcfg.flags & NS_FLAG_EMIT_WHOLE) ? 0u : (uint32_t)UREAD_CTA_MIN_LEN;
     const unsigned ublocks = std::min<unsigned>((n + UREAD_WARPS - 1) / UREAD_WARPS, (unsigned)ctx->sm_count * 8u);
     if (chim && !ctx->hcfg.perfect) {
         // chimeric gaps of every read's first attempt, a warp per read (uread_kernel.cuh:gap_kernel)
         GapArgs ga;
-        ga.m = ctx->dmodel;
+        ga.m = tab.dmodel;
         ga.cfg = ctx->dcfg;
         ga.kind = (uint32_t)kind;
         ga.first_id = first_read_id;
@@ -1289,190 +1312,131 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         ga.counter = pa.counter;
         ga.abort = d_abort;
         CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
-        gap_kernel<<<ublocks, UREAD_WARPS * 32, 0, st>>>(ga);
-        CK(cudaGetLastError());
-        launches += 1;
+        CK(launch(ctx, gap_kernel, ublocks, UREAD_WARPS * 32, 0, ga));
     }
     CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
-    if (fast_unaligned) uread_kernel<false><<<ublocks, UREAD_WARPS * 32, 0, st>>>(ua);
-    else plan_kernel<false><<<plan_blocks, plan_tb, 0, st>>>(pa);
-    CK(cudaGetLastError());
+    if (fast_unaligned) CK(launch(ctx, uread_kernel<false>, ublocks, UREAD_WARPS * 32, 0, ua));
+    else CK(launch(ctx, plan_kernel<false>, plan_blocks, plan_tb, 0, pa));
     CK(cudaEventRecord(ctx->ev[2], st));
-    launches += 1;
 
-    // ---- 16-byte aligned sequence slots per read (scan); exact offsets for scripts that overflowed their slot
-    gather_read_bytes<<<gb, tb, 0, st>>>(pa.reads, n, ctx->scan_in.as<uint64_t>());
-    {
-        int rc = exclusive_scan_u64(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n);
-        if (rc) return rc;
-    }
-    scatter_read_off<<<gb, tb, 0, st>>>(pa.reads, n, ctx->scan_out.as<uint64_t>());
-    last_total<<<1, 32, 0, st>>>(ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n, ctx->totals.as<uint64_t>(), 2);
-    sum_bases<<<std::min<unsigned>(gb, 1024u), tb, 0, st>>>(pa.reads, n, (unsigned long long*)(ctx->totals.as<uint64_t>() + 3));
-    gather_flagged_ops<<<gp, tb, 0, st>>>(pa.pieces, pa.reads, n_pieces, ctx->scan_in.as<uint64_t>());
-    {
-        int rc = exclusive_scan_u64(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n_pieces);
-        if (rc) return rc;
-    }
-    last_total<<<1, 32, 0, st>>>(ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n_pieces, ctx->totals.as<uint64_t>(), 1);
-    uint64_t overflow_ops = 0, seq_bytes = 0, total_bases = 0, n_ops = 0;
-    uint32_t n_flagged = 0;
-    if (optimistic) {
-        capacity_stage_b<<<1, 32, 0, st>>>(d_totals, ops_cap, seq_cap);
-        n_flagged = 1;                     // unknown without a round trip: the (normally empty) replay is always submitted
+    // ---- sequence slots per read (scan); exact offsets for scripts that overflowed their slot
+    if (int rc = read_layout(ctx, n)) return rc;
+    CK(launch(ctx, gather_flagged_ops, gp, tb, 0, pieces, reads, n_pieces, scan_in));
+    if (int rc = scan_total(ctx, scan_in, scan_out, n_pieces, 1)) return rc;
+    if (sync_free) {
+        CK(launch(ctx, capacity_stage_b, 1, 32, 0, d_totals, ops_cap, seq_cap));
     } else {
-        publish_totals<<<1, 32, 0, st>>>(d_totals, ctx->h_totals_dev);
-        CK(cudaStreamSynchronize(st));
-        overflow_ops = ctx->h_totals[1], seq_bytes = ctx->h_totals[2], total_bases = ctx->h_totals[3];
-        n_flagged = (uint32_t)(ctx->h_totals[5] & 0xffffffffull);
-        n_ops = primary_ops + overflow_ops;
-        CK(ctx->seq.ensure((size_t)seq_bytes + 16));
-        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)seq_bytes + 16));
+        if (int rc = publish_totals_and_wait(ctx)) return rc;
+        CK(ctx->seq.ensure((size_t)h_totals[2] + 16));
+        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)h_totals[2] + 16));
     }
     CK(cudaEventRecord(ctx->ev[3], st));
-    launches += 9;
-    if (n_flagged > 0) {
-        // ---- rare: replay the flagged reads and write their scripts behind the primary area
-        if (!optimistic) CK(ctx->ops.ensure_keep((size_t)(n_ops + 4) * sizeof(uint32_t), (size_t)primary_ops * sizeof(uint32_t), st));
-        pa.ops = ctx->ops.as<uint32_t>();
-        if (optimistic) scatter_flagged_off_dev<<<gp, tb, 0, st>>>(pa.pieces, pa.reads, n_pieces, ctx->scan_out.as<uint64_t>(), d_totals + NS_T_PRIMARY);
-        else scatter_flagged_off<<<gp, tb, 0, st>>>(pa.pieces, pa.reads, n_pieces, ctx->scan_out.as<uint64_t>(), primary_ops);
+    // rare: replay the flagged reads and write their scripts behind the primary area.  A sync-free batch does not know
+    // whether there are any, so it always submits the (normally empty) replay.
+    if (sync_free || (uint32_t)h_totals[5] > 0) {
+        if (!sync_free)
+            CK(ctx->ops.ensure_keep((size_t)(script_ops() + 4) * sizeof(uint32_t), (size_t)h_totals[NS_T_PRIMARY] * sizeof(uint32_t), st));
+        pa.ops = ua.ops = ctx->ops.as<uint32_t>();
+        CK(launch(ctx, scatter_flagged_off, gp, tb, 0, pieces, reads, n_pieces, scan_out, d_totals + NS_T_PRIMARY));
         CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
-        ua.ops = pa.ops;
-        if (fast_unaligned) uread_kernel<true><<<ublocks, UREAD_WARPS * 32, 0, st>>>(ua);
-        else plan_kernel<true><<<plan_blocks, plan_tb, 0, st>>>(pa);
-        CK(cudaGetLastError());
-        launches += 2;
+        if (fast_unaligned) CK(launch(ctx, uread_kernel<true>, ublocks, UREAD_WARPS * 32, 0, ua));
+        else CK(launch(ctx, plan_kernel<true>, plan_blocks, plan_tb, 0, pa));
     }
-    copy_ev_fields<<<gp, tb, 0, st>>>(pa.pieces, n_pieces);
-    uint64_t n_ops_total = n_ops, seq_bytes_final = seq_bytes, total_bases_final = total_bases;
-    if (ctx->hcfg.kmer_bias > 0 && kind == NS_KIND_ALIGNED && !ctx->hcfg.perfect) {
+    CK(launch(ctx, copy_ev_fields, gp, tb, 0, pieces, n_pieces));
+    if (hp && !ctx->hcfg.perfect) {
         // ---- homopolymer pass (hp_kernel.cuh): count, re-scan lengths and script offsets, write
-        if (!ctx->hmodel.has_hp) return fail(ctx, NS_ESTATE, "ns_simulate: -hp/-k needs homopolymer parameters in the model");
+        if (!tab.hmodel.has_hp) return fail(ctx, NS_ESTATE, "ns_simulate: -hp/-k needs homopolymer parameters in the model");
+        const uint64_t event_ops = script_ops();
         HpArgs ha;
-        ha.ref = ctx->dref;
+        ha.ref = dref;
         ha.cfg = ctx->dcfg;
         ha.first_id = first_read_id;
-        ha.reads = pa.reads;
-        ha.pieces = pa.pieces;
+        ha.reads = reads;
+        ha.pieces = pieces;
         ha.n_pieces = n_pieces;
         ha.ops = pa.ops;
-        ha.out_n_ops = ctx->scan_in.as<uint64_t>();
+        ha.out_n_ops = scan_in;
         ha.out_off = nullptr;
-        memcpy(ha.hp, ctx->hmodel.hp, sizeof ha.hp);
-        ha.hp_mis_rate = ctx->hmodel.hp_mis_rate;
+        memcpy(ha.hp, tab.hmodel.hp, sizeof ha.hp);
+        ha.hp_mis_rate = tab.hmodel.hp_mis_rate;
         ha.counter = ctx->counter.as<uint32_t>();
         {   // segments longest first: the lanes of a warp walk segments of similar length, and the longest one starts first
             CK(ctx->hp_keys.ensure((size_t)n_pieces * 16));
             uint32_t* k_in = ctx->hp_keys.as<uint32_t>();
             uint32_t *k_out = k_in + n_pieces, *v_in = k_out + n_pieces, *v_out = v_in + n_pieces;
-            hp_piece_keys<<<gp, tb, 0, st>>>(pa.pieces, n_pieces, k_in, v_in);
-            size_t tmp = 0;
-            CK(cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp, k_in, k_out, v_in, v_out, (int)n_pieces, 0, 32, st));
-            CK(ctx->sort_tmp.ensure(tmp));
-            CK(cub::DeviceRadixSort::SortPairsDescending(ctx->sort_tmp.p, tmp, k_in, k_out, v_in, v_out, (int)n_pieces, 0, 32, st));
+            CK(launch(ctx, hp_piece_keys, gp, tb, 0, pieces, n_pieces, k_in, v_in));
+            if (int rc = sort_pairs_descending(ctx, k_in, k_out, v_in, v_out, n_pieces)) return rc;
             ha.order = v_out;
         }
         ha.force_exact = (ctx->hcfg.flags & NS_FLAG_EMIT_EXACT) ? 1u : 0u;
         const unsigned hp_blocks = std::min<unsigned>((n_pieces + 127) / 128, (unsigned)ctx->sm_count * 16u);
         CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
-        hp_kernel<false><<<hp_blocks, 128, 0, st>>>(ha);
-        CK(cudaGetLastError());
-        hp_fix_reads<<<gb, tb, 0, st>>>(pa.reads, pa.pieces, n);
+        CK(launch(ctx, hp_kernel<false>, hp_blocks, 128, 0, ha));
+        CK(launch(ctx, hp_fix_reads, gb, tb, 0, reads, pieces, n));
         CK(ctx->hp_off.ensure((size_t)n_pieces * sizeof(uint64_t)));
-        {
-            int rc = exclusive_scan_u64(ctx, ctx->scan_in.as<uint64_t>(), ctx->hp_off.as<uint64_t>(), n_pieces);
-            if (rc) return rc;
-        }
-        last_total<<<1, 32, 0, st>>>(ctx->scan_in.as<uint64_t>(), ctx->hp_off.as<uint64_t>(), n_pieces, ctx->totals.as<uint64_t>(), 6);
-        add_base_u64<<<gp, tb, 0, st>>>(ctx->hp_off.as<uint64_t>(), n_pieces, n_ops);
-        CK(cudaMemsetAsync(ctx->totals.as<uint64_t>() + 3, 0, sizeof(uint64_t), st));
-        gather_read_bytes<<<gb, tb, 0, st>>>(pa.reads, n, ctx->scan_in.as<uint64_t>());
-        {
-            int rc = exclusive_scan_u64(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n);
-            if (rc) return rc;
-        }
-        scatter_read_off<<<gb, tb, 0, st>>>(pa.reads, n, ctx->scan_out.as<uint64_t>());
-        last_total<<<1, 32, 0, st>>>(ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n, ctx->totals.as<uint64_t>(), 2);
-        sum_bases<<<std::min<unsigned>(gb, 1024u), tb, 0, st>>>(pa.reads, n, (unsigned long long*)(ctx->totals.as<uint64_t>() + 3));
-        publish_totals<<<1, 32, 0, st>>>(ctx->totals.as<uint64_t>(), ctx->h_totals_dev);
-        CK(cudaStreamSynchronize(st));
-        n_ops_total = n_ops + ctx->h_totals[6];
-        seq_bytes_final = ctx->h_totals[2];
-        total_bases_final = ctx->h_totals[3];
-        CK(ctx->ops.ensure_keep((size_t)(n_ops_total + 4) * sizeof(uint32_t), (size_t)n_ops * sizeof(uint32_t), st));
-        CK(ctx->seq.ensure((size_t)seq_bytes_final + 16));
-        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)seq_bytes_final + 16));
-        pa.ops = ctx->ops.as<uint32_t>();
-        ha.ops = pa.ops;
+        if (int rc = scan_total(ctx, scan_in, ctx->hp_off.as<uint64_t>(), n_pieces, 6)) return rc;
+        CK(launch(ctx, add_base_u64, gp, tb, 0, ctx->hp_off.as<uint64_t>(), n_pieces, event_ops));
+        if (int rc = read_layout(ctx, n)) return rc;
+        if (int rc = publish_totals_and_wait(ctx)) return rc;
+        CK(ctx->ops.ensure_keep((size_t)(script_ops() + 4) * sizeof(uint32_t), (size_t)event_ops * sizeof(uint32_t), st));
+        CK(ctx->seq.ensure((size_t)h_totals[2] + 16));
+        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)h_totals[2] + 16));
+        ha.ops = ctx->ops.as<uint32_t>();
         ha.out_off = ctx->hp_off.as<uint64_t>();
         CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
-        hp_kernel<true><<<hp_blocks, 128, 0, st>>>(ha);
-        CK(cudaGetLastError());
-        launches += 17;
+        CK(launch(ctx, hp_kernel<true>, hp_blocks, 128, 0, ha));
     }
     CK(cudaEventRecord(ctx->ev[4], st));
-    launches += 3;    // ev copy + split + emit
 
-    // ---- emit
-    {
-        int rc = launch_emit(ctx, kind, first_read_id, n_pieces, chim ? nullptr : vals_out, d_abort, true, ctx->ev[4]);   // one piece per read: the plan's
-        if (rc) return rc;                                                                       // longest-first order serves the emit too
-    }
-    CK(cudaGetLastError());
+    // ---- emit (one piece per read: the plan's longest-first order serves the emit too)
+    if (int rc = launch_emit(ctx, kind, first_read_id, n_pieces, chim ? nullptr : vals_out, d_abort, true, ctx->ev[4])) return rc;
     CK(cudaEventRecord(ctx->ev[5], st));
-    if (ctx->dcfg.metagenome && kind == NS_KIND_ALIGNED) {
+    if (species) {
         // current_species_bases[species] += len(new_seg) (:1004) for the next batch's quotas
-        const uint32_t S = ctx->dref.n_species;
+        const uint32_t S = tab.dref.n_species;
         CK(ctx->sp_bases_dev.ensure((size_t)S * sizeof(double)));
         CK(cudaMemsetAsync(ctx->sp_bases_dev.p, 0, (size_t)S * sizeof(double), st));
-        species_bases_kernel<<<gp, tb, 0, st>>>(pa.pieces, n_pieces, ctx->dref.chrom_species, ctx->sp_bases_dev.as<double>());
+        CK(launch(ctx, species_bases_kernel, gp, tb, 0, pieces, n_pieces, tab.dref.chrom_species, ctx->sp_bases_dev.as<double>()));
         std::vector<double> add(S);
         CK(cudaMemcpyAsync(add.data(), ctx->sp_bases_dev.p, (size_t)S * sizeof(double), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         for (uint32_t k = 0; k < S; ++k) ctx->species_bases[k] += add[k];
     }
-    if (optimistic) publish_totals<<<1, 32, 0, st>>>(d_totals, ctx->h_totals_dev);
-    CK(wait_stream(ctx, n >= 16384u));
-    if (optimistic) {
-        if (ctx->h_totals[NS_T_ABORT]) {
+    if (sync_free) {
+        if (int rc = publish_totals_and_wait(ctx, n >= 16384u)) return rc;
+        if (h_totals[NS_T_ABORT]) {
             // a buffer was too small for this batch: nothing was written past a capacity (the kernels saw the flag and
             // returned); run it again the sized way, which also re-establishes the capacities
             ctx->opt_ok[kind] = false;
             return ns_simulate(ctx, kind, first_read_id, n_reads, info);
         }
-        n_ops_total = ctx->h_totals[NS_T_PRIMARY] + ctx->h_totals[1];
-        seq_bytes_final = ctx->h_totals[2];
-        total_bases_final = ctx->h_totals[3];
-    } else if (!chim && !(ctx->dcfg.metagenome && kind == NS_KIND_ALIGNED)) {
-        ctx->opt_ok[kind] = true;
-        ctx->opt_n[kind] = n;
+    } else {
+        CK(wait_stream(ctx, n >= 16384u));
+        if (may_sync_free) {
+            ctx->opt_ok[kind] = true;
+            ctx->opt_n[kind] = n;
+        }
     }
 
     NsBatchInfo& bi = ctx->last;
-    bi.seq_bytes = seq_bytes_final;
-    bi.n_ops = n_ops_total;
-    bi.total_bases = total_bases_final;
+    bi.seq_bytes = h_totals[2];
+    bi.n_ops = script_ops();
+    bi.total_bases = h_totals[3];
     bi.n_reads = n;
     bi.n_pieces = n_pieces;
-    bi.n_launches = launches;
-    float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[1]);
-    bi.ms_setup = ms;
-    cudaEventElapsedTime(&ms, ctx->ev[1], ctx->ev[2]);
-    bi.ms_plan = ms;
-    cudaEventElapsedTime(&ms, ctx->ev[2], ctx->ev[3]);
-    bi.ms_scan = ms;
-    cudaEventElapsedTime(&ms, ctx->ev[3], ctx->ev[4]);
-    bi.ms_script = ms;
-    cudaEventElapsedTime(&ms, ctx->ev[4], ctx->ev[5]);
-    bi.ms_emit = ms;
-    cudaEventElapsedTime(&ms, ctx->ev[0], ctx->ev[5]);
-    bi.ms_total = ms;
-    cudaEventElapsedTime(&ms, g_base[ctx->device], ctx->ev[0]);
-    bi.t_begin_ms = ms;
-    cudaEventElapsedTime(&ms, g_base[ctx->device], ctx->ev[5]);
-    bi.t_end_ms = ms;
+    auto ms = [](cudaEvent_t a, cudaEvent_t b) {
+        float t = 0;
+        cudaEventElapsedTime(&t, a, b);
+        return t;
+    };
+    bi.ms_setup = ms(ctx->ev[0], ctx->ev[1]);
+    bi.ms_plan = ms(ctx->ev[1], ctx->ev[2]);
+    bi.ms_scan = ms(ctx->ev[2], ctx->ev[3]);
+    bi.ms_script = ms(ctx->ev[3], ctx->ev[4]);
+    bi.ms_emit = ms(ctx->ev[4], ctx->ev[5]);
+    bi.ms_total = ms(ctx->ev[0], ctx->ev[5]);
+    bi.t_begin_ms = ms(g_base[ctx->device], ctx->ev[0]);
+    bi.t_end_ms = ms(g_base[ctx->device], ctx->ev[5]);
     ctx->last_kind = kind;
     ctx->last_first_id = first_read_id;
     ctx->have_batch = true;
@@ -1624,24 +1588,17 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
     if (bi.n_reads == 0) return NS_OK;
     if (qual && !ctx->hcfg.fastq) return fail(ctx, NS_ESTATE, "ns_fetch: qualities requested but the run is not --fastq");
     // 2 bits per base only when reads cannot hold anything but A C G T/U: every reference byte is an IUPAC nucleotide code
-    const int nt = ctx->dref.all_iupac ? unpack_threads() : 0;
+    const int nt = ctx->tables->dref.all_iupac ? unpack_threads() : 0;
     const bool packed = seq && nt > 0 && bi.seq_bytes >= (1u << 20);
     if (packed) {
         // bases: pack on the device, copy a quarter of the bytes, expand on the host while the other copies run
         const uint64_t n16 = (bi.seq_bytes + 15) / 16;            // the seq buffer has 16 bytes of slack
         CK(ctx->pack_dev.ensure((size_t)n16 * 4));
-        if ((size_t)n16 * 4 > ctx->pack_host_cap) {
-            if (ctx->pack_host) cudaFreeHost(ctx->pack_host);
-            ctx->pack_host = nullptr;
-            ctx->pack_host_cap = 0;
-            const size_t want = (size_t)n16 * 4 + (size_t)n16 / 2 + 4096;
-            CK(cudaHostAlloc((void**)&ctx->pack_host, want, cudaHostAllocDefault));
-            ctx->pack_host_cap = want;
-        }
-        if (!ctx->ev_pack) CK(cudaEventCreateWithFlags(&ctx->ev_pack, cudaEventDisableTiming | (blocking_sync_wanted() ? (unsigned)cudaEventBlockingSync : 0u)));
+        CK(ctx->pack_host.ensure((size_t)n16 * 4, cudaHostAllocDefault));
+        if (!ctx->ev_pack) CK(cudaEventCreateWithFlags(&ctx->ev_pack.e, cudaEventDisableTiming | (blocking_sync_wanted() ? (unsigned)cudaEventBlockingSync : 0u)));
         pack_bases_kernel<<<(unsigned)((n16 + 255) / 256), 256, 0, st>>>(ctx->seq.as<uint4>(), ctx->pack_dev.as<uint32_t>(), n16);
         CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(ctx->pack_host, ctx->pack_dev.p, (size_t)n16 * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(ctx->pack_host.p, ctx->pack_dev.p, (size_t)n16 * 4, cudaMemcpyDeviceToHost, st));
         CK(cudaEventRecord(ctx->ev_pack, st));
     } else if (seq) {
         CK(cudaMemcpyAsync(seq, ctx->seq.p, bi.seq_bytes, cudaMemcpyDeviceToHost, st));
@@ -1657,7 +1614,7 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
     if (packed) {
         CK(cudaEventSynchronize(ctx->ev_pack));
         t_packed = ms_since();
-        unpack_bases(ctx->pack_host, seq, bi.seq_bytes, ctx->dcfg.uracil != 0, nt);
+        unpack_bases(ctx->pack_host.as<uint8_t>(), seq, bi.seq_bytes, ctx->dcfg.uracil != 0, nt);
         t_unpacked = ms_since();
     }
     CK(wait_stream(ctx, bi.seq_bytes >= (64u << 20)));
@@ -1669,7 +1626,7 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
 
 int ns_transfer_info(NsContext* ctx, uint32_t* packed_bases, uint32_t* n_threads) {
     if (!ctx) return NS_EINVAL;
-    const int nt = (!ctx->have_ref || ctx->dref.all_iupac) ? unpack_threads() : 0;
+    const int nt = (!ctx->tables->have_ref || ctx->tables->dref.all_iupac) ? unpack_threads() : 0;
     if (packed_bases) *packed_bases = nt > 0 ? 1u : 0u;
     if (n_threads) *n_threads = (uint32_t)nt;
     return NS_OK;
@@ -1694,8 +1651,9 @@ int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_
     }
     for (uint32_t k = 0; k < n_new_pieces; ++k) {
         const NsPieceMeta& p = new_pieces[k];
-        if (p.read_slot >= bi.n_reads || p.chrom >= ctx->dref.n_chrom || p.op_off < old_ops || p.op_off + p.n_ops > old_ops + n_new_ops ||
-            (uint64_t)p.pos + p.ref_len > ctx->h_chrom_off[p.chrom + 1] - ctx->h_chrom_off[p.chrom])
+        const Tables& tab = *ctx->tables;
+        if (p.read_slot >= bi.n_reads || p.chrom >= tab.dref.n_chrom || p.op_off < old_ops || p.op_off + p.n_ops > old_ops + n_new_ops ||
+            (uint64_t)p.pos + p.ref_len > tab.h_chrom_off[p.chrom + 1] - tab.h_chrom_off[p.chrom])
             return fail(ctx, NS_EINVAL, "ns_reemit: piece %u is inconsistent with the batch or the reference", k);
     }
     CK(ctx->pieces.ensure_keep((size_t)(old_np + n_new_pieces + 1) * sizeof(NsPieceMeta), (size_t)old_np * sizeof(NsPieceMeta), st));
@@ -1708,18 +1666,14 @@ int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_
     CK(ctx->sort_vals.ensure((size_t)n_new_pieces * sizeof(uint32_t)));
     CK(cudaMemcpyAsync(ctx->scan_in.p, new_reads, (size_t)n_slots * sizeof(NsReadMeta), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->scan_out.p, read_slots, (size_t)n_slots * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    replace_reads<<<(n_slots + 255) / 256, 256, 0, st>>>(ctx->reads.as<NsReadMeta>(), ctx->scan_out.as<uint32_t>(),
-                                                         ctx->scan_in.as<NsReadMeta>(), n_slots, bi.n_reads);
-    iota_from<<<(n_new_pieces + 255) / 256, 256, 0, st>>>(ctx->sort_vals.as<uint32_t>(), n_new_pieces, old_np);
-    CK(cudaGetLastError());
-    {
-        int rc = launch_emit(ctx, NS_KIND_ALIGNED, ctx->last_first_id, n_new_pieces, ctx->sort_vals.as<uint32_t>(), nullptr, false);
-        if (rc) return rc;
-    }
+    CK(launch(ctx, replace_reads, (n_slots + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), ctx->scan_out.as<uint32_t>(),
+              ctx->scan_in.as<NsReadMeta>(), n_slots, bi.n_reads));
+    CK(launch(ctx, iota_from, (n_new_pieces + 255) / 256, 256, 0, ctx->sort_vals.as<uint32_t>(), n_new_pieces, old_np));
+    if (int rc = launch_emit(ctx, NS_KIND_ALIGNED, ctx->last_first_id, n_new_pieces, ctx->sort_vals.as<uint32_t>(), nullptr, false))
+        return rc;
     CK(cudaStreamSynchronize(st));
     bi.n_pieces = old_np + n_new_pieces;
     bi.n_ops = old_ops + n_new_ops;
-    bi.n_launches += 3;
     return NS_OK;
 }
 
@@ -1745,7 +1699,7 @@ int ns_op_stats(NsContext* ctx, uint64_t* out) {
     const uint32_t n = ctx->last.n_pieces;
     if (n) {
         op_stats_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->pieces.as<NsPieceMeta>(), ctx->reads.as<NsReadMeta>(),
-                                                                   ctx->ops.as<uint32_t>(), n, ctx->dref, ctx->seq.as<uint8_t>(),
+                                                                   ctx->ops.as<uint32_t>(), n, dev_ref(ctx), ctx->seq.as<uint8_t>(),
                                                                    (unsigned long long*)ctx->stats.p);
         const uint32_t nr = ctx->last.n_reads;
         if (nr && ctx->seq.p)
@@ -2426,10 +2380,11 @@ NcclApi& nccl_api() {
 
 int ns_get_reference(NsContext* ctx, uint8_t* bases, uint64_t cap) {
     if (!ctx || !bases) return NS_EINVAL;
-    if (!ctx->have_ref) return fail(ctx, NS_ESTATE, "ns_get_reference: no reference set");
-    if (cap < ctx->dref.genome_len) return fail(ctx, NS_ENOMEM, "ns_get_reference: buffer too small");
+    const Tables& tab = *ctx->tables;
+    if (!tab.have_ref) return fail(ctx, NS_ESTATE, "ns_get_reference: no reference set");
+    if (cap < tab.dref.genome_len) return fail(ctx, NS_ENOMEM, "ns_get_reference: buffer too small");
     CK(cudaSetDevice(ctx->device));
-    CK(cudaMemcpy(bases, ctx->dref.bases, ctx->dref.genome_len, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(bases, tab.dref.bases, tab.dref.genome_len, cudaMemcpyDeviceToHost));
     return NS_OK;
 }
 
@@ -2452,8 +2407,9 @@ int ns_nccl_unique_id(uint8_t* id) {
 int ns_bcast_nccl(NsContext* ctx, const uint8_t* id, int rank, int world, int root) {
     if (!ctx || !id || world < 1 || rank < 0 || rank >= world || root < 0 || root >= world) return fail(ctx, NS_EINVAL, "ns_bcast_nccl: bad argument");
 #if NS_HAVE_NCCL
-    if (ctx->borrowed) return fail(ctx, NS_ESTATE, "ns_bcast_nccl: a cloned context shares its parent's reference");
-    if (rank == root && !ctx->have_ref) return fail(ctx, NS_ESTATE, "ns_bcast_nccl: the root rank sets its reference first (ns_set_reference)");
+    const Tables& tab = *ctx->tables;
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "ns_bcast_nccl: a cloned context shares its parent's reference");
+    if (rank == root && !tab.have_ref) return fail(ctx, NS_ESTATE, "ns_bcast_nccl: the root rank sets its reference first (ns_set_reference)");
     if (world == 1) return NS_OK;
     NcclApi& api = nccl_api();
     if (!api.ok) return fail(ctx, NS_ESTATE, "ns_bcast_nccl: libnccl.so.2 could not be loaded (NANOSIM_B200_NCCL_LIB overrides the path)");
@@ -2469,7 +2425,7 @@ int ns_bcast_nccl(NsContext* ctx, const uint8_t* id, int rank, int world, int ro
     uint64_t* d_head = nullptr;
     void *t_bases = nullptr, *t_off = nullptr, *t_sp = nullptr, *t_circ = nullptr;
     do {
-        uint64_t head[4] = {ctx->dref.genome_len, ctx->dref.n_chrom, ctx->dref.n_species, 0};
+        uint64_t head[4] = {tab.dref.genome_len, tab.dref.n_chrom, tab.dref.n_species, 0};
         if (cudaMalloc((void**)&d_head, sizeof head) != cudaSuccess) { rc = NS_ENOMEM; break; }
         cudaMemcpyAsync(d_head, head, sizeof head, cudaMemcpyHostToDevice, st);
         if (bc(d_head, sizeof head) != ncclSuccess) { rc = NS_ECUDA; break; }
@@ -2478,7 +2434,7 @@ int ns_bcast_nccl(NsContext* ctx, const uint8_t* id, int rank, int world, int ro
         const uint64_t n_bases = head[0];
         const uint32_t n_chrom = (uint32_t)head[1], n_species = (uint32_t)head[2];
         if (rank == root) {
-            t_bases = ctx->ref_bases.p; t_off = ctx->ref_off.p; t_sp = ctx->ref_species.p; t_circ = ctx->ref_circular.p;
+            t_bases = tab.ref_bases.p; t_off = tab.ref_off.p; t_sp = tab.ref_species.p; t_circ = tab.ref_circular.p;
         } else {
             if (cudaMalloc(&t_bases, n_bases ? n_bases : 16) != cudaSuccess || cudaMalloc(&t_off, (n_chrom + 1) * sizeof(uint64_t)) != cudaSuccess ||
                 (n_species && (cudaMalloc(&t_sp, n_chrom * 4) != cudaSuccess || cudaMalloc(&t_circ, n_chrom) != cudaSuccess))) { rc = NS_ENOMEM; break; }
