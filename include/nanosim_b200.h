@@ -213,6 +213,10 @@ typedef struct {
     /* begin / end of the batch on the device timeline, in ms since the first ns_create() of this process on this device;
      * comparable across contexts (streams) of one device, so overlapped pipelines can be timed on the device */
     double t_begin_ms, t_end_ms;
+    /* -hp/-k with intron retention (kmer_bias != 0, trx_records != 0): the op buffer also holds a verbatim copy of the event
+     * scripts as the plan wrote them, before the homopolymer pass filtered them; a segment's unfiltered script starts at
+     * raw_ev_off + ev_off (ev_n_ops ops).  0 = no copy.  ns_reemit leaves it as it is. */
+    uint64_t raw_ev_off;
 } NsBatchInfo;
 
 /* --- lifetime --------------------------------------------------------------------------------------------- */
@@ -281,12 +285,22 @@ int ns_unpack_bases(const uint8_t* packed, uint8_t* seq, uint64_t n_bases, int u
  * emits those reads again.  The host decides which reads retain introns (nanosim_b200/intron_retention.py) and lays each of
  * them out as pieces on the GENOME records of the reference, one per exon / retained-intron interval (NS_PIECE_REF_REV,
  * NS_PIECE_CONT, NS_PIECE_RETAINED), with the read's edit script cut at the interval boundaries.  new_reads[k] replaces
- * read read_slots[k] (same seq_len: the bytes are overwritten in place); new_pieces / new_ops are appended behind the
- * batch's pieces / ops, and piece_first / op_off / ev_off in the new metadata are absolute indices into the grown arrays.
- * All emit randomness is indexed by the position in the read, so inserted, head/tail and polyA bases and every quality
- * value come out as before; only bases taken from the reference change. */
+ * read read_slots[k]; new_pieces / new_ops are appended behind the batch's pieces / ops, and piece_first / op_off / ev_off
+ * in the new metadata are absolute indices into the grown arrays.
+ * Without -hp/-k: same seq_len, the bytes are overwritten in place.  All emit randomness is indexed by the position in the
+ * read, so inserted, head/tail and polyA bases and every quality value come out as before; only bases taken from the
+ * reference change.
+ * With -hp/-k: new_ops are the UNFILTERED event scripts (NsBatchInfo.raw_ev_off) cut at the interval boundaries, and each
+ * read's pieces must form one chain -- genome segments at even offsets, each after the first NS_PIECE_CONT, zero-op gaps
+ * in between, one strand, op_off == ev_off.  The -k filter and mutate_homo run again over each chain as one sequence (the
+ * genomic read); the filtered scripts stay the pieces' event scripts, the rewritten ones are appended behind them.  The
+ * read length changes: each replaced read gets a new 16-byte-aligned slot behind the batch's bytes (the old slot is no
+ * longer referenced), and the batch's totals grow (ns_batch_info).  As positions shift and emit randomness is keyed by
+ * position, such reads keep neither their qualities nor their inserted bases. */
 int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_reads, uint32_t n_slots,
               const NsPieceMeta* new_pieces, uint32_t n_new_pieces, const uint32_t* new_ops, uint64_t n_new_ops);
+/* The totals of the last batch as they stand now (ns_simulate's NsBatchInfo, updated by ns_reemit): what ns_fetch copies. */
+int ns_batch_info(NsContext* ctx, NsBatchInfo* info);
 
 /* Device pointers of the last batch (for consumers that stay on the GPU, e.g. torch tensors / NCCL gathers). */
 int ns_device_buffers(NsContext* ctx, const uint8_t** seq, const uint8_t** qual, const NsReadMeta** reads,

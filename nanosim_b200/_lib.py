@@ -23,7 +23,7 @@ NS_STATS_COMP_OFF = NS_STATS_INS_OFF + 4
 NS_STATS_WORDS = NS_STATS_COMP_OFF + 4
 
 EXPORTS = ["ns_create", "ns_destroy", "ns_last_error", "ns_clone", "ns_set_abundance", "ns_set_expression", "ns_set_reference", "ns_set_model", "ns_configure",
-           "ns_simulate", "ns_fetch", "ns_reemit", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases"]
+           "ns_simulate", "ns_fetch", "ns_reemit", "ns_batch_info", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases"]
 
 
 class NsReference(C.Structure):
@@ -87,7 +87,8 @@ class NsBatchInfo(C.Structure):
     _fields_ = [("seq_bytes", C.c_uint64), ("n_ops", C.c_uint64), ("total_bases", C.c_uint64),
                 ("n_reads", C.c_uint32), ("n_pieces", C.c_uint32), ("n_launches", C.c_uint32),
                 ("ms_setup", C.c_float), ("ms_plan", C.c_float), ("ms_scan", C.c_float), ("ms_script", C.c_float),
-                ("ms_emit", C.c_float), ("ms_total", C.c_float), ("t_begin_ms", C.c_double), ("t_end_ms", C.c_double)]
+                ("ms_emit", C.c_float), ("ms_total", C.c_float), ("t_begin_ms", C.c_double), ("t_end_ms", C.c_double),
+                ("raw_ev_off", C.c_uint64)]
 
 
 # numpy views of the two record types
@@ -167,5 +168,7 @@ def lib():
     L.ns_unpack_bases.restype = C.c_int
     L.ns_reemit.argtypes = [P, P, P, C.c_uint32, P, C.c_uint32, P, C.c_uint64]
     L.ns_reemit.restype = C.c_int
+    L.ns_batch_info.argtypes = [P, C.POINTER(NsBatchInfo)]
+    L.ns_batch_info.restype = C.c_int
     _lib = L
     return L

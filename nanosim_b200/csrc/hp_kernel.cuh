@@ -25,6 +25,23 @@
 //   * the error filter reads the 32 reference bases around a position as one 64-bit word and counts the equal neighbours
 //     of the centre base with two count-leading/trailing-zeros.
 // NS_FLAG_EMIT_EXACT switches both shortcuts off (tests: identical scripts either way).
+//
+// CHAIN = true (ns_reemit on a -hp context, intron retention): a read laid out on the genome is a chain of pieces -- a
+// segment and the NS_PIECE_CONT pieces that continue it, two apart (zero-op gap pieces in between) -- that the reference
+// mutates as ONE sequence (simulator.py:1156-1183).  A lane walks the whole chain as one segment:
+//   * chain offset x lies in piece j at offset x'; on a forward piece the base is converted_ref_base(byte[pos + x'], piece j,
+//     x'), on an NS_PIECE_REF_REV piece the complement of converted_ref_base(byte[pos + ref_len-1-x'], piece j,
+//     ref_len-1-x') -- the keys the emit kernel resolves IUPAC bytes with;
+//   * the pending run and the filter window (in_hp) cross piece boundaries; runs of a chain draw ST_HP with the chain's
+//     FIRST piece and a run counter over the whole chain, substituted / inserted bases ST_EMIT_B with (piece, op index in
+//     that piece's event script) as everywhere else (the error-profile formatters recompute them that way);
+//   * output stays per piece: ops that consume reference stay with the piece whose reference they consume.  A boundary
+//     crossed while a run is pending becomes a marker (kind 4) in the run's part list; when the run is closed, a marker
+//     closes the current piece's script and opens the next one's.  A rewritten run puts its literals into the piece where
+//     it starts and splits its reference skip at the markers (LIT consumes no reference, DEL no output: every piece
+//     stays consistent with its ref_len and out_len).
+// Chains always take the byte-exact route.  The chain code is compiled into the CHAIN instantiations only: the ones
+// ns_simulate launches keep their registers (DESIGN.md §3: this kernel is bound by its instruction cache).
 #pragma once
 #include "device_common.cuh"
 
@@ -41,8 +58,9 @@ struct HpArgs {
     double hp[2][6];            // rows AT, CG: const, alpha1, beta1, breakpoint1, intercept, slope
     double hp_mis_rate;
     uint32_t* counter;
-    const uint32_t* order;      // pieces, longest reference span first (nullptr: identity)
+    const uint32_t* order;      // pieces, longest reference span first (nullptr: identity); CHAIN: the chains' first pieces
     uint32_t force_exact;       // NS_FLAG_EMIT_EXACT: no packed-word shortcuts
+    uint32_t piece_base;        // CHAIN: out_n_ops / out_off are indexed by piece - piece_base
 };
 
 #define HP_MAX_SEG 12
@@ -78,11 +96,41 @@ struct ScriptOut {
     }
 };
 
+template <bool CHAIN>
 struct HpWalker {
     const uint8_t* cb;
     uint64_t clen, seed, rid;
     uint32_t pos, piece_in_read, ref_len, K;
-    __device__ __forceinline__ uint32_t base_at(uint32_t x) const {     // case-converted reference base index at offset x
+    // ---- CHAIN: the pieces chain[2j]; the cursor stands on piece c_j, which holds chain offsets [c_lo, c_lo + c_len)
+    const NsPieceMeta* chain;
+    const uint8_t* bases;
+    const uint64_t* chrom_off;
+    const uint8_t* c_cb;
+    uint32_t head_pir, c_j, c_lo, c_len, c_pos, c_rev;
+    __device__ __forceinline__ void load_piece() {
+        const NsPieceMeta& p = chain[2u * c_j];
+        c_len = p.ref_len;
+        c_pos = p.pos;
+        c_rev = (p.kind & NS_PIECE_REF_REV) != 0;
+        c_cb = bases + chrom_off[p.chrom];
+    }
+    __device__ __forceinline__ uint32_t chain_base_at(uint32_t x) {
+        while (x < c_lo) {
+            --c_j;
+            load_piece();
+            c_lo -= c_len;
+        }
+        while (x >= c_lo + c_len) {
+            c_lo += c_len;
+            ++c_j;
+            load_piece();
+        }
+        const uint32_t f = c_rev ? c_lo + c_len - 1u - x : x - c_lo;      // forward offset in the piece (emit_kernel's key)
+        const uint32_t c = converted_ref_base(__ldg(&c_cb[c_pos + f]), seed, rid, head_pir + 2u * c_j, f);
+        return acgt_fast(c) ? (base_idx(c) ^ (c_rev ? 2u : 0u)) : (4u + (c & 3u));
+    }
+    __device__ __forceinline__ uint32_t base_at(uint32_t x) {           // case-converted reference base index at offset x
+        if (CHAIN) return chain_base_at(x);
         uint64_t ab = (uint64_t)pos + x;
         if (ab >= clen) ab -= clen;
         uint32_t c = converted_ref_base(__ldg(&cb[ab]), seed, rid, piece_in_read, x);
@@ -122,7 +170,7 @@ struct HpWalker {
         return 14u - (top >> 1);
     }
     // is offset x inside a run of >= K equal bases of the unmutated segment?
-    __device__ __forceinline__ bool in_hp(int64_t x) const {
+    __device__ __forceinline__ bool in_hp(int64_t x) {
         if (packed) return in_hp_packed(x);
         if (x < 0 || x >= (int64_t)ref_len) return false;
         const uint32_t b = base_at((uint32_t)x);
@@ -137,7 +185,7 @@ struct HpWalker {
 #ifndef HP_MIN_BLOCKS
 #define HP_MIN_BLOCKS 4
 #endif
-template <bool WRITE>
+template <bool WRITE, bool CHAIN = false>
 __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_constant__ HpArgs a) {
     const uint2 key = make_uint2((uint32_t)a.cfg.seed, (uint32_t)(a.cfg.seed >> 32));
     const uint32_t K = a.cfg.kmer_bias;
@@ -150,13 +198,14 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
     // per-lane loops left 2-5 of 32 lanes active and a kernel that mostly waited for its instruction cache.
     enum : int { ST_FETCH = 0, ST_OP = 1, ST_WORD = 2, ST_BASE = 3 };
     enum : int { SRC_WORD = 0, SRC_EXACT = 1, SRC_MIS = 2, SRC_INS = 3 };
-    enum : int { P_NONE = 0, P_END, P_HT, P_LIT, P_COPY, P_DEL, P_BASES, P_SLOW, P_ALL, P_MID };
+    enum : int { P_NONE = 0, P_END, P_HT, P_LIT, P_COPY, P_DEL, P_BASES, P_SLOW, P_ALL, P_MID, P_NEXT };
     int st = ST_FETCH, bsrc = SRC_WORD;
     uint32_t this_piece = 0;
     NsReadMeta rm;
     NsPieceMeta* pmp = nullptr;
     uint64_t rid = 0;
-    HpWalker w = {};
+    HpWalker<CHAIN> w = {};
+    uint32_t out_piece = 0, chain_left = 0;                 // CHAIN: piece whose script is being written; pieces still to walk
     uint32_t* ev = nullptr;
     uint32_t n_ev = 0, k = 0, kk = 0, rpos = 0;
     uint32_t len = 0, t = 0, w16 = 0, cur = 0, n = 0;      // the stretch being walked: t of len done; cur / n = rest of its current word
@@ -166,12 +215,30 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
     // ---- current run of equal bases in the mutated stream
     uint32_t run_base = 0xffu, run_len = 0, run_ref = 0, nseg = 0, n_runs = 0;
     uint32_t seg_kind[HP_MAX_SEG], seg_cnt[HP_MAX_SEG];     // in order: 0 copy, 1 mis, 2 ins, 3 deleted reference bases
+                                                            // (CHAIN: 4 = piece boundary)
+    // CHAIN: the script of piece out_piece is complete; the next piece's begins
+    auto close_out = [&]() {
+        out.flush();
+        NsPieceMeta& pm = a.pieces[out_piece];
+        if (!WRITE) {
+            a.out_n_ops[out_piece - a.piece_base] = out.n;
+            pm.out_len = out.out_len;
+        } else {
+            pm.op_off = a.out_off[out_piece - a.piece_base];
+            pm.n_ops = out.n;
+        }
+    };
+    auto next_out = [&]() {
+        close_out();
+        out_piece += 2;
+        out.begin(WRITE ? a.ops + a.out_off[out_piece - a.piece_base] : nullptr);
+    };
 
     auto flush_run = [&]() {
         if (run_len == 0) return;
         if (run_len >= K && run_base < 4u) {
             // new length ~ N(mu(L), sigma(L)), clipped at 0, Python round()
-            const uint4 r = philox4x32_10(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_HP, 0, w.piece_in_read), n_runs), key);
+            const uint4 r = philox4x32_10(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_HP, 0, CHAIN ? w.head_pir : w.piece_in_read), n_runs), key);
             const uint32_t cls = (run_base == 0u || run_base == 2u) ? 0u : 1u;      // A,T -> "AT" ; C,G -> "CG"
             const double* p = a.hp[cls];
             const double L = (double)run_len;
@@ -185,12 +252,12 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
             uint32_t skip = run_len > nn ? run_len - nn : 0u;
             bool mis_q_used = false;
             Rng mr;
-            if (a.hp_mis_rate > 0.0) mr.init(a.cfg.seed, rid, stream_word(ST_HP, 1, w.piece_in_read) ^ (n_runs << 4));
+            if (a.hp_mis_rate > 0.0) mr.init(a.cfg.seed, rid, stream_word(ST_HP, 1, CHAIN ? w.head_pir : w.piece_in_read) ^ (n_runs << 4));
             uint32_t produced = 0;
             for (uint32_t s = 0; s <= nseg && produced < nn; ++s) {
                 uint32_t cnt, state;
                 if (s < nseg) {
-                    if (seg_kind[s] == 3) continue;       // deleted reference bases carry no quality
+                    if (seg_kind[s] == 3 || (CHAIN && seg_kind[s] == 4)) continue;     // deleted reference bases carry no quality
                     cnt = seg_cnt[s];
                     state = seg_kind[s] == 0 ? 2u : (seg_kind[s] == 1 ? 0u : 1u);
                     if (skip >= cnt) {
@@ -222,7 +289,21 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
                 }
                 produced += cnt;
             }
-            out.add(NS_OP_DEL << 28, run_ref);            // the reference bases the run stood on
+            if (!CHAIN) {
+                out.add(NS_OP_DEL << 28, run_ref);        // the reference bases the run stood on
+            } else {
+                uint32_t skip_ref = 0;                    // ... each piece's share of them
+                for (uint32_t s = 0; s < nseg; ++s) {
+                    if (seg_kind[s] == 4) {
+                        out.add(NS_OP_DEL << 28, skip_ref);
+                        next_out();
+                        skip_ref = 0;
+                    } else if (seg_kind[s] != 2) {
+                        skip_ref += seg_cnt[s];
+                    }
+                }
+                out.add(NS_OP_DEL << 28, skip_ref);
+            }
             ++n_runs;
         } else {
             for (uint32_t s = 0; s < nseg; ++s) {
@@ -230,6 +311,8 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
                     out.add(NS_OP_COPY << 28, seg_cnt[s]);
                 } else if (seg_kind[s] == 3) {
                     out.add(NS_OP_DEL << 28, seg_cnt[s]);
+                } else if (CHAIN && seg_kind[s] == 4) {
+                    next_out();
                 } else {
                     out.add((NS_OP_LIT << 28) | ((run_base & 3u) << 26) | ((seg_kind[s] == 1 ? 0u : 1u) << 24), seg_cnt[s]);
                     if (seg_kind[s] == 1) out.add(NS_OP_DEL << 28, seg_cnt[s]);
@@ -310,7 +393,10 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
             }
             need_flush = b != run_base || b > 3u;
         } else if (st == ST_OP) {
-            if (k >= n_ev) {                                // end of the segment's script
+            if (CHAIN && k >= n_ev && chain_left > 0) {     // end of a piece's script inside a chain
+                path = P_NEXT;                              // no room for a boundary marker (pathological run): closed here
+                need_flush = run_len != 0 && nseg >= HP_MAX_SEG - 1u;
+            } else if (k >= n_ev) {                         // end of the segment's script
                 path = P_END;
                 need_flush = true;
             } else {
@@ -398,16 +484,35 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
             }
         } else if (st == ST_OP) {
             if (path == P_END) {
-                NsPieceMeta& pm = *pmp;
-                out.flush();
-                if (!WRITE) {
-                    a.out_n_ops[this_piece] = out.n;
-                    pm.out_len = out.out_len;
+                if (CHAIN) {
+                    close_out();
                 } else {
-                    pm.op_off = a.out_off[this_piece];
-                    pm.n_ops = out.n;
+                    NsPieceMeta& pm = *pmp;
+                    out.flush();
+                    if (!WRITE) {
+                        a.out_n_ops[this_piece] = out.n;
+                        pm.out_len = out.out_len;
+                    } else {
+                        pm.op_off = a.out_off[this_piece];
+                        pm.n_ops = out.n;
+                    }
                 }
                 st = ST_FETCH;
+            } else if (CHAIN && path == P_NEXT) {
+                if (run_len == 0) {
+                    next_out();
+                } else {                                    // the pending run carries over: mark where the piece ends
+                    seg_kind[nseg] = 4;
+                    seg_cnt[nseg] = 0;
+                    ++nseg;
+                }
+                this_piece += 2;
+                --chain_left;
+                const NsPieceMeta& pm = a.pieces[this_piece];
+                w.piece_in_read = this_piece - rm.piece_first;
+                ev = a.ops + pm.ev_off;
+                n_ev = pm.ev_n_ops;
+                k = 0;
             } else if (path == P_HT) {
                 out.add(NS_OP_HT << 28, len);
             } else if (path == P_LIT) {
@@ -447,6 +552,41 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
             //      would otherwise keep one lane busy five times as long as any other)
             const uint32_t wi = atomicAdd(a.counter, 1u);
             if (wi >= a.n_pieces) break;
+            if (CHAIN) {
+                // ---- a chain: its first piece, then every NS_PIECE_CONT piece two further on
+                this_piece = a.order[wi];
+                const NsPieceMeta& pm = a.pieces[this_piece];
+                rm = a.reads[pm.read_slot];
+                rid = a.first_id + pm.read_slot;
+                w.seed = a.cfg.seed;
+                w.rid = rid;
+                w.K = K;
+                w.packed = false;
+                w.piece_in_read = w.head_pir = this_piece - rm.piece_first;
+                w.chain = &pm;
+                w.bases = a.ref.bases;
+                w.chrom_off = a.ref.chrom_off;
+                w.c_j = 0;
+                w.c_lo = 0;
+                w.load_piece();
+                uint32_t total = pm.ref_len;
+                chain_left = 0;
+                for (uint32_t q = w.head_pir + 2u; q < rm.n_pieces && (a.pieces[rm.piece_first + q].kind & NS_PIECE_CONT); q += 2u) {
+                    total += a.pieces[rm.piece_first + q].ref_len;
+                    ++chain_left;
+                }
+                w.ref_len = total;
+                ev = a.ops + pm.ev_off;
+                n_ev = pm.ev_n_ops;
+                k = 0;
+                rpos = 0;
+                out_piece = this_piece;
+                out.begin(WRITE ? a.ops + a.out_off[this_piece - a.piece_base] : nullptr);
+                run_base = 0xffu;
+                run_len = run_ref = nseg = n_runs = 0;
+                st = ST_OP;
+                continue;
+            }
             this_piece = a.order ? a.order[wi] : wi;
             pmp = &a.pieces[this_piece];
             NsPieceMeta& pm = *pmp;

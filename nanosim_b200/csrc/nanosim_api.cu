@@ -1107,13 +1107,19 @@ __global__ void hp_piece_keys(const NsPieceMeta* pieces, uint32_t n, uint32_t* k
     vals[i] = i;
 }
 
-__global__ void replace_reads(NsReadMeta* reads, const uint32_t* slots, const NsReadMeta* repl, uint32_t n, uint32_t n_reads) {
+// keep_off: the read keeps its slot in the sequence buffer (its bytes are overwritten in place)
+__global__ void replace_reads(NsReadMeta* reads, const uint32_t* slots, const NsReadMeta* repl, uint32_t n, uint32_t n_reads,
+                              uint32_t keep_off) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n && slots[i] < n_reads) {
         NsReadMeta r = repl[i];
-        r.seq_off = reads[slots[i]].seq_off;         // the bytes are overwritten in place
+        if (keep_off) r.seq_off = reads[slots[i]].seq_off;
         reads[slots[i]] = r;
     }
+}
+__global__ void gather_seq_len(const NsReadMeta* reads, const uint32_t* slots, uint32_t n, uint32_t n_reads, uint32_t* out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = slots[i] < n_reads ? reads[slots[i]].seq_len : 0u;
 }
 __global__ void iota_from(uint32_t* v, uint32_t n, uint32_t first) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1343,6 +1349,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         else CK(launch(ctx, plan_kernel<true>, plan_blocks, plan_tb, 0, pa));
     }
     CK(launch(ctx, copy_ev_fields, gp, tb, 0, pieces, n_pieces));
+    uint64_t raw_ev_off = 0, raw_ops = 0;
     if (hp && !ctx->hcfg.perfect) {
         // ---- homopolymer pass (hp_kernel.cuh): count, re-scan lengths and script offsets, write
         if (!tab.hmodel.has_hp) return fail(ctx, NS_ESTATE, "ns_simulate: -hp/-k needs homopolymer parameters in the model");
@@ -1369,6 +1376,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
             ha.order = v_out;
         }
         ha.force_exact = (ctx->hcfg.flags & NS_FLAG_EMIT_EXACT) ? 1u : 0u;
+        ha.piece_base = 0;
         const unsigned hp_blocks = std::min<unsigned>((n_pieces + 127) / 128, (unsigned)ctx->sm_count * 16u);
         CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
         CK(launch(ctx, hp_kernel<false>, hp_blocks, 128, 0, ha));
@@ -1378,9 +1386,16 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         CK(launch(ctx, add_base_u64, gp, tb, 0, ctx->hp_off.as<uint64_t>(), n_pieces, event_ops));
         if (int rc = read_layout(ctx, n)) return rc;
         if (int rc = publish_totals_and_wait(ctx)) return rc;
-        CK(ctx->ops.ensure_keep((size_t)(script_ops() + 4) * sizeof(uint32_t), (size_t)event_ops * sizeof(uint32_t), st));
+        // with intron retention, a verbatim copy of the event scripts goes behind the rewritten ones before the WRITE pass
+        // filters them in place: ns_reemit lays retaining reads out on the genome by cutting the unfiltered scripts
+        raw_ops = ctx->hcfg.trx_records ? event_ops : 0;
+        CK(ctx->ops.ensure_keep((size_t)(script_ops() + raw_ops + 4) * sizeof(uint32_t), (size_t)event_ops * sizeof(uint32_t), st));
         CK(ctx->seq.ensure((size_t)h_totals[2] + 16));
         if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)h_totals[2] + 16));
+        if (raw_ops) {
+            raw_ev_off = script_ops();
+            CK(cudaMemcpyAsync(ctx->ops.as<uint32_t>() + raw_ev_off, ctx->ops.p, (size_t)raw_ops * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+        }
         ha.ops = ctx->ops.as<uint32_t>();
         ha.out_off = ctx->hp_off.as<uint64_t>();
         CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
@@ -1420,7 +1435,8 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
 
     NsBatchInfo& bi = ctx->last;
     bi.seq_bytes = h_totals[2];
-    bi.n_ops = script_ops();
+    bi.n_ops = script_ops() + raw_ops;
+    bi.raw_ev_off = raw_ev_off;
     bi.total_bases = h_totals[3];
     bi.n_reads = n;
     bi.n_pieces = n_pieces;
@@ -1632,6 +1648,97 @@ int ns_transfer_info(NsContext* ctx, uint32_t* packed_bases, uint32_t* n_threads
     return NS_OK;
 }
 
+// ns_reemit on a -hp context, after the new pieces, their event scripts and the staging copies (scan_in: replacement reads,
+// scan_out: slots) are on the device: homopolymer pass over the chains, new sequence slots, emit, new totals
+static int reemit_hp(NsContext* ctx, uint32_t n_slots, uint32_t n_new_pieces, uint64_t n_new_ops,
+                     const std::vector<uint32_t>& heads) {
+    cudaStream_t st = ctx->stream;
+    const Tables& tab = *ctx->tables;
+    NsBatchInfo& bi = ctx->last;
+    const uint32_t old_np = bi.n_pieces, n_chains = (uint32_t)heads.size();
+    const uint64_t ev_end = bi.n_ops + n_new_ops;            // the new pieces' event scripts end here
+    const unsigned rb = (n_slots + 255) / 256;
+    NsReadMeta* staged = ctx->scan_in.as<NsReadMeta>();
+    const uint32_t* d_slots = ctx->scan_out.as<uint32_t>();
+    uint32_t* d_old_len = ctx->scan_out.as<uint32_t>() + n_slots;
+    CK(launch(ctx, gather_seq_len, rb, 256, 0, ctx->reads.as<NsReadMeta>(), d_slots, n_slots, bi.n_reads, d_old_len));
+    // the pass looks the chains up through the batch's reads: they point at the new pieces from here on
+    CK(launch(ctx, replace_reads, rb, 256, 0, ctx->reads.as<NsReadMeta>(), d_slots, staged, n_slots, bi.n_reads, 1u));
+    CK(ctx->hp_keys.ensure((size_t)n_chains * sizeof(uint32_t)));
+    CK(cudaMemcpyAsync(ctx->hp_keys.p, heads.data(), (size_t)n_chains * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CK(ctx->hp_off.ensure((size_t)n_new_pieces * sizeof(uint64_t)));
+    CK(cudaMemsetAsync(ctx->hp_off.p, 0, (size_t)n_new_pieces * sizeof(uint64_t), st));
+    HpArgs ha;
+    ha.ref = dev_ref(ctx);
+    ha.cfg = ctx->dcfg;
+    ha.first_id = ctx->last_first_id;
+    ha.reads = ctx->reads.as<NsReadMeta>();
+    ha.pieces = ctx->pieces.as<NsPieceMeta>();
+    ha.n_pieces = n_chains;
+    ha.ops = ctx->ops.as<uint32_t>();
+    ha.out_n_ops = ctx->hp_off.as<uint64_t>();
+    ha.out_off = nullptr;
+    memcpy(ha.hp, tab.hmodel.hp, sizeof ha.hp);
+    ha.hp_mis_rate = tab.hmodel.hp_mis_rate;
+    ha.counter = ctx->counter.as<uint32_t>();
+    ha.order = ctx->hp_keys.as<uint32_t>();
+    ha.force_exact = 1u;                                      // (chains take the byte-exact route regardless)
+    ha.piece_base = old_np;
+    const unsigned hp_blocks = std::min<unsigned>((n_chains + 127) / 128, (unsigned)ctx->sm_count * 16u);
+    CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
+    CK(launch(ctx, hp_kernel<false, true>, hp_blocks, 128, 0, ha));
+    CK(launch(ctx, hp_fix_reads, rb, 256, 0, staged, ha.pieces, n_slots));
+    // lay out on the host: the rewritten scripts behind the new event scripts, each replaced read in a new 16-byte-aligned
+    // slot behind the batch's bytes (its old slot is left unreferenced)
+    std::vector<NsReadMeta> hr(n_slots);
+    std::vector<uint64_t> off(n_new_pieces);
+    std::vector<uint32_t> old_len(n_slots);
+    CK(cudaMemcpyAsync(hr.data(), staged, (size_t)n_slots * sizeof(NsReadMeta), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(off.data(), ctx->hp_off.p, (size_t)n_new_pieces * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(old_len.data(), d_old_len, (size_t)n_slots * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    uint64_t op_end = ev_end;
+    for (uint32_t q = 0; q < n_new_pieces; ++q) {
+        const uint64_t c = off[q];
+        off[q] = op_end;
+        op_end += c;
+    }
+    uint64_t seq_end = bi.seq_bytes, total = bi.total_bases;
+    for (uint32_t k = 0; k < n_slots; ++k) {
+        seq_end = (seq_end + 15u) & ~(uint64_t)15u;
+        hr[k].seq_off = seq_end;
+        seq_end += hr[k].seq_len;
+        total += (uint64_t)hr[k].seq_len - old_len[k];
+    }
+    seq_end = (seq_end + 15u) & ~(uint64_t)15u;
+    CK(ctx->ops.ensure_keep((size_t)(op_end + 4) * sizeof(uint32_t), (size_t)ev_end * sizeof(uint32_t), st));
+    CK(ctx->seq.ensure_keep((size_t)seq_end + 16, (size_t)bi.seq_bytes, st));
+    if (ctx->hcfg.fastq) CK(ctx->qual.ensure_keep((size_t)seq_end + 16, (size_t)bi.seq_bytes, st));
+    CK(cudaMemcpyAsync(ctx->hp_off.p, off.data(), (size_t)n_new_pieces * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(staged, hr.data(), (size_t)n_slots * sizeof(NsReadMeta), cudaMemcpyHostToDevice, st));
+    CK(launch(ctx, replace_reads, rb, 256, 0, ctx->reads.as<NsReadMeta>(), d_slots, staged, n_slots, bi.n_reads, 0u));
+    ha.ops = ctx->ops.as<uint32_t>();
+    ha.out_off = ctx->hp_off.as<uint64_t>();
+    CK(cudaMemsetAsync(ctx->counter.p, 0, 64, st));
+    CK(launch(ctx, hp_kernel<true, true>, hp_blocks, 128, 0, ha));
+    CK(launch(ctx, iota_from, (n_new_pieces + 255) / 256, 256, 0, ctx->sort_vals.as<uint32_t>(), n_new_pieces, old_np));
+    if (int rc = launch_emit(ctx, NS_KIND_ALIGNED, ctx->last_first_id, n_new_pieces, ctx->sort_vals.as<uint32_t>(), nullptr, false))
+        return rc;
+    CK(cudaStreamSynchronize(st));
+    bi.n_pieces = old_np + n_new_pieces;
+    bi.n_ops = op_end;
+    bi.seq_bytes = seq_end;
+    bi.total_bases = total;
+    return NS_OK;
+}
+
+int ns_batch_info(NsContext* ctx, NsBatchInfo* info) {
+    if (!ctx || !info) return NS_EINVAL;
+    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "ns_batch_info: no simulated batch");
+    *info = ctx->last;
+    return NS_OK;
+}
+
 int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_reads, uint32_t n_slots,
               const NsPieceMeta* new_pieces, uint32_t n_new_pieces, const uint32_t* new_ops, uint64_t n_new_ops) {
     if (!ctx) return NS_EINVAL;
@@ -1656,18 +1763,46 @@ int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_
             (uint64_t)p.pos + p.ref_len > tab.h_chrom_off[p.chrom + 1] - tab.h_chrom_off[p.chrom])
             return fail(ctx, NS_EINVAL, "ns_reemit: piece %u is inconsistent with the batch or the reference", k);
     }
+    // -hp: the homopolymer pass runs again over each replaced read's pieces, as one chain (hp_kernel.cuh, CHAIN): they must
+    // be laid out as intron_retention.py lays them out -- genome segments two apart, every one but the first continuing the
+    // one before, zero-op gaps in between, one strand, event script == emitted script, no piece shared between reads
+    const bool hp = ctx->hcfg.kmer_bias > 0 && !ctx->hcfg.perfect;
+    std::vector<uint32_t> heads;
+    if (hp) {
+        uint64_t prev_end = old_np;
+        for (uint32_t k = 0; k < n_slots; ++k) {
+            const NsReadMeta& r = new_reads[k];
+            bool ok = r.piece_first >= prev_end && (r.n_pieces & 1u);
+            prev_end = (uint64_t)r.piece_first + r.n_pieces;
+            const NsPieceMeta* pc = new_pieces + (r.piece_first - old_np);
+            for (uint32_t q = 0; ok && q < r.n_pieces; ++q) {
+                const NsPieceMeta& p = pc[q];
+                ok = p.read_slot == read_slots[k];
+                if (q & 1u) {
+                    ok = ok && NS_PIECE_KIND(p.kind) == NS_PIECE_GAP && p.n_ops == 0;
+                } else {
+                    ok = ok && NS_PIECE_KIND(p.kind) == NS_PIECE_SEGMENT && (p.kind & NS_PIECE_GENOME) &&
+                         ((p.kind & NS_PIECE_CONT) != 0) == (q > 0) && (p.kind & NS_PIECE_REF_REV) == (pc[0].kind & NS_PIECE_REF_REV) &&
+                         p.ev_off == p.op_off && p.ev_n_ops == p.n_ops && p.ref_len > 0;
+                }
+            }
+            if (!ok) return fail(ctx, NS_EINVAL, "ns_reemit: the pieces of read %u do not form one chain of genome pieces", read_slots[k]);
+            heads.push_back(r.piece_first);
+        }
+    }
     CK(ctx->pieces.ensure_keep((size_t)(old_np + n_new_pieces + 1) * sizeof(NsPieceMeta), (size_t)old_np * sizeof(NsPieceMeta), st));
     CK(ctx->ops.ensure_keep((size_t)(old_ops + n_new_ops + 4) * sizeof(uint32_t), (size_t)old_ops * sizeof(uint32_t), st));
     CK(cudaMemcpyAsync(ctx->pieces.as<NsPieceMeta>() + old_np, new_pieces, (size_t)n_new_pieces * sizeof(NsPieceMeta), cudaMemcpyHostToDevice, st));
     if (n_new_ops) CK(cudaMemcpyAsync(ctx->ops.as<uint32_t>() + old_ops, new_ops, (size_t)n_new_ops * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     // staging for the slots / replacement reads / piece order: the scan buffers are free between batches
     CK(ctx->scan_in.ensure((size_t)n_slots * sizeof(NsReadMeta)));
-    CK(ctx->scan_out.ensure((size_t)n_slots * sizeof(uint32_t)));
+    CK(ctx->scan_out.ensure((size_t)n_slots * 2 * sizeof(uint32_t)));
     CK(ctx->sort_vals.ensure((size_t)n_new_pieces * sizeof(uint32_t)));
     CK(cudaMemcpyAsync(ctx->scan_in.p, new_reads, (size_t)n_slots * sizeof(NsReadMeta), cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(ctx->scan_out.p, read_slots, (size_t)n_slots * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    if (hp) return reemit_hp(ctx, n_slots, n_new_pieces, n_new_ops, heads);
     CK(launch(ctx, replace_reads, (n_slots + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), ctx->scan_out.as<uint32_t>(),
-              ctx->scan_in.as<NsReadMeta>(), n_slots, bi.n_reads));
+              ctx->scan_in.as<NsReadMeta>(), n_slots, bi.n_reads, 1u));
     CK(launch(ctx, iota_from, (n_new_pieces + 255) / 256, 256, 0, ctx->sort_vals.as<uint32_t>(), n_new_pieces, old_np));
     if (int rc = launch_emit(ctx, NS_KIND_ALIGNED, ctx->last_first_id, n_new_pieces, ctx->sort_vals.as<uint32_t>(), nullptr, false))
         return rc;

@@ -207,15 +207,16 @@ class Engine:
 
     def reemit(self, slots, new_reads, new_pieces, new_ops):
         """Intron retention (intron_retention.py): replaces the piece lists of reads `slots` of the last aligned batch and
-        emits those reads again in place (ns_reemit)."""
+        emits those reads again (ns_reemit; with -hp/-k they change length and move to new slots)."""
         slots = np.ascontiguousarray(slots, dtype=np.uint32)
         new_reads = np.ascontiguousarray(new_reads, dtype=L.READ_DTYPE)
         new_pieces = np.ascontiguousarray(new_pieces, dtype=L.PIECE_DTYPE)
         new_ops = np.ascontiguousarray(new_ops, dtype=np.uint32)
         self._check(self._lib.ns_reemit(self._ctx, _ptr(slots), _ptr(new_reads), len(slots), _ptr(new_pieces), len(new_pieces),
                                         _ptr(new_ops), C.c_uint64(len(new_ops))))
-        self.info.n_pieces += len(new_pieces)
-        self.info.n_ops += len(new_ops)
+        info = L.NsBatchInfo()
+        self._check(self._lib.ns_batch_info(self._ctx, C.byref(info)))
+        self.info = info
 
     def fetch_meta(self, want_ops=True):
         """reads / pieces / (ops) of the last batch without the sequence bytes."""

@@ -11,7 +11,9 @@ the read's pieces (one per interval, walked backwards for transcripts on the min
 cut at the interval boundaries.  ``ns_reemit`` uploads those pieces and runs the emit kernel on them again; as all emit
 randomness is indexed by the position in the read, inserted / head / tail bases and every quality value stay what they
 were -- only the bases copied or substituted from the reference change, exactly as when ``mutate_read`` is handed the
-genomic sequence instead of the spliced one (:1163-1181).
+genomic sequence instead of the spliced one (:1163-1181).  With -hp/-k the reference filters and rewrites the genomic
+read: the device then keeps the unfiltered event scripts (``raw_ev_off``), those are cut, and ``ns_reemit`` runs the
+homopolymer pass again over the read's genome pieces; the read changes length and its qualities are drawn anew.
 
 Kept from the device's first pass (documented deviation): whether the read carries a polyA tail (the reference re-decides
 it from the genomic end of the last feature, :186-189, which would change the read length).
@@ -222,10 +224,12 @@ class IntronRetention:
     def __init__(self, p_no_ir, structures, trx_lengths, genome_first_record):
         self.p_no_ir, self.st, self.trx_len, self.g0 = p_no_ir, structures, np.asarray(trx_lengths, dtype=np.int64), int(genome_first_record)
 
-    def plan_batch(self, reads, pieces, ops, first_id, seed, n_pieces_total, n_ops_total):
+    def plan_batch(self, reads, pieces, ops, first_id, seed, n_pieces_total, n_ops_total, raw_ev_off=0):
         """reads / pieces / ops: the fetched metadata of an aligned batch.  Returns None when no read of the batch retains an
         intron, else (slots, new_reads, new_pieces, new_ops): the patch ``Engine.reemit`` takes.  Offsets in the new
-        pieces are absolute (they land behind the batch's n_pieces_total pieces / n_ops_total ops)."""
+        pieces are absolute (they land behind the batch's n_pieces_total pieces / n_ops_total ops).
+        raw_ev_off (NsBatchInfo.raw_ev_off, -hp/-k): where the unfiltered event scripts start; the read's script is cut from
+        there (the -k filter and mutate_homo run again on the genomic read), else from the emitted script."""
         st = self.st
         p0 = reads["piece_first"].astype(np.int64)
         trx = pieces["chrom"][p0].astype(np.int64)
@@ -262,7 +266,10 @@ class IntronRetention:
                 continue                                     # a chromosome the genome file lacks (:1168-1170) / inconsistent annotation
             minus = bool(ivs[-1][3])                         # `interval.strand` after the loop (:1177)
             order = ivs[::-1] if minus else ivs              # pieces in the direction of the transcript
-            script = ops[int(pc["op_off"]):int(pc["op_off"]) + int(pc["n_ops"])]
+            if raw_ev_off:
+                script = ops[int(raw_ev_off) + int(pc["ev_off"]):int(raw_ev_off) + int(pc["ev_off"]) + int(pc["ev_n_ops"])]
+            else:
+                script = ops[int(pc["op_off"]):int(pc["op_off"]) + int(pc["n_ops"])]
             parts = split_script(script, np.cumsum([e - s for _, s, e, _, _ in order]).tolist())
             rd = reads[i].copy()
             rd["piece_first"] = piece_cursor

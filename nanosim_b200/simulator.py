@@ -291,7 +291,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             # intron retention (:1156-1183): decided on the host from the batch's metadata, the few affected reads are laid
             # out on the genome and emitted again (intron_retention.py)
             reads, pieces, ops = engine.fetch_meta()
-            patch = prof.ir.plan_batch(reads, pieces, ops, job[1], prof.seed, info.n_pieces, info.n_ops)
+            patch = prof.ir.plan_batch(reads, pieces, ops, job[1], prof.seed, info.n_pieces, info.n_ops, info.raw_ev_off)
             if patch is not None:
                 engine.reemit(*patch)
 
@@ -486,9 +486,6 @@ def main_transcriptome(args, parser_t):
     if max_len < min_len:
         sys.stderr.write("\nMaximum read length must be longer than Minimum read length!\n")
         parser_t.print_help(sys.stderr)
-        sys.exit(1)
-    if model_ir and args.homopolymer:
-        sys.stderr.write("\nnanosim_b200: -hp/-k cannot be combined with intron retention yet; add --no_model_ir\n")
         sys.exit(1)
     if model_ir and args.ref_g == '':
         sys.stderr.write("\nPlease provide a reference genome to simulate intron retention events!\n")
