@@ -237,3 +237,22 @@ __device__ __forceinline__ uint32_t converted_ref_base(uint32_t c, uint64_t seed
     uint32_t r8 = h & 0xffu, r3 = h >> 8;
     return resolve_iupac(c, r8, r3 == 255u ? 0u : r3 % 3u);
 }
+
+// Bases of a MIS / INS event that the homopolymer pass rewrites (hp_kernel.cuh, ST_BASE); the error-profile formatter
+// (host_io.cu) gives those events the same bases.  Base t of the event comes from byte t % 16 of Philox-7 block
+// (event index in the piece's event script << 8) + (t >> 4) on stream ST_EMIT_B of the piece (key: the seed).
+__host__ __device__ __forceinline__ uint4 event_base_block(uint2 key, uint64_t rid, uint32_t piece_in_read, uint32_t event,
+                                                           uint32_t t) {
+    return philox4x32_7(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_EMIT_B, 0, piece_in_read), (event << 8) + (t >> 4)), key);
+}
+__host__ __device__ __forceinline__ uint32_t event_byte(const uint4& blk, uint32_t t) {
+    const uint32_t wd = (t & 8u) ? ((t & 4u) ? blk.w : blk.z) : ((t & 4u) ? blk.y : blk.x);
+    return (wd >> (8u * (t & 3u))) & 0xffu;
+}
+// base index (A 0, C 1, T 2, G 3) from that byte: an inserted base is r8 & 3, a substituted one differs from the original
+// base index `orig`
+__host__ __device__ __forceinline__ uint32_t event_base(uint32_t r8, bool mis, uint32_t orig) {
+    if (!mis) return r8 & 3u;
+    const uint32_t rr = r8 == 255u ? 0u : r8;
+    return ((orig & 3u) + 1u + rr % 3u) & 3u;
+}

@@ -377,17 +377,13 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
             } else if (bsrc == SRC_EXACT) {
                 b = w.base_at(rpos + t);
             } else {
-                if ((t & 15u) == 0)
-                    rblk = philox4x32_7(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_EMIT_B, 0, w.piece_in_read), (kk << 8) + (t >> 4)), key);
-                const uint32_t wd = (t & 8u) ? ((t & 4u) ? rblk.w : rblk.z) : ((t & 4u) ? rblk.y : rblk.x);
-                const uint32_t r8 = (wd >> (8u * (t & 3u))) & 0xffu;
+                if ((t & 15u) == 0) rblk = event_base_block(key, rid, w.piece_in_read, kk, t);
+                const uint32_t r8 = event_byte(rblk, t);
                 if (bsrc == SRC_MIS) {
-                    const uint32_t orig = w.packed ? (w.bases16(rpos + t) & 3u) : w.base_at(rpos + t);
-                    const uint32_t rr = r8 == 255u ? 0u : r8;
-                    b = ((orig & 3u) + 1u + rr % 3u) & 3u;
+                    b = event_base(r8, true, w.packed ? (w.bases16(rpos + t) & 3u) : w.base_at(rpos + t));
                     bkind = 1;
                 } else {
-                    b = r8 & 3u;
+                    b = event_base(r8, false, 0u);
                     bkind = 2;
                 }
             }

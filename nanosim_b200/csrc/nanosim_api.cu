@@ -1,27 +1,17 @@
 // C ABI of libnanosim_b200.so (include/nanosim_b200.h): context, HBM residency of reference + model tables,
-// batch orchestration (plan -> scan -> script -> emit) on one CUDA stream, device->host fetch.
+// batch orchestration (plan -> scan -> script -> emit) on one CUDA stream, device->host fetch.  The entry points that need
+// no context (formatters, FASTA reader, expansion of the 2-bit bases) are in host_io.cu.
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
-#include <chrono>
-#if defined(__x86_64__)
-#include <immintrin.h>
-#endif
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <dlfcn.h>
-#include <fcntl.h>
-#include <sched.h>
-#include <sys/mman.h>
-#include <sys/stat.h>
-#include <unistd.h>
 #include <string>
 #include <memory>
-#include <mutex>
-#include <thread>
 #include <vector>
 
 #if __has_include(<nccl.h>)
@@ -37,6 +27,7 @@
 #include "emit_kernel.cuh"
 #include "uread_kernel.cuh"
 #include "hp_kernel.cuh"
+#include "host_io.h"
 
 namespace {
 
@@ -1460,141 +1451,6 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     return NS_OK;
 }
 
-namespace {
-// expands 2-bit bases (pack_bases_kernel) into ASCII with `nt` host threads
-#if defined(__x86_64__)
-// 32 characters from 8 packed bytes per step: every output byte gets its source byte (vpshufb), the three shifted copies
-// bring the byte's other 2-bit fields down, constant masks keep field j & 3 at output byte j, a second vpshufb turns the
-// indices into letters.  ~14 instructions per 32 bases instead of four table lookups: the expansion then runs at memory
-// speed, which is what 8 GPU processes sharing one host need.
-__attribute__((target("avx2"))) void unpack_range_avx2(const uint8_t* packed, uint8_t* seq, uint64_t lo, uint64_t hi, const char* abc) {
-    const __m256i spread = _mm256_setr_epi8(0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 6, 6, 6, 6, 7, 7, 7, 7);
-    const __m256i m0 = _mm256_set1_epi32(0x00000003), m1 = _mm256_set1_epi32(0x00000300), m2 = _mm256_set1_epi32(0x00030000),
-                  m3 = _mm256_set1_epi32(0x03000000);
-    const __m256i letters = _mm256_setr_epi8(abc[0], abc[1], abc[2], abc[3], 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, abc[0], abc[1], abc[2], abc[3], 0,
-                                             0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0);
-    const bool aligned32 = (reinterpret_cast<uintptr_t>(seq) & 31u) == 0;
-    for (uint64_t i = lo; i < hi; ++i) {              // unit: 32 characters
-        const __m128i x = _mm_loadl_epi64(reinterpret_cast<const __m128i*>(packed + 8 * i));
-        const __m256i src = _mm256_shuffle_epi8(_mm256_broadcastsi128_si256(x), spread);
-        const __m256i idx = _mm256_or_si256(_mm256_or_si256(_mm256_and_si256(src, m0), _mm256_and_si256(_mm256_srli_epi16(src, 2), m1)),
-                                            _mm256_or_si256(_mm256_and_si256(_mm256_srli_epi16(src, 4), m2), _mm256_and_si256(_mm256_srli_epi16(src, 6), m3)));
-        const __m256i out = _mm256_shuffle_epi8(letters, idx);
-        if (aligned32) _mm256_stream_si256(reinterpret_cast<__m256i*>(seq + 32 * i), out);     // written once, read much later
-        else _mm256_storeu_si256(reinterpret_cast<__m256i*>(seq + 32 * i), out);
-    }
-    _mm_sfence();
-}
-#endif
-
-void unpack_bases(const uint8_t* packed, uint8_t* seq, uint64_t seq_bytes, bool uracil, int nt) {
-#if defined(__x86_64__)
-    static const bool have_avx2 = __builtin_cpu_supports("avx2") && !getenv("NANOSIM_B200_NO_AVX2");
-    if (have_avx2) {
-        const char* abc2 = uracil ? "ACUG" : "ACTG";
-        const uint64_t whole32 = seq_bytes / 32;
-        nt = std::max(1, std::min(nt, 64));
-        if (nt == 1 || whole32 < (1u << 14)) {
-            unpack_range_avx2(packed, seq, 0, whole32, abc2);
-        } else {
-            std::vector<std::thread> th;
-            for (int t = 0; t < nt; ++t) {
-                const uint64_t lo = whole32 * t / nt, hi = whole32 * (t + 1) / nt;
-                if (hi > lo) th.emplace_back(unpack_range_avx2, packed, seq, lo, hi, abc2);
-            }
-            for (auto& x : th) x.join();
-        }
-        for (uint64_t k = whole32 * 32; k < seq_bytes; ++k) seq[k] = (uint8_t)abc2[(packed[k >> 2] >> (2 * (k & 3))) & 3u];
-        return;
-    }
-#endif
-    // two packed bytes -> eight characters per table lookup (512 KB table per alphabet, built once)
-    static std::vector<uint64_t> tables[2];
-    static std::once_flag once[2];
-    const char* abc = uracil ? "ACUG" : "ACTG";
-    std::call_once(once[uracil ? 1 : 0], [&] {
-        std::vector<uint64_t>& t = tables[uracil ? 1 : 0];
-        t.resize(65536);
-        for (uint32_t b = 0; b < 65536; ++b) {
-            uint64_t w = 0;
-            for (int j = 0; j < 8; ++j) w |= (uint64_t)(uint8_t)abc[(b >> (2 * j)) & 3u] << (8 * j);
-            t[b] = w;
-        }
-    });
-    const uint64_t* lut = tables[uracil ? 1 : 0].data();
-    const uint64_t whole = seq_bytes / 8;             // 16-bit groups that expand to 8 in-range characters
-    auto work = [&](uint64_t lo, uint64_t hi) {
-        const bool aligned8 = (reinterpret_cast<uintptr_t>(seq) & 7u) == 0;
-        for (uint64_t i = lo; i < hi; ++i) {
-            uint16_t b;
-            memcpy(&b, packed + 2 * i, 2);
-            const uint64_t w = lut[b];
-#if defined(__x86_64__)
-            // streaming store: the destination is written once and read much later (no read-for-ownership traffic)
-            if (aligned8) _mm_stream_si64(reinterpret_cast<long long*>(seq + 8 * i), (long long)w);
-            else memcpy(seq + 8 * i, &w, 8);
-#else
-            memcpy(seq + 8 * i, &w, 8);
-#endif
-        }
-#if defined(__x86_64__)
-        _mm_sfence();
-#endif
-    };
-    nt = std::max(1, std::min(nt, 64));
-    if (nt == 1 || whole < (1u << 16)) {
-        work(0, whole);
-    } else {
-        std::vector<std::thread> th;
-        for (int t = 0; t < nt; ++t) {
-            const uint64_t lo = whole * t / nt, hi = whole * (t + 1) / nt;
-            if (hi > lo) th.emplace_back(work, lo, hi);
-        }
-        for (auto& x : th) x.join();
-    }
-    for (uint64_t k = whole * 8; k < seq_bytes; ++k) seq[k] = (uint8_t)abc[(packed[k >> 2] >> (2 * (k & 3))) & 3u];
-}
-
-// CPUs this process can really use: the affinity mask, capped by the container's cgroup CPU quota (cpu.max) -- a container
-// can show many more logical CPUs than its quota grants
-unsigned effective_cpus() {
-    unsigned n = std::thread::hardware_concurrency();
-    cpu_set_t set;
-    if (sched_getaffinity(0, sizeof set, &set) == 0) n = (unsigned)CPU_COUNT(&set);
-    if (FILE* f = fopen("/sys/fs/cgroup/cpu.max", "r")) {
-        char q[64] = {0};
-        unsigned long long period = 0;
-        if (fscanf(f, "%63s %llu", q, &period) == 2 && strcmp(q, "max") != 0 && period > 0) {
-            const unsigned long long quota = strtoull(q, nullptr, 10);
-            const unsigned cores = (unsigned)((quota + period / 2) / period);
-            if (cores >= 1 && cores < n) n = cores;
-        }
-        fclose(f);
-    }
-    return n ? n : 4u;
-}
-
-int unpack_threads() {
-    static const int n = [] {
-        const char* e = getenv("NANOSIM_B200_UNPACK_THREADS");     // 0: copy the bases as ASCII (no packing)
-        if (e && *e) return std::max(0, atoi(e));
-        // packing only pays when the host can expand faster than PCIe delivers: one expanding thread per core this GPU
-        // process can count on (torchrun exports LOCAL_WORLD_SIZE), at most 16; with fewer than 6 the bases travel as ASCII
-        const char* lw = getenv("LOCAL_WORLD_SIZE");
-        const unsigned ranks = (lw && *lw) ? (unsigned)std::max(1, atoi(lw)) : 1u;
-        const unsigned per_rank = effective_cpus() / ranks;
-        return per_rank >= 6u ? (int)std::min(per_rank, 16u) : 0;
-    }();
-    return n;
-}
-}  // namespace
-
-int ns_unpack_bases(const uint8_t* packed, uint8_t* seq, uint64_t n_bases, int uracil, int threads) {
-    if (!packed || !seq) return NS_EINVAL;
-    unpack_bases(packed, seq, n_bases, uracil != 0, threads);
-    return NS_OK;
-}
-
 int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsPieceMeta* pieces, uint32_t* ops) {
     if (!ctx) return NS_EINVAL;
     if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "ns_fetch: no simulated batch");
@@ -1623,20 +1479,11 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
     if (reads) CK(cudaMemcpyAsync(reads, ctx->reads.p, (size_t)bi.n_reads * sizeof(NsReadMeta), cudaMemcpyDeviceToHost, st));
     if (pieces) CK(cudaMemcpyAsync(pieces, ctx->pieces.p, (size_t)bi.n_pieces * sizeof(NsPieceMeta), cudaMemcpyDeviceToHost, st));
     if (ops) CK(cudaMemcpyAsync(ops, ctx->ops.p, (size_t)bi.n_ops * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    static const bool trace = getenv("NANOSIM_B200_TRACE_FETCH") != nullptr;
-    const auto t0 = std::chrono::steady_clock::now();
-    auto ms_since = [&] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); };
-    double t_packed = 0, t_unpacked = 0;
     if (packed) {
         CK(cudaEventSynchronize(ctx->ev_pack));
-        t_packed = ms_since();
         unpack_bases(ctx->pack_host.as<uint8_t>(), seq, bi.seq_bytes, ctx->dcfg.uracil != 0, nt);
-        t_unpacked = ms_since();
     }
     CK(wait_stream(ctx, bi.seq_bytes >= (64u << 20)));
-    if (trace)
-        fprintf(stderr, "ns_fetch: %.2f GB bases; packed copy done after %.1f ms, expansion %.1f ms (%d threads), everything after %.1f ms\n",
-                bi.seq_bytes / 1e9, t_packed, t_unpacked - t_packed, nt, ms_since());
     return NS_OK;
 }
 
@@ -1845,632 +1692,6 @@ int ns_op_stats(NsContext* ctx, uint64_t* out) {
     CK(cudaMemcpyAsync(out, ctx->stats.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     return NS_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// host-side FASTA/FASTQ record formatting (simulator.py:1437-1443), multi-threaded memcpy-style assembly
-// ---------------------------------------------------------------------------------------------------------
-namespace {
-// Sink of a formatter thread: either the caller's buffer, or a private chunk that is written with pwrite() at the right
-// file position whenever it fills up (the records of one thread are contiguous in the output).
-struct ChunkSink {
-    char* out;                // buffer mode: start of the whole output
-    int fd;                   // file mode: descriptor + offset of the output's first byte in the file
-    uint64_t file_off;
-    std::vector<char> buf;
-    size_t used = 0;
-    uint64_t start = 0;       // output position of buf[0]
-    bool ok = true;
-    ChunkSink(char* o, int f, uint64_t fo) : out(o), fd(f), file_off(fo) {
-        if (fd >= 0) buf.resize(size_t(8) << 20);
-    }
-    char* reserve(uint64_t at, size_t n) {       // n bytes at output position `at` (positions only grow within a thread)
-        if (fd < 0) return out + at;
-        if (used + n > buf.size()) {
-            flush();
-            if (n > buf.size()) buf.resize(n);
-        }
-        if (used == 0) start = at;
-        char* p = buf.data() + used;
-        used += n;
-        return p;
-    }
-    void flush() {
-        size_t done = 0;
-        while (fd >= 0 && done < used) {
-            const ssize_t w = pwrite(fd, buf.data() + done, used - done, (off_t)(file_off + start + done));
-            if (w <= 0) {
-                ok = false;
-                break;
-            }
-            done += (size_t)w;
-        }
-        used = 0;
-    }
-};
-
-int64_t format_records_impl(const uint8_t* seq, const uint8_t* qual, const NsReadMeta* reads, uint32_t n_reads,
-                            const char* names, const uint64_t* name_off, int fastq, char* out, uint64_t out_cap,
-                            int n_threads, int fd, uint64_t file_off) {
-    if (!seq || !reads || !names || !name_off || (fastq && !qual)) return NS_EINVAL;
-    std::vector<uint64_t> off((size_t)n_reads + 1, 0);
-    for (uint32_t i = 0; i < n_reads; ++i) {
-        uint64_t nl = strlen(names + name_off[i]);
-        uint64_t rec = 1 + nl + 1 + reads[i].seq_len + 1;
-        if (fastq) rec += 2 + reads[i].seq_len + 1;
-        off[i + 1] = off[i] + rec;
-    }
-    if (fd < 0) {
-        if (!out) return (int64_t)off[n_reads];
-        if (off[n_reads] > out_cap) return NS_ENOMEM;
-    }
-    int nt = std::max(1, std::min(n_threads, 64));
-    std::vector<char> failed((size_t)nt, 0);
-    auto work = [&](uint32_t lo, uint32_t hi, int tid) {
-        ChunkSink sink(out, fd, file_off);
-        for (uint32_t i = lo; i < hi; ++i) {
-            char* p = sink.reserve(off[i], (size_t)(off[i + 1] - off[i]));
-            const char* nm = names + name_off[i];
-            size_t nl = strlen(nm);
-            *p++ = fastq ? '@' : '>';
-            memcpy(p, nm, nl);
-            p += nl;
-            *p++ = '\n';
-            memcpy(p, seq + reads[i].seq_off, reads[i].seq_len);
-            p += reads[i].seq_len;
-            *p++ = '\n';
-            if (fastq) {
-                *p++ = '+';
-                *p++ = '\n';
-                memcpy(p, qual + reads[i].seq_off, reads[i].seq_len);
-                p += reads[i].seq_len;
-                *p++ = '\n';
-            }
-        }
-        sink.flush();
-        if (!sink.ok) failed[tid] = 1;
-    };
-    if (nt == 1 || n_reads < 64) {
-        work(0, n_reads, 0);
-    } else {
-        std::vector<std::thread> th;
-        // split by bytes, not by reads, so threads carry equal copy volume
-        uint32_t lo = 0;
-        for (int t = 0; t < nt; ++t) {
-            uint64_t goal = off[n_reads] * (uint64_t)(t + 1) / nt;
-            uint32_t hi = (uint32_t)(std::upper_bound(off.begin(), off.end(), goal) - off.begin());
-            hi = std::min<uint32_t>(std::max<uint32_t>(hi, lo), n_reads);
-            if (t == nt - 1) hi = n_reads;
-            if (hi > lo) th.emplace_back(work, lo, hi, t);
-            lo = hi;
-        }
-        for (auto& x : th) x.join();
-    }
-    for (char f : failed)
-        if (f) return NS_EINVAL;
-    return (int64_t)off[n_reads];
-}
-}  // namespace
-
-int64_t ns_format_records(const uint8_t* seq, const uint8_t* qual, const NsReadMeta* reads, uint32_t n_reads,
-                          const char* names, const uint64_t* name_off, int fastq, char* out, uint64_t out_cap,
-                          int n_threads) {
-    return format_records_impl(seq, qual, reads, n_reads, names, name_off, fastq, out, out_cap, n_threads, -1, 0);
-}
-
-int64_t ns_write_records(int fd, uint64_t file_off, const uint8_t* seq, const uint8_t* qual, const NsReadMeta* reads,
-                         uint32_t n_reads, const char* names, const uint64_t* name_off, int fastq, int n_threads) {
-    if (fd < 0) return NS_EINVAL;
-    return format_records_impl(seq, qual, reads, n_reads, names, name_off, fastq, nullptr, 0, n_threads, fd, file_off);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// host-side <out>_aligned_error_profile rows (mutate_read's log, simulator.py:2006-2008; header written by the caller):
-// for every aligned segment, its error events right to left: name, position in the segment's reference, type, length,
-// reference bases, read bases.  Events come from the segment's EVENT script (after the -k filter); when the
-// homopolymer pass rewrote the emitted script, the bases of an event are the ones that pass fixed (hp_kernel.cuh:
-// byte t of Philox-7 block (event index << 8) + (t >> 4) of stream ST_EMIT_B), otherwise they are read back from the
-// sequence.  Two-call protocol like ns_format_records.
-// ---------------------------------------------------------------------------------------------------------
-namespace {
-inline int dec_len(uint64_t v) {
-    int n = 1;
-    while (v >= 10) {
-        v /= 10;
-        ++n;
-    }
-    return n;
-}
-inline char* put_dec(char* p, uint64_t v) {
-    char tmp[24];
-    int n = 0;
-    do {
-        tmp[n++] = (char)('0' + v % 10);
-        v /= 10;
-    } while (v);
-    while (n) *p++ = tmp[--n];
-    return p;
-}
-struct EvRow {
-    uint32_t type, len, ref_start, out_start, index, piece, ref_base;
-    bool rewritten;
-};
-}  // namespace
-
-static int64_t format_error_profile_impl(const uint8_t* seq, const NsReadMeta* reads, const NsPieceMeta* pieces, const uint32_t* ops,
-                                         uint32_t n_reads, const uint8_t* ref_bases, const uint64_t* chrom_off, const char* names,
-                                         const uint64_t* name_off, uint64_t seed, uint64_t first_id, char* out, uint64_t out_cap,
-                                         int n_threads, int fd, uint64_t file_off) {
-    if (!seq || !reads || !pieces || !ops || !ref_bases || !chrom_off || !names || !name_off) return NS_EINVAL;
-    static const char kTypes[3][4] = {"mis", "ins", "del"};
-    uint8_t comp[256];
-    for (int c = 0; c < 256; ++c) comp[c] = (uint8_t)c;
-    comp['A'] = 'T'; comp['T'] = 'A'; comp['C'] = 'G'; comp['G'] = 'C';
-    const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-    // one read: returns the bytes its rows take; writes them when p != nullptr
-    auto do_read = [&](uint32_t i, char* p) -> uint64_t {
-        const NsReadMeta& r = reads[i];
-        const char* nm = names + name_off[i];
-        const size_t nl = strlen(nm);
-        const uint64_t rid = first_id + i;
-        const uint32_t L = r.seq_len;
-        const uint8_t* rs = seq + r.seq_off;
-        const bool rev = r.reversed != 0;
-        uint64_t bytes = 0;
-        std::vector<EvRow> ev;
-        // the pieces of one mutate_read call: a segment plus the pieces that continue it (NS_PIECE_CONT, intron retention)
-        auto flush = [&]() {
-            for (size_t e = ev.size(); e-- > 0;) {
-                const EvRow& w = ev[e];
-                const NsPieceMeta& pc = pieces[r.piece_first + w.piece];
-                const uint64_t shown = (uint64_t)w.ref_base + w.ref_start;
-                const uint64_t row = nl + 1 + dec_len(shown) + 1 + 3 + 1 + dec_len(w.len) + 1 + (uint64_t)w.len + 1 + w.len + 1;
-                bytes += row;
-                if (!p) continue;
-                const uint64_t cstart = chrom_off[pc.chrom], clen = chrom_off[pc.chrom + 1] - cstart;
-                const bool back = (pc.kind & NS_PIECE_REF_REV) != 0;
-                memcpy(p, nm, nl);
-                p += nl;
-                *p++ = '\t';
-                p = put_dec(p, shown);
-                *p++ = '\t';
-                memcpy(p, kTypes[w.type - 1], 3);
-                p += 3;
-                *p++ = '\t';
-                p = put_dec(p, w.len);
-                *p++ = '\t';
-                char* refp = p;
-                if (w.type == NS_OP_INS) {
-                    memset(p, '-', w.len);
-                } else {
-                    for (uint32_t t = 0; t < w.len; ++t) {
-                        const uint32_t f = w.ref_start + t;             // offset in the piece, in the direction of the read
-                        uint64_t ab = (uint64_t)pc.pos + (back ? pc.ref_len - 1 - f : f);
-                        if (ab >= clen) ab -= clen;
-                        uint8_t c = ref_bases[cstart + ab];
-                        if (c >= 'a' && c <= 'z') c = (uint8_t)(c - 32);
-                        p[t] = (char)(back ? comp[c] : c);
-                    }
-                }
-                p += w.len;
-                *p++ = '\t';
-                if (w.type == NS_OP_DEL) {
-                    memset(p, '-', w.len);
-                } else if (w.rewritten) {
-                    for (uint32_t t = 0; t < w.len; ++t) {
-                        const uint4 blk = philox4x32_7(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_EMIT_B, 0, w.piece),
-                                                                  (w.index << 8) + (t >> 4)), key);
-                        const uint32_t word = ((t >> 2) & 3u) == 0 ? blk.x : (((t >> 2) & 3u) == 1 ? blk.y : (((t >> 2) & 3u) == 2 ? blk.z : blk.w));
-                        const uint32_t r8 = (word >> (8u * (t & 3u))) & 0xffu;
-                        uint32_t bi;
-                        if (w.type == NS_OP_INS) {
-                            bi = r8 & 3u;
-                        } else {
-                            const char rc = refp[t];
-                            const uint32_t orig = rc == 'C' ? 1u : (rc == 'T' ? 2u : (rc == 'G' ? 3u : 0u));
-                            const uint32_t rr = r8 == 255u ? 0u : r8;
-                            bi = (orig + 1u + rr % 3u) & 3u;
-                        }
-                        p[t] = "ACTG"[bi];
-                    }
-                } else {
-                    for (uint32_t t = 0; t < w.len; ++t) {
-                        const uint32_t x = w.out_start + t;
-                        p[t] = (char)(rev ? comp[rs[L - 1 - x]] : rs[x]);
-                    }
-                }
-                p += w.len;
-                *p++ = '\n';
-            }
-            ev.clear();
-        };
-        uint32_t ref_base = 0;
-        for (uint32_t k = 0; k < r.n_pieces; k += 2) {
-            const NsPieceMeta& pc = pieces[r.piece_first + k];
-            if (NS_PIECE_KIND(pc.kind) != NS_PIECE_SEGMENT) continue;
-            if (!(pc.kind & NS_PIECE_CONT)) {
-                flush();
-                ref_base = 0;
-            }
-            const uint32_t* sc = ops + pc.ev_off;
-            const bool rewritten = pc.ev_off != pc.op_off;
-            uint32_t o = pc.out_rel, rf = 0;
-            for (uint32_t j = 0; j < pc.ev_n_ops; ++j) {
-                const uint32_t op = sc[j], ty = NS_OP_TYPE(op), ln = NS_OP_LEN(op);
-                if (ty >= NS_OP_MIS && ty <= NS_OP_DEL && ln) ev.push_back(EvRow{ty, ln, rf, o, j, k, ref_base, rewritten});
-                if (ty != NS_OP_DEL) o += ln;
-                if (ty == NS_OP_COPY || ty == NS_OP_MIS || ty == NS_OP_DEL) rf += ln;
-            }
-            ref_base += pc.ref_len;
-        }
-        flush();
-        return bytes;
-    };
-    int nt = std::max(1, std::min(n_threads, 64));
-    std::vector<uint64_t> off((size_t)n_reads + 1, 0);
-    {
-        auto count = [&](uint32_t lo, uint32_t hi) {
-            for (uint32_t i = lo; i < hi; ++i) off[i + 1] = do_read(i, nullptr);
-        };
-        if (nt == 1 || n_reads < 64) {
-            count(0, n_reads);
-        } else {
-            std::vector<std::thread> th;
-            for (int t = 0; t < nt; ++t) {
-                uint32_t lo = (uint32_t)((uint64_t)n_reads * t / nt), hi = (uint32_t)((uint64_t)n_reads * (t + 1) / nt);
-                if (hi > lo) th.emplace_back(count, lo, hi);
-            }
-            for (auto& x : th) x.join();
-        }
-        for (uint32_t i = 0; i < n_reads; ++i) off[i + 1] += off[i];
-    }
-    if (fd < 0) {
-        if (!out) return (int64_t)off[n_reads];
-        if (off[n_reads] > out_cap) return NS_ENOMEM;
-    }
-    std::vector<char> failed((size_t)nt + 1, 0);
-    int next_tid = 0;
-    auto fill = [&](uint32_t lo, uint32_t hi, int tid) {
-        ChunkSink sink(out, fd, file_off);
-        for (uint32_t i = lo; i < hi; ++i)
-            if (off[i + 1] > off[i]) do_read(i, sink.reserve(off[i], (size_t)(off[i + 1] - off[i])));
-        sink.flush();
-        if (!sink.ok) failed[tid] = 1;
-    };
-    if (nt == 1 || n_reads < 64) {
-        fill(0, n_reads, 0);
-    } else {
-        std::vector<std::thread> th;
-        uint32_t lo = 0;
-        for (int t = 0; t < nt; ++t) {
-            uint64_t goal = off[n_reads] * (uint64_t)(t + 1) / nt;
-            uint32_t hi = (uint32_t)(std::upper_bound(off.begin(), off.end(), goal) - off.begin());
-            hi = std::min<uint32_t>(std::max<uint32_t>(hi, lo), n_reads);
-            if (t == nt - 1) hi = n_reads;
-            if (hi > lo) th.emplace_back(fill, lo, hi, next_tid++);
-            lo = hi;
-        }
-        for (auto& x : th) x.join();
-    }
-    for (char f : failed)
-        if (f) return NS_EINVAL;
-    return (int64_t)off[n_reads];
-}
-
-int64_t ns_format_error_profile(const uint8_t* seq, const NsReadMeta* reads, const NsPieceMeta* pieces, const uint32_t* ops,
-                                uint32_t n_reads, const uint8_t* ref_bases, const uint64_t* chrom_off, const char* names,
-                                const uint64_t* name_off, uint64_t seed, uint64_t first_id, char* out, uint64_t out_cap,
-                                int n_threads) {
-    return format_error_profile_impl(seq, reads, pieces, ops, n_reads, ref_bases, chrom_off, names, name_off, seed, first_id, out,
-                                     out_cap, n_threads, -1, 0);
-}
-
-int64_t ns_write_error_profile(int fd, uint64_t file_off, const uint8_t* seq, const NsReadMeta* reads, const NsPieceMeta* pieces,
-                               const uint32_t* ops, uint32_t n_reads, const uint8_t* ref_bases, const uint64_t* chrom_off,
-                               const char* names, const uint64_t* name_off, uint64_t seed, uint64_t first_id, int n_threads) {
-    if (fd < 0) return NS_EINVAL;
-    return format_error_profile_impl(seq, reads, pieces, ops, n_reads, ref_bases, chrom_off, names, name_off, seed, first_id, nullptr,
-                                     0, n_threads, fd, file_off);
-}
-
-
-// ---------------------------------------------------------------------------------------------------------
-// host-side read names (simulator.py:1390-1402 genome, :965-969 metagenome, :1188-1219 transcriptome, :1332-1343 perfect,
-// :1511/:1529-1534 unaligned), written as NUL-terminated strings back to back -- the layout ns_format_records and
-// ns_format_error_profile take.  flags: bit 0 perfect, bit 1 metagenome (gap lengths in the name), bit 2 transcriptome.
-// ---------------------------------------------------------------------------------------------------------
-int64_t ns_format_names(const NsReadMeta* reads, const NsPieceMeta* pieces, uint32_t n_reads, int kind, uint32_t flags,
-                        uint64_t index_base, const char* chrom_names, const uint64_t* chrom_name_off, char* out,
-                        uint64_t out_cap, uint64_t* name_off) {
-    if (!reads || !pieces || !chrom_names || !chrom_name_off) return NS_EINVAL;
-    const bool perfect = flags & 1u, meta = flags & 2u, trx = flags & 4u;
-    // the reads are cut into ranges, one per thread; every thread builds the names of its range back to back in its own blob
-    static const int name_threads = std::max(1, std::min(env_int("NANOSIM_B200_NAME_THREADS", 8), 64));
-    const int nt = n_reads < 4096 ? 1 : name_threads;
-    std::vector<std::string> blobs((size_t)nt);
-    std::vector<std::vector<uint32_t>> lens((size_t)nt);
-    auto work = [&](int tid) {
-    const uint32_t lo = (uint32_t)((uint64_t)n_reads * tid / nt), hi = (uint32_t)((uint64_t)n_reads * (tid + 1) / nt);
-    std::string& blob = blobs[tid];
-    std::vector<uint32_t>& ln = lens[tid];
-    blob.reserve((size_t)(hi - lo) * 64);
-    ln.reserve(hi - lo);
-    std::string nm;
-    char num[32];
-    auto add_num = [&](uint64_t v) {
-        char* e = put_dec(num, v);
-        nm.append(num, (size_t)(e - num));
-    };
-    for (uint32_t i = lo; i < hi; ++i) {
-        const NsReadMeta& r = reads[i];
-        const NsPieceMeta* pc = pieces + r.piece_first;
-        const char strand = r.reversed ? 'R' : 'F';
-        nm.clear();
-        if (kind == NS_KIND_UNALIGNED) {
-            nm += chrom_names + chrom_name_off[pc[0].chrom];
-            nm += '_';
-            add_num(pc[0].pos);
-            nm += "_unaligned_";
-            add_num(index_base + i);
-            nm += '_';
-            nm += strand;
-            nm += "_0_";
-            add_num(pc[0].ref_len);
-            nm += "_0";
-        } else if (trx && (pc[0].kind & NS_PIECE_GENOME)) {
-            // intron-retention layout (:1188-1192, :1217-1219): transcript, genomic start of the first interval, the
-            // retained-intron intervals the read covers in genomic order
-            uint64_t first_pos = pc[0].pos, mid = 0;
-            for (uint32_t k = 0; k < r.n_pieces; k += 2) {
-                first_pos = std::min<uint64_t>(first_pos, pc[k].pos);
-                mid += pc[k].ref_len;
-            }
-            nm += chrom_names + chrom_name_off[pc[0].ref_req];
-            nm += '_';
-            add_num(first_pos);
-            nm += "_aligned_";
-            add_num(index_base + i);
-            bool any = false;
-            for (uint32_t k = 0; k < r.n_pieces; k += 2) any = any || (pc[k].kind & NS_PIECE_RETAINED);
-            if (any) {
-                nm += "_RetainedIntron_";
-                std::vector<std::pair<uint64_t, uint64_t>> ivs;              // in genomic order, whatever the strand
-                for (uint32_t k = 0; k < r.n_pieces; k += 2)
-                    if (pc[k].kind & NS_PIECE_RETAINED) ivs.emplace_back(pc[k].pos, (uint64_t)pc[k].pos + pc[k].ref_len);
-                std::stable_sort(ivs.begin(), ivs.end());
-                for (const auto& iv : ivs) {
-                    add_num(iv.first);
-                    nm += '-';
-                    add_num(iv.second);
-                    nm += ';';
-                }
-            }
-            nm += '_';
-            nm += strand;
-            nm += '_';
-            add_num(r.head);
-            nm += '_';
-            add_num(mid);
-            nm += '_';
-            add_num((uint64_t)r.tail + pc[0].polya_len);
-        } else if (trx) {
-            nm += chrom_names + chrom_name_off[pc[0].chrom];
-            nm += '_';
-            add_num(pc[0].pos);
-            nm += perfect ? "_perfect_" : "_aligned_";
-            add_num(index_base + i);
-            nm += '_';
-            nm += strand;
-            nm += '_';
-            add_num(r.head);
-            nm += '_';
-            add_num(pc[0].ref_len);
-            nm += '_';
-            add_num((uint64_t)r.tail + pc[0].polya_len);
-        } else if (perfect) {
-            uint64_t sum = 0;
-            for (uint32_t k = 0; k < r.n_pieces; k += 2) {
-                nm += chrom_names + chrom_name_off[pc[k].chrom];
-                nm += '_';
-                add_num(pc[k].pos);
-                sum += pc[k].ref_len;
-            }
-            nm += "_perfect_";
-            add_num(index_base + i);
-            nm += '_';
-            nm += strand;
-            nm += "_0_";
-            add_num(sum);
-            nm += "_0";
-        } else {
-            for (uint32_t k = 0; k < r.n_pieces; ++k) {
-                if (k & 1u) {
-                    if (!meta) continue;
-                    nm += ";gap_";
-                    add_num(pc[k].out_len);
-                    continue;
-                }
-                if (k) nm += ';';
-                nm += chrom_names + chrom_name_off[pc[k].chrom];
-                nm += '_';
-                add_num(pc[k].pos);
-            }
-            nm += "_aligned_";
-            add_num(index_base + i);
-            if (r.n_pieces > 1) nm += "_chimeric";
-            nm += '_';
-            nm += strand;
-            nm += '_';
-            add_num(r.head);
-            nm += '_';
-            for (uint32_t k = 0; k < r.n_pieces; k += 2) {
-                if (k) nm += ';';
-                add_num(pc[k].ref_len);
-            }
-            nm += '_';
-            add_num(r.tail);
-        }
-        blob.append(nm.c_str(), nm.size() + 1);
-        ln.push_back((uint32_t)nm.size() + 1);
-    }
-    };
-    if (nt == 1) {
-        work(0);
-    } else {
-        std::vector<std::thread> th;
-        for (int t = 1; t < nt; ++t) th.emplace_back(work, t);
-        work(0);
-        for (auto& x : th) x.join();
-    }
-    uint64_t total = 0;
-    for (const std::string& bl : blobs) total += bl.size();
-    if (!out) return (int64_t)total;
-    if (total > out_cap) return NS_ENOMEM;
-    uint64_t pos = 0;
-    uint32_t i = 0;
-    for (int t = 0; t < nt; ++t) {
-        memcpy(out + pos, blobs[t].data(), blobs[t].size());
-        if (name_off)
-            for (uint32_t l : lens[t]) {
-                name_off[i++] = pos;
-                pos += l;
-            }
-        else
-            pos += blobs[t].size();
-    }
-    return (int64_t)total;
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// FASTA / FASTQ reader of read_profile (simulator.py:341-349 with readfq :709-740): the file is mmap()ed and cut into
-// line-aligned chunks; every thread finds the record headers of its chunk and counts its sequence bytes (pass 1), a prefix
-// sum places the chunks, and the threads copy their sequence lines behind one another (pass 2).  Bytes are kept as they are
-// (case, IUPAC codes); line ends (\n, \r\n) are dropped.  A FASTQ file (first byte '@') is read by one thread: its
-// quality lines can begin with '>' or '@'.
-// Two-call protocol: with bases == NULL only *n_records, *n_bases and *header_bytes are set.  rec_off gets n_records + 1
-// offsets into bases; headers gets the header lines (without the marker) NUL-terminated back to back, header_off their starts.
-// ---------------------------------------------------------------------------------------------------------
-namespace {
-struct FaChunk {
-    const char* lo;
-    const char* hi;
-    uint64_t n_bases = 0;
-    std::vector<std::pair<const char*, uint64_t>> heads;      // header line start (at the marker), sequence bytes of the chunk before it
-};
-inline const char* line_end(const char* p, const char* end) {
-    const char* nl = (const char*)memchr(p, '\n', (size_t)(end - p));
-    return nl ? nl : end;
-}
-inline size_t trimmed(const char* p, const char* e) {         // line length without a trailing \r
-    return (e > p && e[-1] == '\r') ? (size_t)(e - p - 1) : (size_t)(e - p);
-}
-}  // namespace
-
-int64_t ns_read_fasta(const char* path, uint8_t* bases, uint64_t bases_cap, uint64_t* rec_off, char* headers, uint64_t headers_cap,
-                      uint64_t* header_off, uint32_t* n_records, uint64_t* n_bases, uint64_t* header_bytes, int n_threads) {
-    if (!path || !n_records || !n_bases || !header_bytes) return NS_EINVAL;
-    const int fd = open(path, O_RDONLY);
-    if (fd < 0) return NS_EINVAL;
-    struct stat sb;
-    if (fstat(fd, &sb) != 0) {
-        close(fd);
-        return NS_EINVAL;
-    }
-    const size_t size = (size_t)sb.st_size;
-    *n_records = 0;
-    *n_bases = *header_bytes = 0;
-    if (size == 0) {
-        close(fd);
-        return 0;
-    }
-    const char* base = (const char*)mmap(nullptr, size, PROT_READ, MAP_PRIVATE, fd, 0);
-    close(fd);
-    if (base == MAP_FAILED) return NS_ENOMEM;
-    madvise((void*)base, size, MADV_SEQUENTIAL);
-    const char* end = base + size;
-    const bool fastq = base[0] == '@';
-    int nt = fastq ? 1 : std::max(1, std::min(n_threads, 64));
-    if (size < (size_t(1) << 22)) nt = 1;
-    std::vector<FaChunk> ch((size_t)nt);
-    for (int t = 0; t < nt; ++t) {                             // line-aligned chunk boundaries
-        const char* p = base + size * (size_t)t / (size_t)nt;
-        if (t > 0) {
-            p = line_end(p - 1, end);
-            if (p < end) ++p;
-        }
-        ch[t].lo = p;
-        if (t > 0) ch[t - 1].hi = p;
-    }
-    ch[nt - 1].hi = end;
-    const bool fill = bases != nullptr;
-    // pass 1 / pass 2 over one chunk; FASTQ: sequence lines run to the '+' line, then as many quality bytes are skipped
-    auto walk = [&](FaChunk& c, uint8_t* dst) {
-        const char* p = c.lo;
-        uint64_t count = 0;
-        bool in_qual = false;
-        uint64_t qual_left = 0, rec_bases = 0;
-        while (p < c.hi) {
-            const char* e = line_end(p, c.hi);
-            const size_t len = trimmed(p, e);
-            if (fastq && in_qual) {
-                if (qual_left <= len) in_qual = false; else qual_left -= len;
-            } else if (len && (p[0] == '>' || (fastq && p[0] == '@'))) {
-                if (!dst) c.heads.emplace_back(p, count);
-                rec_bases = 0;
-            } else if (fastq && len && p[0] == '+') {
-                in_qual = rec_bases > 0;
-                qual_left = rec_bases;
-            } else if (len) {
-                if (dst) memcpy(dst + count, p, len);
-                count += len;
-                rec_bases += len;
-            }
-            p = e < c.hi ? e + 1 : c.hi;
-        }
-        if (!dst) c.n_bases = count;
-    };
-    {
-        std::vector<std::thread> th;
-        for (int t = 1; t < nt; ++t) th.emplace_back([&, t] { walk(ch[t], nullptr); });
-        walk(ch[0], nullptr);
-        for (auto& x : th) x.join();
-    }
-    uint64_t total = 0, n_rec = 0, hbytes = 0;
-    std::vector<uint64_t> chunk_off((size_t)nt);
-    for (int t = 0; t < nt; ++t) {
-        chunk_off[t] = total;
-        total += ch[t].n_bases;
-        n_rec += ch[t].heads.size();
-        for (auto& h : ch[t].heads) hbytes += trimmed(h.first, line_end(h.first, end));       // marker dropped, NUL added
-    }
-    *n_records = (uint32_t)n_rec;
-    *n_bases = total;
-    *header_bytes = hbytes;
-    int64_t rc = (int64_t)total;
-    if (fill) {
-        if (total > bases_cap || hbytes > headers_cap || !rec_off || !headers || !header_off) {
-            rc = NS_ENOMEM;
-        } else {
-            uint64_t r = 0, hpos = 0;
-            for (int t = 0; t < nt; ++t)
-                for (auto& h : ch[t].heads) {
-                    rec_off[r] = chunk_off[t] + h.second;
-                    const size_t hl = trimmed(h.first, line_end(h.first, end)) - 1;
-                    header_off[r] = hpos;
-                    memcpy(headers + hpos, h.first + 1, hl);
-                    headers[hpos + hl] = 0;
-                    hpos += hl + 1;
-                    ++r;
-                }
-            rec_off[n_rec] = total;
-            std::vector<std::thread> th;
-            for (int t = 1; t < nt; ++t) th.emplace_back([&, t] { walk(ch[t], bases + chunk_off[t]); });
-            walk(ch[0], bases + chunk_off[0]);
-            for (auto& x : th) x.join();
-        }
-    }
-    munmap((void*)base, size);
-    return rc;
 }
 
 // ---------------------------------------------------------------------------------------------------------
