@@ -350,6 +350,16 @@ int64_t ns_write_error_profile(int fd, uint64_t file_off, const uint8_t* seq, co
                                const uint32_t* ops, uint32_t n_reads, const uint8_t* ref_bases, const uint64_t* chrom_off,
                                const char* names, const uint64_t* name_off, uint64_t seed, uint64_t first_id, int n_threads);
 
+/* The last batch's FASTA/FASTQ text (ns_format_records' bytes, after ns_reemit as well) as BGZF, built on the device: the
+ * text is cut into blocks of 56 KiB (the last one shorter) and every block becomes one gzip member of at most 64 KiB with
+ * the BGZF extra field, one dynamic-Huffman DEFLATE block each, so gzip, zcat and htslib read the members and their
+ * concatenation.  The end-of-file block is not included.  names / name_off: the layout ns_format_records takes (uploaded
+ * by this call).  The members stay in HBM until the next ns_simulate / ns_reemit; *nbytes = their size.  NS_ESTATE if a
+ * member came out larger than 64 KiB (cannot happen: see nanosim_b200/csrc/bgzf_kernel.cuh). */
+int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
+/* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' *nbytes. */
+int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap);
+
 /* Host-side read names of a fetched batch in the reference's formats (genome :1390-1402, metagenome :965-969,
  * transcriptome :1188-1219, perfect :1332-1343, unaligned :1511/:1529-1534), written as NUL-terminated strings back to
  * back (name_off[i] = start of read i's name): the layout the two formatters above take.  flags: bit 0 perfect,

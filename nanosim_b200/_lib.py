@@ -23,7 +23,8 @@ NS_STATS_COMP_OFF = NS_STATS_INS_OFF + 4
 NS_STATS_WORDS = NS_STATS_COMP_OFF + 4
 
 EXPORTS = ["ns_create", "ns_destroy", "ns_last_error", "ns_clone", "ns_set_abundance", "ns_set_expression", "ns_set_reference", "ns_set_model", "ns_configure",
-           "ns_simulate", "ns_fetch", "ns_reemit", "ns_batch_info", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases"]
+           "ns_simulate", "ns_fetch", "ns_reemit", "ns_batch_info", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases",
+           "ns_compress_records", "ns_fetch_compressed"]
 
 
 class NsReference(C.Structure):
@@ -170,5 +171,9 @@ def lib():
     L.ns_reemit.restype = C.c_int
     L.ns_batch_info.argtypes = [P, C.POINTER(NsBatchInfo)]
     L.ns_batch_info.restype = C.c_int
+    L.ns_compress_records.argtypes = [P, P, P, C.POINTER(C.c_uint64)]
+    L.ns_compress_records.restype = C.c_int
+    L.ns_fetch_compressed.argtypes = [P, P, C.c_uint64]
+    L.ns_fetch_compressed.restype = C.c_int
     _lib = L
     return L

@@ -27,6 +27,7 @@
 #include "emit_kernel.cuh"
 #include "uread_kernel.cuh"
 #include "hp_kernel.cuh"
+#include "bgzf_kernel.cuh"
 #include "host_io.h"
 
 namespace {
@@ -153,6 +154,11 @@ struct NsContext {
     PinnedBuf pack_host;
     Event ev_pack;
     Event ev_block;                 // cudaEventBlockingSync: long waits sleep instead of spinning (wait_stream)
+    // ns_compress_records: the uploaded names, record layout, members as the deflate kernel leaves them, and the packed
+    // BGZF members of the last batch (z_bytes of z_out; valid while have_z)
+    DevBuf z_names, z_name_off, z_name_len, z_rec_off, z_stage, z_msize, z_moff, z_trailer, z_out;
+    uint64_t z_bytes = 0;
+    bool have_z = false;
     // Batches of one job have near-identical sizes: once a batch of a kind has run with host-sized buffers, the next ones
     // are submitted in one go (no host round trip between the first and the last kernel) against those capacities; a
     // kernel checks them on the device and a batch that does not fit is simply run again the sized way.
@@ -1135,6 +1141,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     ctx->have_batch = false;
+    ctx->have_z = false;
     memset(&ctx->last, 0, sizeof ctx->last);
     if (n_reads == 0) {
         if (info) *info = ctx->last;
@@ -1487,6 +1494,96 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
     return NS_OK;
 }
 
+// totals[] slots of ns_compress_records (behind the batch's): text bytes, compressed bytes, members above 64 KiB
+#define NS_T_Z_TEXT 12
+#define NS_T_Z_BYTES 13
+#define NS_T_Z_OVERSIZE 14
+
+int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    if (!ctx) return NS_EINVAL;
+    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "ns_compress_records: null argument");
+    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "ns_compress_records: no simulated batch");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    const NsBatchInfo& bi = ctx->last;
+    const uint32_t n = bi.n_reads;
+    ctx->have_z = false;
+    ctx->z_bytes = 0;
+    if (n == 0) {
+        ctx->have_z = true;
+        *nbytes = 0;
+        return NS_OK;
+    }
+    uint64_t blob = 0;                      // the names' extent: every name with its NUL
+    for (uint32_t i = 0; i < n; ++i) blob = std::max<uint64_t>(blob, name_off[i] + strlen(names + name_off[i]) + 1);
+    CK(upload(ctx->z_names, names, blob, st));
+    CK(upload(ctx->z_name_off, name_off, (size_t)n * sizeof(uint64_t), st));
+    CK(ctx->z_name_len.ensure((size_t)n * sizeof(uint32_t)));
+    CK(ctx->z_rec_off.ensure((size_t)n * sizeof(uint64_t)));
+    CK(ctx->scan_in.ensure((size_t)n * sizeof(uint64_t)));
+    uint64_t* totals = ctx->totals.as<uint64_t>();
+    CK(cudaMemsetAsync(totals + NS_T_Z_TEXT, 0, 3 * sizeof(uint64_t), st));
+    const uint32_t fastq = ctx->hcfg.fastq ? 1u : 0u;
+    CK(launch(ctx, bgzf_record_size, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
+              ctx->z_name_off.as<uint64_t>(), fastq, ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>()));
+    if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->z_rec_off.as<uint64_t>(), n, NS_T_Z_TEXT)) return rc;
+    if (int rc = publish_totals_and_wait(ctx)) return rc;
+    const uint64_t text = ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT];
+    const uint64_t n_blocks64 = (text + BGZF_BLOCK - 1) / BGZF_BLOCK;
+    if (n_blocks64 > 0x7fffffffu) return fail(ctx, NS_EINVAL, "ns_compress_records: %llu bytes of text is too much for one call",
+                                              (unsigned long long)text);
+    const uint32_t n_blocks = (uint32_t)n_blocks64;
+    CK(ctx->z_stage.ensure((size_t)n_blocks * BGZF_SLOT));
+    CK(ctx->z_msize.ensure((size_t)n_blocks * sizeof(uint64_t)));
+    CK(ctx->z_moff.ensure((size_t)n_blocks * sizeof(uint64_t)));
+    CK(ctx->z_trailer.ensure((size_t)n_blocks * sizeof(uint2)));
+    BgzfArgs za;
+    za.reads = ctx->reads.as<NsReadMeta>();
+    za.seq = ctx->seq.as<uint8_t>();
+    za.qual = fastq ? ctx->qual.as<uint8_t>() : nullptr;
+    za.names = ctx->z_names.as<char>();
+    za.name_off = ctx->z_name_off.as<uint64_t>();
+    za.name_len = ctx->z_name_len.as<uint32_t>();
+    za.rec_off = ctx->z_rec_off.as<uint64_t>();
+    za.n_reads = n;
+    za.fastq = fastq;
+    za.text_bytes = text;
+    za.stage = ctx->z_stage.as<uint8_t>();
+    za.member_size = ctx->z_msize.as<uint64_t>();
+    za.trailer = ctx->z_trailer.as<uint2>();
+    za.oversize = (unsigned long long*)(totals + NS_T_Z_OVERSIZE);
+    CK(cudaFuncSetAttribute(bgzf_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BgzfSmem)));
+    CK(launch(ctx, bgzf_deflate_kernel, n_blocks, BGZF_THREADS, sizeof(BgzfSmem), za));
+    if (int rc = scan_total(ctx, ctx->z_msize.as<uint64_t>(), ctx->z_moff.as<uint64_t>(), n_blocks, NS_T_Z_BYTES)) return rc;
+    if (int rc = publish_totals_and_wait(ctx)) return rc;
+    const uint64_t* h = ctx->h_totals.as<uint64_t>();
+    if (h[NS_T_Z_OVERSIZE])
+        return fail(ctx, NS_ESTATE, "ns_compress_records: %llu BGZF members exceed %u bytes", (unsigned long long)h[NS_T_Z_OVERSIZE],
+                    BGZF_MAX_MEMBER);
+    const uint64_t total = h[NS_T_Z_BYTES];
+    CK(ctx->z_out.ensure((size_t)total));
+    CK(launch(ctx, bgzf_pack_kernel, n_blocks, 256, 0, (const uint8_t*)ctx->z_stage.p, (const uint64_t*)ctx->z_msize.p,
+              (const uint64_t*)ctx->z_moff.p, (const uint2*)ctx->z_trailer.p, ctx->z_out.as<uint8_t>()));
+    CK(wait_stream(ctx, false));
+    ctx->z_bytes = total;
+    ctx->have_z = true;
+    *nbytes = total;
+    return NS_OK;
+}
+
+int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap) {
+    if (!ctx) return NS_EINVAL;
+    if (!ctx->have_z) return fail(ctx, NS_ESTATE, "ns_fetch_compressed: the last batch has not been compressed");
+    if (cap < ctx->z_bytes) return fail(ctx, NS_ENOMEM, "ns_fetch_compressed: %llu bytes do not fit in %llu",
+                                        (unsigned long long)ctx->z_bytes, (unsigned long long)cap);
+    if (ctx->z_bytes == 0) return NS_OK;
+    if (!out) return fail(ctx, NS_EINVAL, "ns_fetch_compressed: null argument");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(out, ctx->z_out.p, ctx->z_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(wait_stream(ctx, ctx->z_bytes >= (64u << 20)));
+    return NS_OK;
+}
+
 int ns_transfer_info(NsContext* ctx, uint32_t* packed_bases, uint32_t* n_threads) {
     if (!ctx) return NS_EINVAL;
     const int nt = (!ctx->tables->have_ref || ctx->tables->dref.all_iupac) ? unpack_threads() : 0;
@@ -1594,6 +1691,7 @@ int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_
     if (!read_slots || !new_reads || !new_pieces || (n_new_ops && !new_ops)) return fail(ctx, NS_EINVAL, "ns_reemit: null argument");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
+    ctx->have_z = false;
     NsBatchInfo& bi = ctx->last;
     const uint32_t old_np = bi.n_pieces;
     const uint64_t old_ops = bi.n_ops;

@@ -44,6 +44,7 @@ class Engine:
         self._keep = {}
         self.fastq = False
         self.info = None
+        self._z_bytes = 0
 
     def clone(self):
         """A context that shares this engine's reference + model in HBM (own stream and batch buffers)."""
@@ -52,6 +53,7 @@ class Engine:
         other._ctx = C.c_void_p()
         self._check(self._lib.ns_clone(self._ctx, C.byref(other._ctx)))
         other.device, other._keep, other.fastq, other.info = self.device, {}, self.fastq, None
+        other._z_bytes = 0
         other._parent = self            # keep the parent alive
         for k in ("ref", "tables"):
             if hasattr(self, k):
@@ -242,6 +244,27 @@ class Engine:
         def vp(x):
             return C.c_void_p(int(x)) if x else None
         self._check(self._lib.ns_fetch(self._ctx, vp(seq_ptr), vp(qual_ptr), vp(reads_ptr), vp(pieces_ptr), vp(ops_ptr)))
+
+    def compress_records(self, names):
+        """The last batch's FASTA/FASTQ records (read ``names``: a records.NameTable or a list of str) as BGZF members,
+        built on the device and kept there (ns_compress_records).  Returns their size in bytes; no end-of-file block."""
+        from .records import _name_blob
+        blob, offs = _name_blob(names)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        if len(offs) != int(self.info.n_reads):
+            raise ValueError("compress_records: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
+        n = C.c_uint64()
+        self._check(self._lib.ns_compress_records(self._ctx, blob, _ptr(offs), C.byref(n)))
+        self._z_bytes = int(n.value)
+        return self._z_bytes
+
+    def fetch_compressed(self, out=None):
+        """The members of the last compress_records() -> uint8 array (into ``out`` when given: a uint8 array, pinned
+        memory recommended, at least that large)."""
+        if out is None:
+            out = np.empty(self._z_bytes, dtype=np.uint8)
+        self._check(self._lib.ns_fetch_compressed(self._ctx, _ptr(out), C.c_uint64(len(out))))
+        return out[:self._z_bytes]
 
     def device_buffers(self):
         ps = [C.c_void_p() for _ in range(5)]

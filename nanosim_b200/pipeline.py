@@ -23,7 +23,7 @@ class _HostBuffers:
 
     def __init__(self, fastq):
         self.fastq = fastq
-        self.cap = {"seq": 0, "qual": 0, "reads": 0, "pieces": 0, "ops": 0}
+        self.cap = {"seq": 0, "qual": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0}
         self.t = {}
 
     def _alloc(self, nbytes):
@@ -49,12 +49,17 @@ class _HostBuffers:
 
 
 class BatchPipeline:
-    def __init__(self, engine, depth=2, fetch=True, want_ops=False, want_pieces=True):
+    """compress: None, or names(batch, job) -> the batch's read names (records.NameTable).  With it the pipeline runs in
+    compressed mode: the worker fetches the read and piece metadata (and the bases and ops when want_ops, for the error
+    profile; never the qualities), builds the names, compresses the records on the device (ns_compress_records) and fetches
+    the BGZF members into pinned memory; the consumer gets them as ``batch.gz`` and the names as ``batch.names``."""
+
+    def __init__(self, engine, depth=2, fetch=True, want_ops=False, want_pieces=True, compress=None):
         self.engines = [engine] + [engine.clone() for _ in range(max(1, depth) - 1)]
         self.depth = len(self.engines)
-        self.fetch, self.want_ops, self.want_pieces = fetch, want_ops, want_pieces
+        self.fetch, self.want_ops, self.want_pieces, self.compress = fetch, want_ops, want_pieces, compress
         self.bufs = [_HostBuffers(engine.fastq) for _ in self.engines]
-        self.hint = {"seq": 0, "reads": 0, "pieces": 0, "ops": 0}     # largest batch seen by any slot (pinned allocs are slow)
+        self.hint = {"seq": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0}     # largest batch seen by any slot (pinned allocs are slow)
 
     def close(self):
         for e in self.engines[1:]:
@@ -65,6 +70,8 @@ class BatchPipeline:
         return self.engines[slot].simulate(kind, first, n)
 
     def _fetch(self, slot, job, info):
+        if self.compress is not None:
+            return self._fetch_compressed(slot, job, info)
         kind, first, n = job
         eng, hb = self.engines[slot], self.bufs[slot]
         fastq = eng.fastq
@@ -85,6 +92,32 @@ class BatchPipeline:
                        hb.ptr("pieces") if pieces is not None else None, hb.ptr("ops") if ops is not None else None)
         return Batch(info, seq, qual, reads.view(L.READ_DTYPE), pieces.view(L.PIECE_DTYPE) if pieces is not None else None,
                      ops.view(np.uint32) if ops is not None else np.zeros(0, dtype=np.uint32) if self.want_ops else None, kind, first)
+
+    def _fetch_compressed(self, slot, job, info):
+        kind, first, n = job
+        eng, hb = self.engines[slot], self.bufs[slot]
+        nb = {"seq": int(info.seq_bytes), "reads": int(info.n_reads) * L.READ_DTYPE.itemsize,
+              "pieces": int(info.n_pieces) * L.PIECE_DTYPE.itemsize, "ops": int(info.n_ops) * 4}
+        for k, v in nb.items():
+            if v > self.hint[k]:
+                self.hint[k] = v
+        reads = hb.ensure("reads", nb["reads"], self.hint["reads"])[:nb["reads"]]
+        pieces = hb.ensure("pieces", nb["pieces"], self.hint["pieces"])[:nb["pieces"]]
+        seq = ops = None
+        if self.want_ops:                  # the error-profile formatter reads bases back from the sequence
+            seq = hb.ensure("seq", nb["seq"], self.hint["seq"])[:nb["seq"]]
+            if info.n_ops:
+                ops = hb.ensure("ops", nb["ops"], self.hint["ops"])[:nb["ops"]]
+        eng.fetch_into(hb.ptr("seq") if seq is not None else None, None, hb.ptr("reads"), hb.ptr("pieces"),
+                       hb.ptr("ops") if ops is not None else None)
+        b = Batch(info, seq, None, reads.view(L.READ_DTYPE), pieces.view(L.PIECE_DTYPE),
+                  ops.view(np.uint32) if ops is not None else np.zeros(0, dtype=np.uint32) if self.want_ops else None, kind, first)
+        b.names = self.compress(b, job)
+        nz = eng.compress_records(b.names)
+        if nz > self.hint["gz"]:
+            self.hint["gz"] = nz
+        b.gz = eng.fetch_compressed(hb.ensure("gz", max(nz, 1), self.hint["gz"]))
+        return b
 
     def warm(self, jobs):
         """Runs every job once on EVERY context (results discarded) so that device and pinned buffers reach their

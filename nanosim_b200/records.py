@@ -142,10 +142,12 @@ def name_table(batch, ref_names, index_base, perfect=False, metagenome=False, tr
     """read_names() through the library (ns_format_names): same strings, no per-read Python."""
     lib = L.lib()
     key = id(ref_names)
-    if key not in _CHROM_CACHE or _CHROM_CACHE[key][0] is not ref_names:
+    entry = _CHROM_CACHE.get(key)          # one lookup: pipeline workers call this concurrently
+    if entry is None or entry[0] is not ref_names:
+        entry = (ref_names,) + _name_blob(ref_names)
         _CHROM_CACHE.clear()
-        _CHROM_CACHE[key] = (ref_names,) + _name_blob(ref_names)
-    _, cblob, coffs = _CHROM_CACHE[key]
+        _CHROM_CACHE[key] = entry
+    _, cblob, coffs = entry
     reads = np.ascontiguousarray(batch.reads)
     pieces = np.ascontiguousarray(batch.pieces)
     flags = (1 if perfect else 0) | (2 if metagenome else 0) | (4 if transcriptome else 0)

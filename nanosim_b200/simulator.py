@@ -30,6 +30,9 @@ from .model import build_alias
 
 VERSION = "3.2.2-b200"
 
+# BGZF end-of-file marker: an empty member (SAM/BAM format specification §4.1.2), once at the end of every .gz file
+BGZF_EOF = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")
+
 
 def _log(msg):
     sys.stdout.write(strftime("%Y-%m-%d %H:%M:%S") + ": " + msg + "\n")
@@ -232,7 +235,9 @@ def _shard(n, rank, world):
 
 def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min_l, num_threads, fastq,
                median_l=None, sd_l=None, model_ir=False, uracil=False, polya=None, chimeric=False,
-               batch_reads=65536, error_profile=True, rank=0, world=1):
+               batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False):
+    """gzip: write the reads as BGZF (``.gz``), compressed on the GPU; the error profile stays plain text.  Under torchrun
+    (world > 1) the per-rank files carry no end-of-file block: merge_rank_files appends it."""
     fmt_threads = max(1, min(num_threads, os.cpu_count() or 1))     # host threads of the record formatter
     eng = prof.engine
     meta = mode == "metagenome"
@@ -245,21 +250,37 @@ def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min
                   # the reference's 2-D KDE sample has one row per read of a WORKER (:1072): -t sets its size as it does there
                   kde2d_sample=max(1, (hi_a - lo_a) // max(1, num_threads)),
                   trx_records=prof.n_trx if (trx and prof.ir is not None) else 0)
-    ext = ".fastq" if fastq else ".fasta"
+    ext = (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
     suffix = "" if world == 1 else str(rank)
     want_err = error_profile and not per
     pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err)
     totals = {"reads": 0, "bases": 0, "bytes": 0}
     try:
-        _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals)
+        _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
+                         gzip)
     finally:
         pipe.close()         # the cloned contexts own device batch buffers and pinned staging
     return totals            # what this rank simulated and wrote (the reference returns nothing)
 
 
-def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals):
+def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
+                     gzip=False):
     def jobs(kind, lo, hi):
         return [(kind, start, min(batch_reads, hi - start)) for start in range(lo, hi, batch_reads)]
+
+    def put_reads(f, b, names):
+        if not gzip:
+            f.pos += write_records(f.fd, f.pos, b, names, fastq, n_threads=fmt_threads)
+            return
+        view = memoryview(b.gz)
+        while len(view):
+            w = os.pwrite(f.fd, view, f.pos)
+            f.pos += w
+            view = view[w:]
+
+    def end_reads(f):
+        if gzip and world == 1:
+            f.pos += os.pwrite(f.fd, BGZF_EOF, f.pos)
 
     class _Out:
         """An output file written at explicit offsets: the library's formatter threads pwrite() into it."""
@@ -279,9 +300,12 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
     f_err = _Out(out + ("_aligned_error_profile" if world == 1 else "_error_profile" + suffix),
                  b"Seq_name\tSeq_pos\terror_type\terror_length\tref_base\tseq_base\n" if world == 1 else b"")
     try:
+        def aligned_names(b, job):
+            return name_table(b, prof.ref.names, job[1], perfect=per, metagenome=meta, transcriptome=trx)
+
         def sink_aligned(info, b, job):
-            names = name_table(b, prof.ref.names, job[1], perfect=per, metagenome=meta, transcriptome=trx)
-            f_reads.pos += write_records(f_reads.fd, f_reads.pos, b, names, fastq, n_threads=fmt_threads)
+            names = b.names if gzip else aligned_names(b, job)
+            put_reads(f_reads, b, names)
             totals["reads"] += int(info.n_reads)
             totals["bases"] += int(info.total_bases)
             if want_err:
@@ -295,8 +319,10 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             if patch is not None:
                 engine.reemit(*patch)
 
+        pipe.compress = aligned_names if gzip else None
         pipe.run(jobs(L.NS_KIND_ALIGNED, lo, hi), sink_aligned, static_assign=meta,
                  after_simulate=retain_introns if (trx and prof.ir is not None and not per) else None)
+        end_reads(f_reads)
     finally:
         totals["bytes"] += f_reads.pos + f_err.pos
         f_reads.close()
@@ -307,27 +333,33 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
         pipe.want_ops = False                              # unaligned reads are not logged (:1482-1549)
         f_un = _Out(out + "_unaligned_reads" + suffix + ext)
         try:
-            def sink_unaligned(info, b, job):
+            def unaligned_names(b, job):
                 # the reference's read index keeps counting after the aligned reads (shared total_simulated, :1574)
-                names = name_table(b, prof.ref.names, prof.number_aligned + job[1])
-                f_un.pos += write_records(f_un.fd, f_un.pos, b, names, fastq, n_threads=fmt_threads)
+                return name_table(b, prof.ref.names, prof.number_aligned + job[1])
+
+            def sink_unaligned(info, b, job):
+                put_reads(f_un, b, b.names if gzip else unaligned_names(b, job))
                 totals["reads"] += int(info.n_reads)
                 totals["bases"] += int(info.total_bases)
 
+            pipe.compress = unaligned_names if gzip else None
             pipe.run(jobs(L.NS_KIND_UNALIGNED, lo, hi), sink_unaligned, static_assign=meta)
+            end_reads(f_un)
         finally:
             totals["bytes"] += f_un.pos
             f_un.close()
 
 
-def merge_rank_files(out, fastq, per, world):
-    """Rank 0: concatenate per-rank sub-files in rank order and delete them (:1626-1639, :1667-1672)."""
-    ext = ".fastq" if fastq else ".fasta"
-    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, None)]
-    jobs.append(("_error_profile%d", "_aligned_error_profile", "Seq_name\tSeq_pos\terror_type\terror_length\tref_base\tseq_base\n"))
+def merge_rank_files(out, fastq, per, world, gzip=False):
+    """Rank 0: concatenate per-rank sub-files in rank order and delete them (:1626-1639, :1667-1672).  gzip: the reads
+    files are BGZF members without an end-of-file block; the merged file gets it once, at its end."""
+    ext = (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
+    trailer = BGZF_EOF if gzip else b""
+    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, None, trailer)]
+    jobs.append(("_error_profile%d", "_aligned_error_profile", "Seq_name\tSeq_pos\terror_type\terror_length\tref_base\tseq_base\n", b""))
     if not per:
-        jobs.append(("_unaligned_reads%d" + ext, "_unaligned_reads" + ext, None))
-    for pat, dst, header in jobs:
+        jobs.append(("_unaligned_reads%d" + ext, "_unaligned_reads" + ext, None, trailer))
+    for pat, dst, header, end in jobs:
         with open(out + dst, "wb") as o:
             if header:
                 o.write(header.encode())
@@ -340,6 +372,12 @@ def merge_rank_files(out, fastq, per, world):
                             break
                         o.write(blk)
                 os.remove(p)
+            o.write(end)
+
+
+GZIP_HELP = ('Write the reads as BGZF-compressed <out>_aligned_reads.fast{a,q}.gz and <out>_unaligned_reads.fast{a,q}.gz, '
+             'compressed on the GPU (gzip, zcat and samtools read them). The error profile is still written as plain '
+             'text (Default = False)')
 
 
 def build_parser():
@@ -385,6 +423,7 @@ def build_parser():
     g.add_argument('--batch_reads', help='Reads simulated per GPU batch (Default = 65536)', type=int, default=65536)
     g.add_argument('--no_error_profile', help='Skip writing <out>_aligned_error_profile', action='store_true', default=False)
     g.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
+    g.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     mg = sub.add_parser('metagenome', help="Run the simulator on metagenome mode")
     mg.add_argument('-gl', '--genome_list', help="Reference metagenome list, tsv file, the first column is species/strain "
                     "name, the second column is the reference genome fasta/fastq file directory", required=True)
@@ -417,6 +456,7 @@ def build_parser():
     mg.add_argument('--batch_reads', help='Reads simulated per GPU batch (Default = 65536)', type=int, default=65536)
     mg.add_argument('--no_error_profile', help='Skip writing <out>_aligned_error_profile', action='store_true', default=False)
     mg.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
+    mg.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     t = sub.add_parser('transcriptome', help="Run the simulator on transcriptome mode")
     t.add_argument('-rt', '--ref_t', help='Input reference transcriptome', required=True)
     t.add_argument('-rg', '--ref_g', help='Input reference genome, required if intron retention simulation is on', default='')
@@ -455,6 +495,7 @@ def build_parser():
     t.add_argument('--batch_reads', help='Reads simulated per GPU batch (Default = 65536)', type=int, default=65536)
     t.add_argument('--no_error_profile', help='Skip writing <out>_aligned_error_profile', action='store_true', default=False)
     t.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
+    t.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     return parser, g, mg, t
 
 
@@ -513,14 +554,15 @@ def main_transcriptome(args, parser_t):
     max_len = min(max_len, prof.max_chrom)
     simulation(prof, "transcriptome", args.output, "transcriptome", args.perfect, args.KmerBias if args.homopolymer else None,
                args.basecaller, max_len, min_len, max(args.num_threads, 1), args.fastq, None, None, model_ir, args.uracil,
-               args.polya, batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world)
+               args.polya, batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world,
+               gzip=args.gzip)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
             dist.init_process_group("gloo")
         dist.barrier()
         if rank == 0:
-            merge_rank_files(args.output, args.fastq, args.perfect, world)
+            merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip)
         dist.barrier()
     _log("Finished!")
 
@@ -578,14 +620,14 @@ def main_metagenome(args, parser_mg):
         prof.number_aligned, prof.number_unaligned = prof.counts[s_idx]
         simulation(prof, "metagenome", args.output + "_sample%d" % s_idx, "metagenome", args.perfect, None, None, max_len,
                    min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len, chimeric=args.chimeric,
-                   batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world)
+                   batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world, gzip=args.gzip)
         if world > 1:
             import torch.distributed as dist
             if not dist.is_initialized():
                 dist.init_process_group("gloo")
             dist.barrier()
             if rank == 0:
-                merge_rank_files(args.output + "_sample%d" % s_idx, args.fastq, args.perfect, world)
+                merge_rank_files(args.output + "_sample%d" % s_idx, args.fastq, args.perfect, world, gzip=args.gzip)
             dist.barrier()
     _log("Finished!")
 
@@ -657,14 +699,14 @@ def main(argv=None):
     simulation(prof, args.mode, args.output, args.dna_type, args.perfect, args.KmerBias if args.homopolymer else None,
                None, max_len, min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len,
                chimeric=args.chimeric, batch_reads=args.batch_reads, error_profile=not args.no_error_profile,
-               rank=rank, world=world)
+               rank=rank, world=world, gzip=args.gzip)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
             dist.init_process_group("gloo")
         dist.barrier()
         if rank == 0:
-            merge_rank_files(args.output, args.fastq, args.perfect, world)
+            merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip)
         dist.barrier()
     _log("Finished!")
 
