@@ -359,6 +359,16 @@ int64_t ns_write_error_profile(int fd, uint64_t file_off, const uint8_t* seq, co
 int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
 /* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' *nbytes. */
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap);
+/* The rows of <out>_aligned_error_profile for the last aligned batch (ns_format_error_profile's bytes, after ns_reemit as
+ * well; no header line) as BGZF, formatted and compressed on the device from the batch's reads, pieces, event scripts and
+ * sequence and the resident reference: 56 KiB blocks, one member each, in which every row's read name is sent as a
+ * back-reference to the row before it (the rule is in nanosim_b200/csrc/bgzf_kernel.cuh).  Same name layout as
+ * ns_compress_records; the seed is the context's.  The members stay in HBM in a buffer of their own (ns_compress_records
+ * before or after this call keeps its members) until the next ns_simulate / ns_reemit; *nbytes = their size, 0 for a
+ * batch without error events.  NS_EINVAL when the last batch is not aligned. */
+int ns_compress_error_profile(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
+/* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_error_profile's *nbytes. */
+int ns_fetch_compressed_error_profile(NsContext* ctx, uint8_t* out, uint64_t cap);
 
 /* Host-side read names of a fetched batch in the reference's formats (genome :1390-1402, metagenome :965-969,
  * transcriptome :1188-1219, perfect :1332-1343, unaligned :1511/:1529-1534), written as NUL-terminated strings back to

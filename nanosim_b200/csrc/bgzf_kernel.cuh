@@ -9,6 +9,21 @@
 // takes at most 9 * (BGZF_BLOCK + 1) bits = 64 513 bytes.  The header sends 259 code lengths with a code-length code
 // of at most 7 bits (no run-length symbols), 3 + 14 + 19 * 3 + 259 * 7 bits = 237 bytes, and the gzip framing is 26
 // bytes: 64 776 <= 65 536.  The kernel still checks every member and reports a violation (no stored-block fallback).
+//
+// Error-profile rows (bgzf_deflate_rows_kernel, ns_compress_error_profile): flat text in HBM, cut and framed the same way.
+// Every row starts with the read's name and a read has hundreds of rows, so each row's name is sent as a back-reference
+// to the row before it.  The rule, a pure function of the text and the block cut [b0, b1): take a row starting at s
+// whose previous row starts at p >= b0, and let f be the number of bytes before the row's first TAB.  If
+// text[p, p+f+1) == text[s, s+f+1) and s - p <= 32768, then text[s, min(s+f+1, b1)) is coded as back-references with
+// distance s - p when that span is at least 4 bytes long: pieces of 258 bytes, except that a piece shorter than 4 at the
+// end borrows from the one before it (bgzf_rows_piece).  Every other byte is a literal.  The literal/length alphabet has
+// 286 symbols and the distance alphabet 30; both codes are built with package-merge (limit 15), and a block with fewer
+// than two distance symbols gets a second one of length 1, as zlib does.
+// Size bound.  A complete code of at most 9 bits exists for 286 literal/length symbols and one of 5 bits for 30
+// distance codes; a match of 4 or more bytes then costs at most 9 + 5 + 5 + 13 = 32 bits, at most 8 bits per byte.  So
+// the optimal codes still spend at most 9 bits per text byte: at most 64 513 bytes of data per block.  The header sends
+// all 286 + 30 code lengths, at most (3 + 14 + 19 * 3 + 316 * 7) / 8 -> 286 bytes, and with the 26 bytes of framing a
+// member takes at most 64 825 <= 65 536 bytes.  Checked on the device like the records kernel.
 #pragma once
 #include <cub/block/block_scan.cuh>
 
@@ -104,8 +119,9 @@ __device__ __forceinline__ uint32_t bgzf_crc_combine(const uint32_t* x2n, uint32
 // Optimal code lengths under a length limit (package-merge) for n >= 2 weights sorted ascending; len[k] belongs to w[k].
 // Level 0 lists the leaves; level j merges the leaves with the pairs of level j-1's list.  The first 2n - 2 items of the
 // top level are the solution: every leaf among the first m items of a level gains one bit, and the packages among them
-// select the first 2 * packages items of the level below.
-__device__ void bgzf_package_merge(BgzfSmem& s, const uint32_t* w, int n, int limit, uint8_t* len) {
+// select the first 2 * packages items of the level below.  S: the kernel's shared-memory layout (its u.pm lists).
+template <class S>
+__device__ void bgzf_package_merge(S& s, const uint32_t* w, int n, int limit, uint8_t* len) {
     const int cap = 2 * n - 2;
     uint32_t* prev = s.u.pm.w[0];
     uint32_t* cur = s.u.pm.w[1];
@@ -368,6 +384,332 @@ __global__ void __launch_bounds__(BGZF_THREADS) bgzf_deflate_kernel(BgzfArgs a) 
                 fill -= 32;
             }
         }
+        if (fill > 0) atomicOr(out + w, (uint32_t)acc);
+    }
+    if (tid == 0) {
+        a.member_size[blockIdx.x] = payload + BGZF_FRAME;
+        a.trailer[blockIdx.x] = make_uint2(s.span_crc[0], blen);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// flat text of rows (the error profile) with one back-reference per row for the repeated read name; see the header
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int BGZF_LL_SYMS = 286;                   // literals, end-of-block, length codes 257..285
+constexpr int BGZF_D_SYMS = 30;                     // distance codes
+constexpr uint32_t BGZF_WINDOW = 32768u;
+
+struct BgzfRowsArgs {
+    const uint8_t* text;
+    uint64_t text_bytes;
+    uint8_t* stage;                 // BGZF_SLOT bytes per member: its DEFLATE data
+    uint64_t* member_size;          // BGZF_FRAME + DEFLATE bytes
+    uint2* trailer;                 // CRC32, ISIZE
+    unsigned long long* oversize;   // members above BGZF_MAX_MEMBER
+};
+
+// its own layout, sized for 286 symbols (the records kernel's BgzfSmem stays as it is)
+struct BgzfRowsSmem {
+    uint8_t text[BGZF_BLOCK];
+    union {
+        uint32_t hist[BGZF_THREADS / 32][BGZF_LL_SYMS];         // per-warp literal/length histograms
+        struct {
+            uint32_t w[2][2 * BGZF_LL_SYMS];
+            uint8_t pkg[15][2 * BGZF_LL_SYMS];
+        } pm;                                                   // package-merge lists
+    } u;
+    uint32_t crc_tab[256];
+    uint32_t x2n[32];
+    uint32_t span_crc[BGZF_THREADS];
+    uint32_t span_len[BGZF_THREADS];
+    uint32_t freq[BGZF_LL_SYMS];
+    uint32_t code[BGZF_LL_SYMS];
+    uint16_t sorted[BGZF_LL_SYMS];
+    uint8_t len[BGZF_LL_SYMS];
+    uint8_t len_sorted[BGZF_LL_SYMS];
+    uint32_t dfreq[BGZF_D_SYMS];
+    uint32_t dcode[BGZF_D_SYMS];
+    uint8_t dlen[BGZF_D_SYMS];
+    uint32_t cl_code[19];
+    uint8_t cl_len[19];
+    uint32_t hclen;
+    uint32_t hdr_bits;
+    typename cub::BlockScan<uint32_t, BGZF_THREADS>::TempStorage scan;
+};
+
+// length symbol (RFC 1951 §3.2.5) of a match of 3..258 bytes: symbol, extra bits, their value
+__device__ __forceinline__ uint3 bgzf_len_sym(uint32_t n) {
+    if (n == 258) return make_uint3(285, 0, 0);
+    const uint32_t v = n - 3;
+    if (v < 8) return make_uint3(257 + v, 0, 0);
+    const uint32_t e = 29 - __clz(v);                          // floor(log2 v) - 2
+    return make_uint3(261 + 4 * e + ((v >> e) & 3u), e, v & ((1u << e) - 1));
+}
+// distance symbol of a distance of 1..32768
+__device__ __forceinline__ uint3 bgzf_dist_sym(uint32_t d) {
+    const uint32_t v = d - 1;
+    if (v < 4) return make_uint3(v, 0, 0);
+    const uint32_t e = 30 - __clz(v);                          // floor(log2 v) - 1
+    return make_uint3(2 * e + 2 + ((v >> e) & 1u), e, v & ((1u << e) - 1));
+}
+// the next piece of a back-reference with `rem` >= 4 bytes left: 258 bytes, or fewer so that at least 4 remain
+__device__ __forceinline__ uint32_t bgzf_rows_piece(uint32_t rem) { return rem <= 258 ? rem : (rem - 258 < 4 ? rem - 4 : 258); }
+
+// where thread t's tokens start: the first row start at or after its byte span (thread 0: the block's first byte).  A
+// back-reference never crosses a row, so every thread codes its rows on its own.
+__device__ __forceinline__ uint32_t bgzf_rows_cut(const BgzfRowsSmem& s, uint32_t t, uint32_t span, uint32_t blen) {
+    if (t == 0) return 0;
+    uint32_t k = min(t * span, blen);
+    while (k < blen && s.text[k - 1] != '\n') ++k;
+    return k;
+}
+
+// The back-reference of the row starting at block offset k (k >= 1, text[k-1] == '\n'): (length, distance), length 0
+// when there is none.  g: the text at the block's start (the row's name may run past the block); left: text bytes from
+// there; row0: the block starts with a row.
+__device__ uint2 bgzf_row_match(const BgzfRowsSmem& s, const uint8_t* __restrict__ g, uint32_t k, uint32_t blen, uint64_t left,
+                                bool row0) {
+    uint32_t p = k - 1;                                         // the previous row's start
+    while (p > 0 && s.text[p - 1] != '\n') --p;
+    if ((p == 0 && !row0) || k - p > BGZF_WINDOW) return make_uint2(0, 0);
+    uint32_t f = 0;                                             // bytes before the row's first TAB
+    for (;; ++f) {
+        if (k + f >= left) return make_uint2(0, 0);
+        const uint8_t c = k + f < blen ? s.text[k + f] : g[k + f];
+        if (c == '\t') break;
+        if (c == '\n') return make_uint2(0, 0);
+    }
+    for (uint32_t t = 0; t <= f; ++t)                           // p + t < k <= blen: the previous row is in shared memory
+        if (s.text[p + t] != (k + t < blen ? s.text[k + t] : g[k + t])) return make_uint2(0, 0);
+    const uint32_t m = min(f + 1, blen - k);
+    return m >= 4 ? make_uint2(m, k - p) : make_uint2(0, 0);
+}
+
+// the tokens of [lo, hi): fn(c, 0, 0) for a literal byte c, fn(0, n, d) for a back-reference piece of n bytes, distance d
+template <class Fn>
+__device__ __forceinline__ void bgzf_rows_tokens(const BgzfRowsSmem& s, const uint8_t* __restrict__ g, uint32_t lo, uint32_t hi,
+                                                 uint32_t blen, uint64_t left, bool row0, Fn fn) {
+    for (uint32_t k = lo; k < hi;) {
+        if (k > 0 && s.text[k - 1] == '\n') {
+            const uint2 m = bgzf_row_match(s, g, k, blen, left, row0);
+            if (m.x) {
+                for (uint32_t rem = m.x; rem;) {
+                    const uint32_t n = bgzf_rows_piece(rem);
+                    fn(0u, n, m.y);
+                    rem -= n;
+                }
+                k += m.x;
+                continue;
+            }
+        }
+        fn((uint32_t)s.text[k], 0u, 0u);
+        ++k;
+    }
+}
+
+__global__ void __launch_bounds__(BGZF_THREADS) bgzf_deflate_rows_kernel(BgzfRowsArgs a) {
+    extern __shared__ __align__(16) unsigned char bgzf_rows_smem_raw[];
+    BgzfRowsSmem& s = *reinterpret_cast<BgzfRowsSmem*>(bgzf_rows_smem_raw);
+    const uint32_t tid = threadIdx.x, warp = tid >> 5;
+    const uint64_t t0 = (uint64_t)blockIdx.x * BGZF_BLOCK;
+    const uint32_t blen = (uint32_t)min((uint64_t)BGZF_BLOCK, a.text_bytes - t0);
+    const uint32_t span = (blen + BGZF_THREADS - 1) / BGZF_THREADS;
+    const uint32_t lo = min(tid * span, blen), hi = min(lo + span, blen);
+    const uint8_t* g = a.text + t0;
+    const uint64_t left = a.text_bytes - t0;
+    const bool row0 = t0 == 0 || a.text[t0 - 1] == '\n';
+
+    if (tid < 256) {
+        uint32_t c = tid;
+        for (int k = 0; k < 8; ++k) c = (c & 1) ? (c >> 1) ^ BGZF_CRC_POLY : c >> 1;
+        s.crc_tab[tid] = c;
+    }
+    if (tid == 0) {
+        uint32_t p = 1u << 30;                                  // x^1
+        s.x2n[0] = p;
+        for (int k = 1; k < 32; ++k) s.x2n[k] = p = bgzf_multmodp(p, p);
+    }
+    for (uint32_t k = tid; k < (BGZF_THREADS / 32) * BGZF_LL_SYMS; k += BGZF_THREADS) (&s.u.hist[0][0])[k] = 0;
+    if (tid < BGZF_D_SYMS) s.dfreq[tid] = 0;
+    for (uint32_t k = tid; k < blen; k += BGZF_THREADS) s.text[k] = g[k];
+    __syncthreads();
+
+    // CRC of the byte span; symbols of the rows this thread codes
+    uint32_t crc = 0xffffffffu;
+    for (uint32_t k = lo; k < hi; ++k) crc = s.crc_tab[(crc ^ s.text[k]) & 0xffu] ^ (crc >> 8);
+    s.span_crc[tid] = lo < hi ? ~crc : 0u;
+    s.span_len[tid] = hi - lo;
+    const uint32_t tlo = bgzf_rows_cut(s, tid, span, blen), thi = bgzf_rows_cut(s, tid + 1, span, blen);
+    bgzf_rows_tokens(s, g, tlo, thi, blen, left, row0, [&](uint32_t c, uint32_t n, uint32_t d) {
+        if (n == 0) {
+            atomicAdd(&s.u.hist[warp][c], 1u);
+        } else {
+            atomicAdd(&s.u.hist[warp][bgzf_len_sym(n).x], 1u);
+            atomicAdd(&s.dfreq[bgzf_dist_sym(d).x], 1u);
+        }
+    });
+    __syncthreads();
+    for (uint32_t d = 1; d < BGZF_THREADS; d <<= 1) {
+        if ((tid & (2 * d - 1)) == 0 && s.span_len[tid + d])
+            s.span_crc[tid] = bgzf_crc_combine(s.x2n, s.span_crc[tid], s.span_crc[tid + d], s.span_len[tid + d]);
+        __syncthreads();
+        if ((tid & (2 * d - 1)) == 0) s.span_len[tid] += s.span_len[tid + d];
+        __syncthreads();
+    }
+    if (tid < BGZF_LL_SYMS) {
+        uint32_t f = 0;
+        for (int w = 0; w < BGZF_THREADS / 32; ++w) f += s.u.hist[w][tid];
+        s.freq[tid] = tid == 256 ? 1u : f;                      // end-of-block
+    }
+    __syncthreads();
+
+    // literal/length symbols in use, ascending by (frequency, symbol)
+    if (tid < BGZF_LL_SYMS && s.freq[tid]) {
+        const uint32_t f = s.freq[tid];
+        uint32_t rank = 0;
+        for (int t = 0; t < BGZF_LL_SYMS; ++t) {
+            const uint32_t g2 = s.freq[t];
+            rank += (g2 && (g2 < f || (g2 == f && t < (int)tid))) ? 1u : 0u;
+        }
+        s.sorted[rank] = (uint16_t)tid;
+    }
+    const int n_used = __syncthreads_count(tid < BGZF_LL_SYMS && s.freq[tid] != 0);
+
+    if (tid == 0) {
+        // literal/length code (the histograms and the span lengths are dead: their space holds the lists and the weights)
+        uint32_t* w = s.span_len;
+        for (int k = 0; k < n_used; ++k) w[k] = s.freq[s.sorted[k]];
+        bgzf_package_merge(s, w, n_used, 15, s.len_sorted);
+        for (int k = 0; k < BGZF_LL_SYMS; ++k) s.len[k] = 0;
+        for (int k = 0; k < n_used; ++k) s.len[s.sorted[k]] = s.len_sorted[k];
+        bgzf_canonical(s.len, BGZF_LL_SYMS, s.code);
+        // distance code: the used symbols by (frequency, symbol); fewer than two get a second symbol of length 1
+        uint8_t dsym[BGZF_D_SYMS], dlen_sorted[BGZF_D_SYMS];
+        int nd = 0;
+        for (int v = 0; v < BGZF_D_SYMS; ++v) {
+            s.dlen[v] = 0;
+            if (s.dfreq[v]) {
+                int at = nd++;
+                while (at > 0 && (w[at - 1] > s.dfreq[v])) {
+                    w[at] = w[at - 1];
+                    dsym[at] = dsym[at - 1];
+                    --at;
+                }
+                w[at] = s.dfreq[v];
+                dsym[at] = (uint8_t)v;
+            }
+        }
+        if (nd >= 2) {
+            bgzf_package_merge(s, w, nd, 15, dlen_sorted);
+            for (int k = 0; k < nd; ++k) s.dlen[dsym[k]] = dlen_sorted[k];
+        } else {
+            const int c = nd ? dsym[0] : 0;
+            s.dlen[c] = 1;
+            s.dlen[c == 0 ? 1 : 0] = 1;
+        }
+        bgzf_canonical(s.dlen, BGZF_D_SYMS, s.dcode);
+        // code-length code over the 286 literal/length and the 30 distance code lengths, limit 7
+        uint32_t clf[16] = {0};
+        for (int k = 0; k < BGZF_LL_SYMS; ++k) ++clf[s.len[k]];
+        for (int k = 0; k < BGZF_D_SYMS; ++k) ++clf[s.dlen[k]];
+        uint8_t cl_sym[16], cl_len_sorted[16];
+        uint32_t cl_w[16];
+        uint8_t* cl_len = s.cl_len;
+        for (int k = 0; k < 19; ++k) cl_len[k] = 0;
+        int nc = 0;
+        for (int v = 0; v < 16; ++v)
+            if (clf[v]) {
+                int at = nc++;
+                while (at > 0 && cl_w[at - 1] > clf[v]) {
+                    cl_w[at] = cl_w[at - 1];
+                    cl_sym[at] = cl_sym[at - 1];
+                    --at;
+                }
+                cl_w[at] = clf[v];
+                cl_sym[at] = (uint8_t)v;
+            }
+        bgzf_package_merge(s, cl_w, nc, 7, cl_len_sorted);
+        for (int k = 0; k < nc; ++k) cl_len[cl_sym[k]] = cl_len_sorted[k];
+        bgzf_canonical(cl_len, 19, s.cl_code);
+        int hclen = 19;
+        while (hclen > 4 && cl_len[kBgzfClOrder[hclen - 1]] == 0) --hclen;
+        s.hclen = (uint32_t)hclen;
+        uint32_t bits = 3 + 5 + 5 + 4 + 3 * hclen;
+        for (int k = 0; k < BGZF_LL_SYMS; ++k) bits += cl_len[s.len[k]];
+        for (int k = 0; k < BGZF_D_SYMS; ++k) bits += cl_len[s.dlen[k]];
+        s.hdr_bits = bits;
+    }
+    __syncthreads();
+
+    // bit count of this thread's tokens, then their offset behind the header
+    uint32_t nbits = 0;
+    bgzf_rows_tokens(s, g, tlo, thi, blen, left, row0, [&](uint32_t c, uint32_t n, uint32_t d) {
+        if (n == 0) {
+            nbits += s.len[c];
+        } else {
+            const uint3 l = bgzf_len_sym(n), q = bgzf_dist_sym(d);
+            nbits += s.len[l.x] + l.y + s.dlen[q.x] + q.y;
+        }
+    });
+    uint32_t off = 0, data_bits = 0;
+    cub::BlockScan<uint32_t, BGZF_THREADS>(s.scan).ExclusiveSum(nbits, off, data_bits);
+    const uint64_t total_bits = (uint64_t)s.hdr_bits + data_bits + s.len[256];
+    const uint32_t payload = (uint32_t)((total_bits + 7) / 8);
+    uint32_t* out = reinterpret_cast<uint32_t*>(a.stage + (uint64_t)blockIdx.x * BGZF_SLOT);
+    const uint32_t n_words = min((uint32_t)((total_bits + 31) / 32), BGZF_SLOT / 4);
+    for (uint32_t k = tid; k < n_words; k += BGZF_THREADS) out[k] = 0;
+    __syncthreads();
+    if (payload + BGZF_FRAME > BGZF_MAX_MEMBER) {              // cannot happen (see the bound above); reported, not written
+        if (tid == 0) {
+            atomicAdd(a.oversize, 1ull);
+            a.member_size[blockIdx.x] = 0;
+            a.trailer[blockIdx.x] = make_uint2(0, 0);
+        }
+        return;
+    }
+
+    if (tid == 0) {
+        uint64_t pos = 0;
+        bgzf_or_bits(out, pos, 1u, 1);                          // BFINAL
+        bgzf_or_bits(out, pos, 2u, 2);                          // BTYPE: dynamic Huffman
+        bgzf_or_bits(out, pos, BGZF_LL_SYMS - 257, 5);          // HLIT: 286 literal/length codes
+        bgzf_or_bits(out, pos, BGZF_D_SYMS - 1, 5);             // HDIST: 30 distance codes
+        bgzf_or_bits(out, pos, s.hclen - 4, 4);
+        for (uint32_t k = 0; k < s.hclen; ++k) bgzf_or_bits(out, pos, s.cl_len[kBgzfClOrder[k]], 3);
+        for (int k = 0; k < BGZF_LL_SYMS; ++k) bgzf_or_bits(out, pos, s.cl_code[s.len[k]], s.cl_len[s.len[k]]);
+        for (int k = 0; k < BGZF_D_SYMS; ++k) bgzf_or_bits(out, pos, s.cl_code[s.dlen[k]], s.cl_len[s.dlen[k]]);
+    }
+
+    // this thread's codes: words wholly inside its stretch are stored, the two it shares with its neighbours are OR-ed
+    {
+        const uint64_t start = (uint64_t)s.hdr_bits + off;
+        uint64_t acc = 0;
+        uint32_t fill = (uint32_t)(start & 31), w = (uint32_t)(start >> 5);
+        bool first = (start & 31) != 0;
+        auto put = [&](uint32_t v, uint32_t nb) {              // nb <= 15: one word completes at most
+            acc |= (uint64_t)v << fill;
+            fill += nb;
+            if (fill >= 32) {
+                if (first) atomicOr(out + w, (uint32_t)acc);
+                else out[w] = (uint32_t)acc;
+                first = false;
+                ++w;
+                acc >>= 32;
+                fill -= 32;
+            }
+        };
+        bgzf_rows_tokens(s, g, tlo, thi, blen, left, row0, [&](uint32_t c, uint32_t n, uint32_t d) {
+            if (n == 0) {
+                put(s.code[c], s.len[c]);
+            } else {
+                const uint3 l = bgzf_len_sym(n), q = bgzf_dist_sym(d);
+                put(s.code[l.x], s.len[l.x]);
+                if (l.y) put(l.z, l.y);
+                put(s.dcode[q.x], s.dlen[q.x]);
+                if (q.y) put(q.z, q.y);
+            }
+        });
+        if (tid == BGZF_THREADS - 1) put(s.code[256], s.len[256]);     // end-of-block closes the stream
         if (fill > 0) atomicOr(out + w, (uint32_t)acc);
     }
     if (tid == 0) {

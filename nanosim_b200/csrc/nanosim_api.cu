@@ -28,6 +28,7 @@
 #include "uread_kernel.cuh"
 #include "hp_kernel.cuh"
 #include "bgzf_kernel.cuh"
+#include "errprof_kernel.cuh"
 #include "host_io.h"
 
 namespace {
@@ -159,6 +160,11 @@ struct NsContext {
     DevBuf z_names, z_name_off, z_name_len, z_rec_off, z_stage, z_msize, z_moff, z_trailer, z_out;
     uint64_t z_bytes = 0;
     bool have_z = false;
+    // ns_compress_error_profile: the rows of the last aligned batch and their BGZF members (ep_bytes of ep_out; valid while
+    // have_ep).  Names, layout and staging are the z_ buffers above: only the members outlive a call.
+    DevBuf ep_text, ep_out;
+    uint64_t ep_bytes = 0;
+    bool have_ep = false;
     // Batches of one job have near-identical sizes: once a batch of a kind has run with host-sized buffers, the next ones
     // are submitted in one go (no host round trip between the first and the last kernel) against those capacities; a
     // kernel checks them on the device and a batch that does not fit is simply run again the sized way.
@@ -1142,6 +1148,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     cudaStream_t st = ctx->stream;
     ctx->have_batch = false;
     ctx->have_z = false;
+    ctx->have_ep = false;
     memset(&ctx->last, 0, sizeof ctx->last);
     if (n_reads == 0) {
         if (info) *info = ctx->last;
@@ -1499,12 +1506,67 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
 #define NS_T_Z_BYTES 13
 #define NS_T_Z_OVERSIZE 14
 
+// the n names (ns_format_records' layout) into z_names / z_name_off; room for the names' lengths, the per-read sizes
+// (scan_in) and their offsets (z_rec_off); the totals slots of a compression zeroed
+static int upload_names(NsContext* ctx, const char* names, const uint64_t* name_off, uint32_t n) {
+    cudaStream_t st = ctx->stream;
+    uint64_t blob = 0;                      // the names' extent: every name with its NUL
+    for (uint32_t i = 0; i < n; ++i) blob = std::max<uint64_t>(blob, name_off[i] + strlen(names + name_off[i]) + 1);
+    CK(upload(ctx->z_names, names, blob, st));
+    CK(upload(ctx->z_name_off, name_off, (size_t)n * sizeof(uint64_t), st));
+    CK(ctx->z_name_len.ensure((size_t)n * sizeof(uint32_t)));
+    CK(ctx->z_rec_off.ensure((size_t)n * sizeof(uint64_t)));
+    CK(ctx->scan_in.ensure((size_t)n * sizeof(uint64_t)));
+    CK(cudaMemsetAsync(ctx->totals.as<uint64_t>() + NS_T_Z_TEXT, 0, 3 * sizeof(uint64_t), st));
+    return NS_OK;
+}
+
+// the last of a compression's steps: member offsets, their total (second host round trip), the members packed into `out`
+static int pack_members(NsContext* ctx, const char* fname, uint32_t n_blocks, DevBuf& out, uint64_t* total) {
+    if (int rc = scan_total(ctx, ctx->z_msize.as<uint64_t>(), ctx->z_moff.as<uint64_t>(), n_blocks, NS_T_Z_BYTES)) return rc;
+    if (int rc = publish_totals_and_wait(ctx)) return rc;
+    const uint64_t* h = ctx->h_totals.as<uint64_t>();
+    if (h[NS_T_Z_OVERSIZE])
+        return fail(ctx, NS_ESTATE, "%s: %llu BGZF members exceed %u bytes", fname, (unsigned long long)h[NS_T_Z_OVERSIZE],
+                    BGZF_MAX_MEMBER);
+    *total = h[NS_T_Z_BYTES];
+    CK(out.ensure((size_t)*total));
+    CK(launch(ctx, bgzf_pack_kernel, n_blocks, 256, 0, (const uint8_t*)ctx->z_stage.p, (const uint64_t*)ctx->z_msize.p,
+              (const uint64_t*)ctx->z_moff.p, (const uint2*)ctx->z_trailer.p, out.as<uint8_t>()));
+    CK(wait_stream(ctx, false));
+    return NS_OK;
+}
+
+// staging of n_blocks members of `text` bytes of text; NS_EINVAL when that is too much for one call
+static int stage_members(NsContext* ctx, const char* fname, uint64_t text, uint32_t* n_blocks) {
+    const uint64_t n_blocks64 = (text + BGZF_BLOCK - 1) / BGZF_BLOCK;
+    if (n_blocks64 > 0x7fffffffu) return fail(ctx, NS_EINVAL, "%s: %llu bytes of text is too much for one call", fname,
+                                              (unsigned long long)text);
+    *n_blocks = (uint32_t)n_blocks64;
+    CK(ctx->z_stage.ensure((size_t)*n_blocks * BGZF_SLOT));
+    CK(ctx->z_msize.ensure((size_t)*n_blocks * sizeof(uint64_t)));
+    CK(ctx->z_moff.ensure((size_t)*n_blocks * sizeof(uint64_t)));
+    CK(ctx->z_trailer.ensure((size_t)*n_blocks * sizeof(uint2)));
+    return NS_OK;
+}
+
+static int fetch_members(NsContext* ctx, const char* fname, bool have, const DevBuf& src, uint64_t bytes, uint8_t* out, uint64_t cap) {
+    if (!have) return fail(ctx, NS_ESTATE, "%s: the last batch has not been compressed", fname);
+    if (cap < bytes) return fail(ctx, NS_ENOMEM, "%s: %llu bytes do not fit in %llu", fname, (unsigned long long)bytes,
+                                 (unsigned long long)cap);
+    if (bytes == 0) return NS_OK;
+    if (!out) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(out, src.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(wait_stream(ctx, bytes >= (64u << 20)));
+    return NS_OK;
+}
+
 int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
     if (!ctx) return NS_EINVAL;
     if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "ns_compress_records: null argument");
     if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "ns_compress_records: no simulated batch");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
     const NsBatchInfo& bi = ctx->last;
     const uint32_t n = bi.n_reads;
     ctx->have_z = false;
@@ -1514,29 +1576,16 @@ int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_
         *nbytes = 0;
         return NS_OK;
     }
-    uint64_t blob = 0;                      // the names' extent: every name with its NUL
-    for (uint32_t i = 0; i < n; ++i) blob = std::max<uint64_t>(blob, name_off[i] + strlen(names + name_off[i]) + 1);
-    CK(upload(ctx->z_names, names, blob, st));
-    CK(upload(ctx->z_name_off, name_off, (size_t)n * sizeof(uint64_t), st));
-    CK(ctx->z_name_len.ensure((size_t)n * sizeof(uint32_t)));
-    CK(ctx->z_rec_off.ensure((size_t)n * sizeof(uint64_t)));
-    CK(ctx->scan_in.ensure((size_t)n * sizeof(uint64_t)));
+    if (int rc = upload_names(ctx, names, name_off, n)) return rc;
     uint64_t* totals = ctx->totals.as<uint64_t>();
-    CK(cudaMemsetAsync(totals + NS_T_Z_TEXT, 0, 3 * sizeof(uint64_t), st));
     const uint32_t fastq = ctx->hcfg.fastq ? 1u : 0u;
     CK(launch(ctx, bgzf_record_size, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
               ctx->z_name_off.as<uint64_t>(), fastq, ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>()));
     if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->z_rec_off.as<uint64_t>(), n, NS_T_Z_TEXT)) return rc;
     if (int rc = publish_totals_and_wait(ctx)) return rc;
     const uint64_t text = ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT];
-    const uint64_t n_blocks64 = (text + BGZF_BLOCK - 1) / BGZF_BLOCK;
-    if (n_blocks64 > 0x7fffffffu) return fail(ctx, NS_EINVAL, "ns_compress_records: %llu bytes of text is too much for one call",
-                                              (unsigned long long)text);
-    const uint32_t n_blocks = (uint32_t)n_blocks64;
-    CK(ctx->z_stage.ensure((size_t)n_blocks * BGZF_SLOT));
-    CK(ctx->z_msize.ensure((size_t)n_blocks * sizeof(uint64_t)));
-    CK(ctx->z_moff.ensure((size_t)n_blocks * sizeof(uint64_t)));
-    CK(ctx->z_trailer.ensure((size_t)n_blocks * sizeof(uint2)));
+    uint32_t n_blocks = 0;
+    if (int rc = stage_members(ctx, "ns_compress_records", text, &n_blocks)) return rc;
     BgzfArgs za;
     za.reads = ctx->reads.as<NsReadMeta>();
     za.seq = ctx->seq.as<uint8_t>();
@@ -1554,17 +1603,8 @@ int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_
     za.oversize = (unsigned long long*)(totals + NS_T_Z_OVERSIZE);
     CK(cudaFuncSetAttribute(bgzf_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BgzfSmem)));
     CK(launch(ctx, bgzf_deflate_kernel, n_blocks, BGZF_THREADS, sizeof(BgzfSmem), za));
-    if (int rc = scan_total(ctx, ctx->z_msize.as<uint64_t>(), ctx->z_moff.as<uint64_t>(), n_blocks, NS_T_Z_BYTES)) return rc;
-    if (int rc = publish_totals_and_wait(ctx)) return rc;
-    const uint64_t* h = ctx->h_totals.as<uint64_t>();
-    if (h[NS_T_Z_OVERSIZE])
-        return fail(ctx, NS_ESTATE, "ns_compress_records: %llu BGZF members exceed %u bytes", (unsigned long long)h[NS_T_Z_OVERSIZE],
-                    BGZF_MAX_MEMBER);
-    const uint64_t total = h[NS_T_Z_BYTES];
-    CK(ctx->z_out.ensure((size_t)total));
-    CK(launch(ctx, bgzf_pack_kernel, n_blocks, 256, 0, (const uint8_t*)ctx->z_stage.p, (const uint64_t*)ctx->z_msize.p,
-              (const uint64_t*)ctx->z_moff.p, (const uint2*)ctx->z_trailer.p, ctx->z_out.as<uint8_t>()));
-    CK(wait_stream(ctx, false));
+    uint64_t total = 0;
+    if (int rc = pack_members(ctx, "ns_compress_records", n_blocks, ctx->z_out, &total)) return rc;
     ctx->z_bytes = total;
     ctx->have_z = true;
     *nbytes = total;
@@ -1573,15 +1613,77 @@ int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_
 
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap) {
     if (!ctx) return NS_EINVAL;
-    if (!ctx->have_z) return fail(ctx, NS_ESTATE, "ns_fetch_compressed: the last batch has not been compressed");
-    if (cap < ctx->z_bytes) return fail(ctx, NS_ENOMEM, "ns_fetch_compressed: %llu bytes do not fit in %llu",
-                                        (unsigned long long)ctx->z_bytes, (unsigned long long)cap);
-    if (ctx->z_bytes == 0) return NS_OK;
-    if (!out) return fail(ctx, NS_EINVAL, "ns_fetch_compressed: null argument");
+    return fetch_members(ctx, "ns_fetch_compressed", ctx->have_z, ctx->z_out, ctx->z_bytes, out, cap);
+}
+
+int ns_compress_error_profile(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    static const char* fname = "ns_compress_error_profile";
+    if (!ctx) return NS_EINVAL;
+    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
+    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
+    if (ctx->last_kind != NS_KIND_ALIGNED) return fail(ctx, NS_EINVAL, "%s: the last batch is unaligned reads, which have no error profile", fname);
     CK(cudaSetDevice(ctx->device));
-    CK(cudaMemcpyAsync(out, ctx->z_out.p, ctx->z_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(wait_stream(ctx, ctx->z_bytes >= (64u << 20)));
+    const NsBatchInfo& bi = ctx->last;
+    const uint32_t n = bi.n_reads;
+    ctx->have_ep = false;
+    ctx->ep_bytes = 0;
+    if (n == 0) {
+        ctx->have_ep = true;
+        *nbytes = 0;
+        return NS_OK;
+    }
+    if (int rc = upload_names(ctx, names, name_off, n)) return rc;
+    const Tables& tab = *ctx->tables;
+    EpArgs ea;
+    ea.reads = ctx->reads.as<NsReadMeta>();
+    ea.pieces = ctx->pieces.as<NsPieceMeta>();
+    ea.ops = ctx->ops.as<uint32_t>();
+    ea.seq = ctx->seq.as<uint8_t>();
+    ea.ref = tab.dref.bases;
+    ea.chrom_off = tab.dref.chrom_off;
+    ea.names = ctx->z_names.as<char>();
+    ea.name_off = ctx->z_name_off.as<uint64_t>();
+    ea.name_len = ctx->z_name_len.as<uint32_t>();
+    ea.n_reads = n;
+    ea.key = make_uint2((uint32_t)ctx->seed, (uint32_t)(ctx->seed >> 32));
+    ea.first_id = ctx->last_first_id;
+    ea.size = ctx->scan_in.as<uint64_t>();
+    ea.off = ctx->z_rec_off.as<uint64_t>();
+    const unsigned warps_grid = (n + 7) / 8;                    // one warp per read, 8 per block
+    CK(launch(ctx, errprof_size_kernel, warps_grid, 256, 0, ea));
+    if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->z_rec_off.as<uint64_t>(), n, NS_T_Z_TEXT)) return rc;
+    if (int rc = publish_totals_and_wait(ctx)) return rc;
+    const uint64_t text = ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT];
+    if (text == 0) {                                            // no error events
+        ctx->have_ep = true;
+        *nbytes = 0;
+        return NS_OK;
+    }
+    uint32_t n_blocks = 0;
+    if (int rc = stage_members(ctx, fname, text, &n_blocks)) return rc;
+    CK(ctx->ep_text.ensure((size_t)text));
+    ea.text = ctx->ep_text.as<uint8_t>();
+    CK(launch(ctx, errprof_write_kernel, warps_grid, 256, 0, ea));
+    BgzfRowsArgs za;
+    za.text = ctx->ep_text.as<uint8_t>();
+    za.text_bytes = text;
+    za.stage = ctx->z_stage.as<uint8_t>();
+    za.member_size = ctx->z_msize.as<uint64_t>();
+    za.trailer = ctx->z_trailer.as<uint2>();
+    za.oversize = (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_OVERSIZE);
+    CK(cudaFuncSetAttribute(bgzf_deflate_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BgzfRowsSmem)));
+    CK(launch(ctx, bgzf_deflate_rows_kernel, n_blocks, BGZF_THREADS, sizeof(BgzfRowsSmem), za));
+    uint64_t total = 0;
+    if (int rc = pack_members(ctx, fname, n_blocks, ctx->ep_out, &total)) return rc;
+    ctx->ep_bytes = total;
+    ctx->have_ep = true;
+    *nbytes = total;
     return NS_OK;
+}
+
+int ns_fetch_compressed_error_profile(NsContext* ctx, uint8_t* out, uint64_t cap) {
+    if (!ctx) return NS_EINVAL;
+    return fetch_members(ctx, "ns_fetch_compressed_error_profile", ctx->have_ep, ctx->ep_out, ctx->ep_bytes, out, cap);
 }
 
 int ns_transfer_info(NsContext* ctx, uint32_t* packed_bases, uint32_t* n_threads) {
@@ -1692,6 +1794,7 @@ int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     ctx->have_z = false;
+    ctx->have_ep = false;
     NsBatchInfo& bi = ctx->last;
     const uint32_t old_np = bi.n_pieces;
     const uint64_t old_ops = bi.n_ops;

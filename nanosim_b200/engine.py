@@ -44,7 +44,7 @@ class Engine:
         self._keep = {}
         self.fastq = False
         self.info = None
-        self._z_bytes = 0
+        self._z_bytes = self._ep_bytes = 0
 
     def clone(self):
         """A context that shares this engine's reference + model in HBM (own stream and batch buffers)."""
@@ -53,7 +53,7 @@ class Engine:
         other._ctx = C.c_void_p()
         self._check(self._lib.ns_clone(self._ctx, C.byref(other._ctx)))
         other.device, other._keep, other.fastq, other.info = self.device, {}, self.fastq, None
-        other._z_bytes = 0
+        other._z_bytes = other._ep_bytes = 0
         other._parent = self            # keep the parent alive
         for k in ("ref", "tables"):
             if hasattr(self, k):
@@ -265,6 +265,28 @@ class Engine:
             out = np.empty(self._z_bytes, dtype=np.uint8)
         self._check(self._lib.ns_fetch_compressed(self._ctx, _ptr(out), C.c_uint64(len(out))))
         return out[:self._z_bytes]
+
+    def compress_error_profile(self, names):
+        """The last aligned batch's error-profile rows (records.format_error_profile's bytes, no header line) as BGZF
+        members, formatted and compressed on the device and kept there (ns_compress_error_profile).  ``names`` as for
+        compress_records.  Returns their size in bytes (0: no error events); no end-of-file block."""
+        from .records import _name_blob
+        blob, offs = _name_blob(names)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        if len(offs) != int(self.info.n_reads):
+            raise ValueError("compress_error_profile: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
+        n = C.c_uint64()
+        self._check(self._lib.ns_compress_error_profile(self._ctx, blob, _ptr(offs), C.byref(n)))
+        self._ep_bytes = int(n.value)
+        return self._ep_bytes
+
+    def fetch_compressed_error_profile(self, out=None):
+        """The members of the last compress_error_profile() -> uint8 array (into ``out`` when given, as for
+        fetch_compressed)."""
+        if out is None:
+            out = np.empty(self._ep_bytes, dtype=np.uint8)
+        self._check(self._lib.ns_fetch_compressed_error_profile(self._ctx, _ptr(out), C.c_uint64(len(out))))
+        return out[:self._ep_bytes]
 
     def device_buffers(self):
         ps = [C.c_void_p() for _ in range(5)]

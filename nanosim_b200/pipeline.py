@@ -23,7 +23,7 @@ class _HostBuffers:
 
     def __init__(self, fastq):
         self.fastq = fastq
-        self.cap = {"seq": 0, "qual": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0}
+        self.cap = {"seq": 0, "qual": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0, "gz_err": 0}
         self.t = {}
 
     def _alloc(self, nbytes):
@@ -51,15 +51,18 @@ class _HostBuffers:
 class BatchPipeline:
     """compress: None, or names(batch, job) -> the batch's read names (records.NameTable).  With it the pipeline runs in
     compressed mode: the worker fetches the read and piece metadata (and the bases and ops when want_ops, for the error
-    profile; never the qualities), builds the names, compresses the records on the device (ns_compress_records) and fetches
-    the BGZF members into pinned memory; the consumer gets them as ``batch.gz`` and the names as ``batch.names``."""
+    profile formatted on the host; never the qualities), builds the names, compresses the records on the device
+    (ns_compress_records) and fetches the BGZF members into pinned memory; the consumer gets them as ``batch.gz`` and the
+    names as ``batch.names``.  compress_profile (compressed mode, aligned batches): the error profile is formatted and
+    compressed on the device as well (ns_compress_error_profile); its members arrive as ``batch.gz_err``."""
 
-    def __init__(self, engine, depth=2, fetch=True, want_ops=False, want_pieces=True, compress=None):
+    def __init__(self, engine, depth=2, fetch=True, want_ops=False, want_pieces=True, compress=None, compress_profile=False):
         self.engines = [engine] + [engine.clone() for _ in range(max(1, depth) - 1)]
         self.depth = len(self.engines)
         self.fetch, self.want_ops, self.want_pieces, self.compress = fetch, want_ops, want_pieces, compress
+        self.compress_profile = compress_profile
         self.bufs = [_HostBuffers(engine.fastq) for _ in self.engines]
-        self.hint = {"seq": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0}     # largest batch seen by any slot (pinned allocs are slow)
+        self.hint = {"seq": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0, "gz_err": 0}     # largest batch seen by any slot (pinned allocs are slow)
 
     def close(self):
         for e in self.engines[1:]:
@@ -117,6 +120,11 @@ class BatchPipeline:
         if nz > self.hint["gz"]:
             self.hint["gz"] = nz
         b.gz = eng.fetch_compressed(hb.ensure("gz", max(nz, 1), self.hint["gz"]))
+        if self.compress_profile:
+            ne = eng.compress_error_profile(b.names)
+            if ne > self.hint["gz_err"]:
+                self.hint["gz_err"] = ne
+            b.gz_err = eng.fetch_compressed_error_profile(hb.ensure("gz_err", max(ne, 1), self.hint["gz_err"]))
         return b
 
     def warm(self, jobs):

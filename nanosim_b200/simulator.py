@@ -13,7 +13,9 @@ read_profile() / simulation() keep the reference's names and argument meaning:
 """
 import argparse
 import os
+import struct
 import sys
+import zlib
 from textwrap import dedent
 from time import strftime
 
@@ -32,6 +34,15 @@ VERSION = "3.2.2-b200"
 
 # BGZF end-of-file marker: an empty member (SAM/BAM format specification §4.1.2), once at the end of every .gz file
 BGZF_EOF = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")
+ERR_HEADER = b"Seq_name\tSeq_pos\terror_type\terror_length\tref_base\tseq_base\n"      # first line of the error profile (:1634)
+
+
+def bgzf_member(text):
+    """``text`` (at most 64 KiB) as one BGZF member, compressed on the host with zlib: the error profile's header line."""
+    c = zlib.compressobj(6, zlib.DEFLATED, -15)
+    payload = c.compress(text) + c.flush()
+    return (b"\x1f\x8b\x08\x04\x00\x00\x00\x00\x00\xff\x06\x00BC\x02\x00" + struct.pack("<H", 18 + len(payload) + 8 - 1) + payload +
+            struct.pack("<II", zlib.crc32(text), len(text)))
 
 
 def _log(msg):
@@ -74,19 +85,20 @@ class _RemoteReference(PackedReference):
 
 def read_profile(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                  polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                 device=0, seed=0, ir_files=None):
+                 device=0, seed=0, ir_files=None, ref_on_host=True):
     """read_profile (:244-591).  Under torchrun (WORLD_SIZE > 1) only rank 0 reads the reference files; the other ranks get
-    names and offsets through torch.distributed and the bases through ONE NCCL broadcast into their HBM (ns_bcast_nccl)."""
+    names and offsets through torch.distributed and the bases through ONE NCCL broadcast into their HBM (ns_bcast_nccl).
+    ref_on_host: those ranks also copy the bases back to the host, which only the plain error profile's formatter reads."""
     rank, world = _dist_world()
     if world > 1:
         return _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun,
-                                         polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files)
+                                         polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host)
     return _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
                                chimeric, homopolymer, fastq, device, seed, ir_files)
 
 
 def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp,
-                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files):
+                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True):
     dist = _dist_init()
     box = [None]
     if rank == 0:
@@ -131,7 +143,8 @@ def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per
         prof.engine = Engine(device=device, seed=seed)
     prof.engine.bcast_reference(info["nccl_id"], rank, world, 0)          # the one NCCL broadcast of the job
     if rank != 0:
-        prof.ref.bases = prof.engine.reference_bases(int(prof.ref.offsets[-1]))   # host copy for the error profile's reference column
+        if ref_on_host:
+            prof.ref.bases = prof.engine.reference_bases(int(prof.ref.offsets[-1]))   # host copy for the error profile's reference column
         prof.engine.ref = prof.ref
         prof.engine.set_model(prof.tables, perfect=per)
         if mode == "transcriptome":
@@ -235,9 +248,11 @@ def _shard(n, rank, world):
 
 def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min_l, num_threads, fastq,
                median_l=None, sd_l=None, model_ir=False, uracil=False, polya=None, chimeric=False,
-               batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False):
-    """gzip: write the reads as BGZF (``.gz``), compressed on the GPU; the error profile stays plain text.  Under torchrun
-    (world > 1) the per-rank files carry no end-of-file block: merge_rank_files appends it."""
+               batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False, gzip_error_profile=False):
+    """gzip: write the reads as BGZF (``.gz``), compressed on the GPU; the error profile stays plain text unless
+    gzip_error_profile (needs gzip): then it is formatted and compressed on the GPU too, ``<out>_aligned_error_profile.gz``,
+    whose first member is the header line.  Under torchrun (world > 1) the per-rank files carry neither the header nor the
+    end-of-file block: merge_rank_files writes them."""
     fmt_threads = max(1, min(num_threads, os.cpu_count() or 1))     # host threads of the record formatter
     eng = prof.engine
     meta = mode == "metagenome"
@@ -253,34 +268,42 @@ def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min
     ext = (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
     suffix = "" if world == 1 else str(rank)
     want_err = error_profile and not per
-    pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err)
+    gz_err = gzip and gzip_error_profile and want_err
+    pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err and not gz_err, compress_profile=gz_err)
     totals = {"reads": 0, "bases": 0, "bytes": 0}
     try:
         _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                         gzip)
+                         gzip, gz_err)
     finally:
         pipe.close()         # the cloned contexts own device batch buffers and pinned staging
     return totals            # what this rank simulated and wrote (the reference returns nothing)
 
 
 def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                     gzip=False):
+                     gzip=False, gz_err=False):
     def jobs(kind, lo, hi):
         return [(kind, start, min(batch_reads, hi - start)) for start in range(lo, hi, batch_reads)]
 
-    def put_reads(f, b, names):
-        if not gzip:
-            f.pos += write_records(f.fd, f.pos, b, names, fastq, n_threads=fmt_threads)
-            return
-        view = memoryview(b.gz)
+    def put_members(f, data):
+        view = memoryview(data)
         while len(view):
             w = os.pwrite(f.fd, view, f.pos)
             f.pos += w
             view = view[w:]
 
-    def end_reads(f):
-        if gzip and world == 1:
+    def put_reads(f, b, names):
+        if not gzip:
+            f.pos += write_records(f.fd, f.pos, b, names, fastq, n_threads=fmt_threads)
+            return
+        put_members(f, b.gz)
+
+    def end_bgzf(f):
+        if world == 1:
             f.pos += os.pwrite(f.fd, BGZF_EOF, f.pos)
+
+    def end_reads(f):
+        if gzip:
+            end_bgzf(f)
 
     class _Out:
         """An output file written at explicit offsets: the library's formatter threads pwrite() into it."""
@@ -297,8 +320,8 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
     _log("Start simulation of aligned reads")
     lo, hi = _shard(prof.number_aligned, rank, world)
     f_reads = _Out(out + "_aligned_reads" + suffix + ext)
-    f_err = _Out(out + ("_aligned_error_profile" if world == 1 else "_error_profile" + suffix),
-                 b"Seq_name\tSeq_pos\terror_type\terror_length\tref_base\tseq_base\n" if world == 1 else b"")
+    f_err = _Out(out + ("_aligned_error_profile" if world == 1 else "_error_profile" + suffix) + (".gz" if gz_err else ""),
+                 b"" if world > 1 else bgzf_member(ERR_HEADER) if gz_err else ERR_HEADER)
     try:
         def aligned_names(b, job):
             return name_table(b, prof.ref.names, job[1], perfect=per, metagenome=meta, transcriptome=trx)
@@ -308,7 +331,9 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             put_reads(f_reads, b, names)
             totals["reads"] += int(info.n_reads)
             totals["bases"] += int(info.total_bases)
-            if want_err:
+            if gz_err:
+                put_members(f_err, b.gz_err)
+            elif want_err:
                 f_err.pos += write_error_profile(f_err.fd, f_err.pos, b, names, prof.ref, seed=prof.seed, n_threads=fmt_threads)
 
         def retain_introns(engine, info, job):
@@ -323,6 +348,8 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
         pipe.run(jobs(L.NS_KIND_ALIGNED, lo, hi), sink_aligned, static_assign=meta,
                  after_simulate=retain_introns if (trx and prof.ir is not None and not per) else None)
         end_reads(f_reads)
+        if gz_err:
+            end_bgzf(f_err)
     finally:
         totals["bytes"] += f_reads.pos + f_err.pos
         f_reads.close()
@@ -330,7 +357,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
     if not per:
         _log("Start simulation of random reads")
         lo, hi = _shard(prof.number_unaligned, rank, world)
-        pipe.want_ops = False                              # unaligned reads are not logged (:1482-1549)
+        pipe.want_ops = pipe.compress_profile = False      # unaligned reads are not logged (:1482-1549)
         f_un = _Out(out + "_unaligned_reads" + suffix + ext)
         try:
             def unaligned_names(b, job):
@@ -350,19 +377,22 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             f_un.close()
 
 
-def merge_rank_files(out, fastq, per, world, gzip=False):
+def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=False):
     """Rank 0: concatenate per-rank sub-files in rank order and delete them (:1626-1639, :1667-1672).  gzip: the reads
-    files are BGZF members without an end-of-file block; the merged file gets it once, at its end."""
+    files are BGZF members without an end-of-file block; the merged file gets it once, at its end.  gzip_error_profile: so
+    are the error-profile files (``_error_profile{r}.gz``); the merged one starts with the header line's member."""
     ext = (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
     trailer = BGZF_EOF if gzip else b""
-    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, None, trailer)]
-    jobs.append(("_error_profile%d", "_aligned_error_profile", "Seq_name\tSeq_pos\terror_type\terror_length\tref_base\tseq_base\n", b""))
+    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, b"", trailer)]
+    if gzip_error_profile:
+        jobs.append(("_error_profile%d.gz", "_aligned_error_profile.gz", bgzf_member(ERR_HEADER), BGZF_EOF))
+    else:
+        jobs.append(("_error_profile%d", "_aligned_error_profile", ERR_HEADER, b""))
     if not per:
-        jobs.append(("_unaligned_reads%d" + ext, "_unaligned_reads" + ext, None, trailer))
+        jobs.append(("_unaligned_reads%d" + ext, "_unaligned_reads" + ext, b"", trailer))
     for pat, dst, header, end in jobs:
         with open(out + dst, "wb") as o:
-            if header:
-                o.write(header.encode())
+            o.write(header)
             for r in range(world):
                 p = out + (pat % r)
                 with open(p, "rb") as i:
@@ -376,8 +406,15 @@ def merge_rank_files(out, fastq, per, world, gzip=False):
 
 
 GZIP_HELP = ('Write the reads as BGZF-compressed <out>_aligned_reads.fast{a,q}.gz and <out>_unaligned_reads.fast{a,q}.gz, '
-             'compressed on the GPU (gzip, zcat and samtools read them). The error profile is still written as plain '
-             'text (Default = False)')
+             'compressed on the GPU (gzip, zcat and samtools read them). The error profile stays plain text unless '
+             '--gzip_error_profile is given (Default = False)')
+GZIP_ERR_HELP = ('With --gzip: write the error profile as BGZF-compressed <out>_aligned_error_profile.gz, formatted and '
+                 'compressed on the GPU (Default = False)')
+
+
+def _plain_error_profile(args):
+    """The run writes the error profile as plain text, formatted on the host from a host copy of the reference."""
+    return not (args.no_error_profile or args.perfect or args.gzip_error_profile)
 
 
 def build_parser():
@@ -424,6 +461,7 @@ def build_parser():
     g.add_argument('--no_error_profile', help='Skip writing <out>_aligned_error_profile', action='store_true', default=False)
     g.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
     g.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
+    g.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     mg = sub.add_parser('metagenome', help="Run the simulator on metagenome mode")
     mg.add_argument('-gl', '--genome_list', help="Reference metagenome list, tsv file, the first column is species/strain "
                     "name, the second column is the reference genome fasta/fastq file directory", required=True)
@@ -457,6 +495,7 @@ def build_parser():
     mg.add_argument('--no_error_profile', help='Skip writing <out>_aligned_error_profile', action='store_true', default=False)
     mg.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
     mg.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
+    mg.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     t = sub.add_parser('transcriptome', help="Run the simulator on transcriptome mode")
     t.add_argument('-rt', '--ref_t', help='Input reference transcriptome', required=True)
     t.add_argument('-rg', '--ref_g', help='Input reference genome, required if intron retention simulation is on', default='')
@@ -496,6 +535,7 @@ def build_parser():
     t.add_argument('--no_error_profile', help='Skip writing <out>_aligned_error_profile', action='store_true', default=False)
     t.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
     t.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
+    t.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     return parser, g, mg, t
 
 
@@ -547,7 +587,7 @@ def main_transcriptome(args, parser_t):
     prof = read_profile(args.ref_g, number, args.model_prefix, args.perfect, "transcriptome", args.strandness,
                         ref_t=args.ref_t, dna_type="linear", model_ir=model_ir, polya=args.polya, exp=args.exp,
                         homopolymer=args.homopolymer, fastq=args.fastq, device=device, seed=args.seed or 0,
-                        ir_files={"markov": args.ir_markov_model, "gff3": args.ir_gff3})
+                        ir_files={"markov": args.ir_markov_model, "gff3": args.ir_gff3}, ref_on_host=_plain_error_profile(args))
     if args.coverage is not None:
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
@@ -555,14 +595,15 @@ def main_transcriptome(args, parser_t):
     simulation(prof, "transcriptome", args.output, "transcriptome", args.perfect, args.KmerBias if args.homopolymer else None,
                args.basecaller, max_len, min_len, max(args.num_threads, 1), args.fastq, None, None, model_ir, args.uracil,
                args.polya, batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world,
-               gzip=args.gzip)
+               gzip=args.gzip, gzip_error_profile=args.gzip_error_profile)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
             dist.init_process_group("gloo")
         dist.barrier()
         if rank == 0:
-            merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip)
+            merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip,
+                             gzip_error_profile=args.gzip_error_profile)
         dist.barrier()
     _log("Finished!")
 
@@ -605,7 +646,7 @@ def main_metagenome(args, parser_mg):
         os.makedirs(dir_name, exist_ok=True)
     prof = read_profile(args.genome_list, [], args.model_prefix, args.perfect, "metagenome", args.strandness,
                         dna_type=args.dna_type_list, abun=args.abun, chimeric=args.chimeric, homopolymer=args.homopolymer,
-                        fastq=args.fastq, device=device, seed=args.seed or 0)
+                        fastq=args.fastq, device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args))
     rnd = random.Random(args.seed)
     L_ = prof.ref.lengths
     total_len = [int(L_[prof.ref.chrom_species == i].sum()) for i in range(len(prof.ref.species))]
@@ -620,14 +661,16 @@ def main_metagenome(args, parser_mg):
         prof.number_aligned, prof.number_unaligned = prof.counts[s_idx]
         simulation(prof, "metagenome", args.output + "_sample%d" % s_idx, "metagenome", args.perfect, None, None, max_len,
                    min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len, chimeric=args.chimeric,
-                   batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world, gzip=args.gzip)
+                   batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world, gzip=args.gzip,
+                   gzip_error_profile=args.gzip_error_profile)
         if world > 1:
             import torch.distributed as dist
             if not dist.is_initialized():
                 dist.init_process_group("gloo")
             dist.barrier()
             if rank == 0:
-                merge_rank_files(args.output + "_sample%d" % s_idx, args.fastq, args.perfect, world, gzip=args.gzip)
+                merge_rank_files(args.output + "_sample%d" % s_idx, args.fastq, args.perfect, world, gzip=args.gzip,
+                                 gzip_error_profile=args.gzip_error_profile)
             dist.barrier()
     _log("Finished!")
 
@@ -650,6 +693,12 @@ def main(argv=None):
     if args.mode is None:
         parser.print_help(sys.stderr)
         sys.exit(1)
+    if args.gzip_error_profile and not args.gzip:
+        sys.stderr.write("\n--gzip_error_profile needs --gzip!\n")
+        {"genome": parser_g, "metagenome": parser_mg, "transcriptome": parser_t}[args.mode].print_help(sys.stderr)
+        sys.exit(1)
+    # no profile is written with --no_error_profile or --perfect: nothing to compress
+    args.gzip_error_profile = args.gzip_error_profile and not args.no_error_profile and not args.perfect
     if args.mode == "metagenome":
         return main_metagenome(args, parser_mg)
     if args.mode == "transcriptome":
@@ -691,7 +740,7 @@ def main(argv=None):
 
     prof = read_profile(args.ref_g, number, args.model_prefix, args.perfect, args.mode, args.strandness,
                         dna_type=args.dna_type, chimeric=args.chimeric, homopolymer=args.homopolymer, fastq=args.fastq,
-                        device=device, seed=args.seed or 0)
+                        device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args))
     if args.coverage is not None:
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
@@ -699,14 +748,15 @@ def main(argv=None):
     simulation(prof, args.mode, args.output, args.dna_type, args.perfect, args.KmerBias if args.homopolymer else None,
                None, max_len, min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len,
                chimeric=args.chimeric, batch_reads=args.batch_reads, error_profile=not args.no_error_profile,
-               rank=rank, world=world, gzip=args.gzip)
+               rank=rank, world=world, gzip=args.gzip, gzip_error_profile=args.gzip_error_profile)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
             dist.init_process_group("gloo")
         dist.barrier()
         if rank == 0:
-            merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip)
+            merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip,
+                             gzip_error_profile=args.gzip_error_profile)
         dist.barrier()
     _log("Finished!")
 

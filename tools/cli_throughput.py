@@ -1,8 +1,10 @@
 """Wall-clock of the CLI end to end (model load, simulation, formatting or compression, file writes) on the 5 Mb synthetic
 reference, writing into /dev/shm when it exists.  Bases are counted from the reads files (text bytes / 2); a ``.gz`` file
 (``--gzip``) is counted by its decompressed size, the sum of its BGZF members' ISIZE fields.  With --gzip the time of
-every ns_compress_records call is reported too (the call ends in a device synchronise)."""
-import os, shutil, struct, sys, time, tempfile
+every ns_compress_records call is reported too, and with --gzip_error_profile that of every ns_compress_error_profile call
+(both calls end in a device synchronise) and the profile's compressed / plain ratio, next to zlib levels 1 and 6 on the
+text of its first 1024 members (decompressed and compressed again on the CPU after the run)."""
+import os, shutil, struct, sys, time, tempfile, zlib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import synth
@@ -25,21 +27,37 @@ def text_bytes(path):
             total += struct.unpack("<I", f.read(4))[0]
 
 
+def profile_sample(path, n_members=1024):
+    """(compressed bytes, text) of the first n_members members after the header member of a .gz error profile."""
+    data, pos, text, size = open(path, "rb").read(), 0, [], 0
+    for k in range(n_members + 1):
+        if pos >= len(data):
+            break
+        bsize = struct.unpack("<H", data[pos + 16:pos + 18])[0] + 1
+        if k:
+            text.append(zlib.decompress(data[pos:pos + bsize], 31))
+            size += bsize
+        pos += bsize
+    return size, b"".join(text)
+
+
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 300000
 extra = sys.argv[2:]
-compress_s = []
-_compress = Engine.compress_records
+timings = {"ns_compress_records": [], "ns_compress_error_profile": []}
 
 
-def timed_compress(self, names):
-    t = time.perf_counter()
-    try:
-        return _compress(self, names)
-    finally:
-        compress_s.append(time.perf_counter() - t)
+def timed(fn, key):
+    def call(self, names):
+        t = time.perf_counter()
+        try:
+            return fn(self, names)
+        finally:
+            timings[key].append(time.perf_counter() - t)
+    return call
 
 
-Engine.compress_records = timed_compress
+Engine.compress_records = timed(Engine.compress_records, "ns_compress_records")
+Engine.compress_error_profile = timed(Engine.compress_error_profile, "ns_compress_error_profile")
 tmp = tempfile.mkdtemp(prefix="cli_tp_", dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
 try:
     ref = os.path.join(tmp, "ecoli5m.fa")
@@ -56,10 +74,16 @@ try:
         n, extra, dt, bases / 1e9, bases / 1e9 / dt, {k: round(v / 1e9, 3) for k, v in sz.items()})
     if any(f.endswith(".gz") for f in reads):
         line += "; compressed / plain %.4f" % (sum(sz[f] for f in reads) / text)
-    if compress_s:
-        c = sorted(compress_s)
-        line += "; ns_compress_records %d calls, median %.1f ms, max %.1f ms, total %.2f s" % (
-            len(c), 1e3 * c[len(c) // 2], 1e3 * c[-1], sum(c))
+    for key, c in timings.items():
+        if c:
+            c = sorted(c)
+            line += "; %s %d calls, median %.1f ms, max %.1f ms, total %.2f s" % (key, len(c), 1e3 * c[len(c) // 2], 1e3 * c[-1], sum(c))
+    err = os.path.join(tmp, "sim_aligned_error_profile.gz")
+    if os.path.exists(err):
+        line += "; error profile compressed / plain %.4f" % (sz["sim_aligned_error_profile.gz"] / text_bytes(err))
+        size, sample = profile_sample(err)
+        line += " (first %.0f MB of text: %.4f, zlib -1 %.4f, zlib -6 %.4f)" % (
+            len(sample) / 1e6, size / len(sample), len(zlib.compress(sample, 1)) / len(sample), len(zlib.compress(sample, 6)) / len(sample))
     print(line)
 finally:
     shutil.rmtree(tmp, ignore_errors=True)
