@@ -357,7 +357,17 @@ int64_t ns_write_error_profile(int fd, uint64_t file_off, const uint8_t* seq, co
  * by this call).  The members stay in HBM until the next ns_simulate / ns_reemit; *nbytes = their size.  NS_ESTATE if a
  * member came out larger than 64 KiB (cannot happen: see nanosim_b200/csrc/bgzf_kernel.cuh). */
 int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
-/* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' *nbytes. */
+/* The last batch's reads as unaligned BAM records (after ns_reemit as well), BGZF-compressed on the device like
+ * ns_compress_records: one record per read, in read order and orientation, with the name ns_format_records would write,
+ * flag 4 (unmapped), refID / pos / next_refID / next_pos -1, mapq 255, bin 4680, no CIGAR and no aux data; the bases as
+ * 4-bit codes ("=ACMGRSVTWYHKDBN" in either case, U as T, any other byte N), the qualities - 33 (0xff each without
+ * --fastq).  Records straddle members where the 56 KiB cut falls.  Neither the BAM header nor the end-of-file block is
+ * included.  The members replace those of the last ns_compress_records (and a later ns_compress_records replaces these);
+ * ns_fetch_compressed copies them.  NS_EINVAL when a name is longer than 254 bytes (the message names the first such read
+ * and its length); names are never truncated. */
+int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
+/* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' (or ns_compress_bam's)
+ * *nbytes. */
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap);
 /* The rows of <out>_aligned_error_profile for the last aligned batch (ns_format_error_profile's bytes, after ns_reemit as
  * well; no header line) as BGZF, formatted and compressed on the device from the batch's reads, pieces, event scripts and

@@ -9,6 +9,8 @@
 // takes at most 9 * (BGZF_BLOCK + 1) bits = 64 513 bytes.  The header sends 259 code lengths with a code-length code
 // of at most 7 bits (no run-length symbols), 3 + 14 + 19 * 3 + 259 * 7 bits = 237 bytes, and the gzip framing is 26
 // bytes: 64 776 <= 65 536.  The kernel still checks every member and reports a violation (no stored-block fallback).
+// The bound does not depend on the bytes, so it holds for the binary BAM records (ns_compress_bam) as well: the record
+// layout is the kernel's template parameter (BgzfTextLayout, BgzfBamLayout).
 //
 // Error-profile rows (bgzf_deflate_rows_kernel, ns_compress_error_profile): flat text in HBM, cut and framed the same way.
 // Every row starts with the read's name and a read has hundreds of rows, so each row's name is sent as a back-reference
@@ -120,8 +122,11 @@ __device__ __forceinline__ uint32_t bgzf_crc_combine(const uint32_t* x2n, uint32
 // Level 0 lists the leaves; level j merges the leaves with the pairs of level j-1's list.  The first 2n - 2 items of the
 // top level are the solution: every leaf among the first m items of a level gains one bit, and the packages among them
 // select the first 2 * packages items of the level below.  S: the kernel's shared-memory layout (its u.pm lists).
+// This and bgzf_canonical are inlined by force: left to the inliner, their code in the records kernel depended on how many
+// kernels call them, and a second instantiation of that kernel left it with 40 registers and 20 B of spills instead of
+// 57 and none.
 template <class S>
-__device__ void bgzf_package_merge(S& s, const uint32_t* w, int n, int limit, uint8_t* len) {
+__device__ __forceinline__ void bgzf_package_merge(S& s, const uint32_t* w, int n, int limit, uint8_t* len) {
     const int cap = 2 * n - 2;
     uint32_t* prev = s.u.pm.w[0];
     uint32_t* cur = s.u.pm.w[1];
@@ -161,7 +166,7 @@ __device__ void bgzf_package_merge(S& s, const uint32_t* w, int n, int limit, ui
 }
 
 // canonical codes (RFC 1951 §3.2.2), bit-reversed
-__device__ void bgzf_canonical(const uint8_t* len, int n, uint32_t* code) {
+__device__ __forceinline__ void bgzf_canonical(const uint8_t* len, int n, uint32_t* code) {
     uint32_t count[16] = {0}, next[16];
     for (int k = 0; k < n; ++k) ++count[len[k]];
     count[0] = 0;
@@ -199,6 +204,94 @@ __device__ __forceinline__ uint8_t bgzf_record_byte(uint64_t q, uint32_t fastq, 
     return q < L ? ql[q] : '\n';
 }
 
+// BAM output (ns_compress_bam): one unmapped record per read in read orientation (SAM/BAM format specification §4.2):
+// block_size, refID -1, pos -1, l_read_name, mapq 255, bin 4680 (reg2bin(-1, 0)), n_cigar_op 0, flag 4, l_seq,
+// next_refID -1, next_pos -1, tlen 0 (36 bytes, little-endian), the name and its NUL, the bases as 4-bit codes (first
+// base in the high nibble, the low nibble of an odd last byte 0), the qualities - 33 (FASTQ) or 0xff each (FASTA)
+constexpr uint32_t BAM_FIXED = 36;
+constexpr uint32_t BAM_MAX_NAME = 254;              // l_read_name is one byte and counts the NUL
+
+// 4-bit codes of the letters a..z of either case ("=ACMGRSVTWYHKDBN" -> 0..15, U as T as htslib reads it, other letters
+// N), 16 nibbles to a word, so that the per-byte lookup is register arithmetic
+constexpr uint64_t bam_letter_nibbles(int first) {
+    const char* abc = "=ACMGRSVTWYHKDBN";
+    uint64_t w = 0;
+    for (int k = 0; k < 16 && first + k < 26; ++k) {
+        const char c = (char)('A' + first + k);
+        uint64_t v = c == 'U' ? 8 : 15;
+        for (int j = 1; j < 16; ++j)
+            if (abc[j] == c) v = (uint64_t)j;
+        w |= v << (4 * k);
+    }
+    return w;
+}
+constexpr uint64_t kBamNibblesAtoP = bam_letter_nibbles(0), kBamNibblesQtoZ = bam_letter_nibbles(16);
+
+__device__ __forceinline__ uint32_t bam_base_code(uint8_t c) {
+    if (c == '=') return 0;
+    const uint32_t k = (uint32_t)(c | 0x20) - 'a';            // 0..25 exactly for the letters of either case
+    if (k >= 26) return 15;
+    return (uint32_t)(((k < 16 ? kBamNibblesAtoP : kBamNibblesQtoZ) >> (4 * (k & 15))) & 15u);
+}
+
+// byte q of a read's BAM record, arguments as for bgzf_record_byte
+__device__ __forceinline__ uint8_t bam_record_byte(uint64_t q, uint32_t fastq, const char* nm, uint32_t nl, const uint8_t* sq,
+                                                   const uint8_t* ql, uint32_t L) {
+    if (q < BAM_FIXED) {
+        uint32_t w;
+        switch ((uint32_t)q >> 2) {
+        case 0: w = BAM_FIXED - 4 + nl + 1 + (L + 1) / 2 + L; break;          // block_size
+        case 3: w = (nl + 1) | (255u << 8) | (4680u << 16); break;          // l_read_name, mapq, bin
+        case 4: w = 4u << 16; break;                                        // n_cigar_op, flag
+        case 5: w = L; break;                                               // l_seq
+        case 8: w = 0; break;                                               // tlen
+        default: w = 0xffffffffu;                                           // refID, pos, next_refID, next_pos
+        }
+        return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
+    }
+    q -= BAM_FIXED;
+    if (q < nl) return (uint8_t)nm[q];
+    if (q == nl) return 0;
+    q -= nl + 1;
+    const uint64_t n_packed = (L + 1) / 2;
+    if (q < n_packed) {
+        const uint64_t b = 2 * q;
+        return (uint8_t)((bam_base_code(sq[b]) << 4) | (b + 1 < L ? bam_base_code(sq[b + 1]) : 0u));
+    }
+    q -= n_packed;
+    return fastq ? (uint8_t)(ql[q] - 33) : 0xffu;
+}
+
+// one read's BAM record size; names longer than BAM_MAX_NAME are counted into *long_names (the call then fails)
+__global__ void bam_record_size(const NsReadMeta* __restrict__ reads, uint32_t n, const char* __restrict__ names,
+                                const uint64_t* __restrict__ name_off, uint32_t* __restrict__ name_len, uint64_t* __restrict__ size,
+                                unsigned long long* long_names) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const char* nm = names + name_off[i];
+    uint32_t nl = 0;
+    while (nm[nl]) ++nl;
+    name_len[i] = nl;
+    if (nl > BAM_MAX_NAME) atomicAdd(long_names, 1ull);
+    const uint64_t L = reads[i].seq_len;
+    size[i] = BAM_FIXED + nl + 1 + (L + 1) / 2 + L;
+}
+
+// the record layouts bgzf_deflate_kernel gathers from
+struct BgzfTextLayout {
+    static __device__ __forceinline__ uint8_t byte(uint64_t q, uint32_t fastq, const char* nm, uint32_t nl, const uint8_t* sq,
+                                                   const uint8_t* ql, uint32_t L) {
+        return bgzf_record_byte(q, fastq, nm, nl, sq, ql, L);
+    }
+};
+struct BgzfBamLayout {
+    static __device__ __forceinline__ uint8_t byte(uint64_t q, uint32_t fastq, const char* nm, uint32_t nl, const uint8_t* sq,
+                                                   const uint8_t* ql, uint32_t L) {
+        return bam_record_byte(q, fastq, nm, nl, sq, ql, L);
+    }
+};
+
+template <class Layout>
 __global__ void __launch_bounds__(BGZF_THREADS) bgzf_deflate_kernel(BgzfArgs a) {
     extern __shared__ __align__(16) unsigned char bgzf_smem_raw[];
     BgzfSmem& s = *reinterpret_cast<BgzfSmem*>(bgzf_smem_raw);
@@ -236,7 +329,7 @@ __global__ void __launch_bounds__(BGZF_THREADS) bgzf_deflate_kernel(BgzfArgs a) 
             const uint32_t nl = a.name_len[r];
             const uint8_t* sq = a.seq + rm.seq_off;
             const uint8_t* ql = a.fastq ? a.qual + rm.seq_off : nullptr;
-            for (; k < hi && p < r1; ++k, ++p) s.text[k] = bgzf_record_byte(p - r0, a.fastq, nm, nl, sq, ql, rm.seq_len);
+            for (; k < hi && p < r1; ++k, ++p) s.text[k] = Layout::byte(p - r0, a.fastq, nm, nl, sq, ql, rm.seq_len);
         }
     }
     __syncthreads();

@@ -1501,10 +1501,12 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
     return NS_OK;
 }
 
-// totals[] slots of ns_compress_records (behind the batch's): text bytes, compressed bytes, members above 64 KiB
+// totals[] slots of ns_compress_records (behind the batch's): text bytes, compressed bytes, members above 64 KiB; of
+// ns_compress_bam: read names too long for BAM
 #define NS_T_Z_TEXT 12
 #define NS_T_Z_BYTES 13
 #define NS_T_Z_OVERSIZE 14
+#define NS_T_Z_LONG_NAMES 15
 
 // the n names (ns_format_records' layout) into z_names / z_name_off; room for the names' lengths, the per-read sizes
 // (scan_in) and their offsets (z_rec_off); the totals slots of a compression zeroed
@@ -1517,7 +1519,7 @@ static int upload_names(NsContext* ctx, const char* names, const uint64_t* name_
     CK(ctx->z_name_len.ensure((size_t)n * sizeof(uint32_t)));
     CK(ctx->z_rec_off.ensure((size_t)n * sizeof(uint64_t)));
     CK(ctx->scan_in.ensure((size_t)n * sizeof(uint64_t)));
-    CK(cudaMemsetAsync(ctx->totals.as<uint64_t>() + NS_T_Z_TEXT, 0, 3 * sizeof(uint64_t), st));
+    CK(cudaMemsetAsync(ctx->totals.as<uint64_t>() + NS_T_Z_TEXT, 0, 4 * sizeof(uint64_t), st));
     return NS_OK;
 }
 
@@ -1562,10 +1564,13 @@ static int fetch_members(NsContext* ctx, const char* fname, bool have, const Dev
     return NS_OK;
 }
 
-int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+// ns_compress_records (FASTA/FASTQ text) and ns_compress_bam (BAM records): the last batch's records in that layout as
+// BGZF members in z_out
+static int compress_records(NsContext* ctx, const char* fname, bool bam, const char* names, const uint64_t* name_off,
+                            uint64_t* nbytes) {
     if (!ctx) return NS_EINVAL;
-    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "ns_compress_records: null argument");
-    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "ns_compress_records: no simulated batch");
+    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
+    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
     CK(cudaSetDevice(ctx->device));
     const NsBatchInfo& bi = ctx->last;
     const uint32_t n = bi.n_reads;
@@ -1579,13 +1584,24 @@ int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_
     if (int rc = upload_names(ctx, names, name_off, n)) return rc;
     uint64_t* totals = ctx->totals.as<uint64_t>();
     const uint32_t fastq = ctx->hcfg.fastq ? 1u : 0u;
-    CK(launch(ctx, bgzf_record_size, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
-              ctx->z_name_off.as<uint64_t>(), fastq, ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>()));
+    if (bam)
+        CK(launch(ctx, bam_record_size, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
+                  ctx->z_name_off.as<uint64_t>(), ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>(),
+                  (unsigned long long*)(totals + NS_T_Z_LONG_NAMES)));
+    else
+        CK(launch(ctx, bgzf_record_size, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
+                  ctx->z_name_off.as<uint64_t>(), fastq, ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>()));
     if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->z_rec_off.as<uint64_t>(), n, NS_T_Z_TEXT)) return rc;
     if (int rc = publish_totals_and_wait(ctx)) return rc;
+    if (const uint64_t n_long = ctx->h_totals.as<uint64_t>()[NS_T_Z_LONG_NAMES]) {
+        uint32_t i = 0;                                         // the first such name, for the message
+        while (i + 1 < n && strlen(names + name_off[i]) <= BAM_MAX_NAME) ++i;
+        return fail(ctx, NS_EINVAL, "%s: read %u has a name of %zu bytes, more than the %u BAM holds (%llu such reads)", fname, i,
+                    strlen(names + name_off[i]), BAM_MAX_NAME, (unsigned long long)n_long);
+    }
     const uint64_t text = ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT];
     uint32_t n_blocks = 0;
-    if (int rc = stage_members(ctx, "ns_compress_records", text, &n_blocks)) return rc;
+    if (int rc = stage_members(ctx, fname, text, &n_blocks)) return rc;
     BgzfArgs za;
     za.reads = ctx->reads.as<NsReadMeta>();
     za.seq = ctx->seq.as<uint8_t>();
@@ -1601,14 +1617,23 @@ int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_
     za.member_size = ctx->z_msize.as<uint64_t>();
     za.trailer = ctx->z_trailer.as<uint2>();
     za.oversize = (unsigned long long*)(totals + NS_T_Z_OVERSIZE);
-    CK(cudaFuncSetAttribute(bgzf_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BgzfSmem)));
-    CK(launch(ctx, bgzf_deflate_kernel, n_blocks, BGZF_THREADS, sizeof(BgzfSmem), za));
+    void (*deflate)(BgzfArgs) = bam ? bgzf_deflate_kernel<BgzfBamLayout> : bgzf_deflate_kernel<BgzfTextLayout>;
+    CK(cudaFuncSetAttribute(deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BgzfSmem)));
+    CK(launch(ctx, deflate, n_blocks, BGZF_THREADS, sizeof(BgzfSmem), za));
     uint64_t total = 0;
-    if (int rc = pack_members(ctx, "ns_compress_records", n_blocks, ctx->z_out, &total)) return rc;
+    if (int rc = pack_members(ctx, fname, n_blocks, ctx->z_out, &total)) return rc;
     ctx->z_bytes = total;
     ctx->have_z = true;
     *nbytes = total;
     return NS_OK;
+}
+
+int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    return compress_records(ctx, "ns_compress_records", false, names, name_off, nbytes);
+}
+
+int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    return compress_records(ctx, "ns_compress_bam", true, names, name_off, nbytes);
 }
 
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap) {

@@ -258,9 +258,23 @@ class Engine:
         self._z_bytes = int(n.value)
         return self._z_bytes
 
+    def compress_bam(self, names):
+        """The last batch's reads as unaligned BAM records (``names`` as for compress_records; at most 254 bytes each)
+        as BGZF members, built on the device and kept there (ns_compress_bam); they replace those of the last
+        compress_records().  Returns their size in bytes; neither the BAM header nor the end-of-file block."""
+        from .records import _name_blob
+        blob, offs = _name_blob(names)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        if len(offs) != int(self.info.n_reads):
+            raise ValueError("compress_bam: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
+        n = C.c_uint64()
+        self._check(self._lib.ns_compress_bam(self._ctx, blob, _ptr(offs), C.byref(n)))
+        self._z_bytes = int(n.value)
+        return self._z_bytes
+
     def fetch_compressed(self, out=None):
-        """The members of the last compress_records() -> uint8 array (into ``out`` when given: a uint8 array, pinned
-        memory recommended, at least that large)."""
+        """The members of the last compress_records() or compress_bam() -> uint8 array (into ``out`` when given: a
+        uint8 array, pinned memory recommended, at least that large)."""
         if out is None:
             out = np.empty(self._z_bytes, dtype=np.uint8)
         self._check(self._lib.ns_fetch_compressed(self._ctx, _ptr(out), C.c_uint64(len(out))))

@@ -54,13 +54,15 @@ class BatchPipeline:
     profile formatted on the host; never the qualities), builds the names, compresses the records on the device
     (ns_compress_records) and fetches the BGZF members into pinned memory; the consumer gets them as ``batch.gz`` and the
     names as ``batch.names``.  compress_profile (compressed mode, aligned batches): the error profile is formatted and
-    compressed on the device as well (ns_compress_error_profile); its members arrive as ``batch.gz_err``."""
+    compressed on the device as well (ns_compress_error_profile); its members arrive as ``batch.gz_err``.  bam
+    (compressed mode): the records are unaligned BAM records (ns_compress_bam) instead of FASTA/FASTQ text."""
 
-    def __init__(self, engine, depth=2, fetch=True, want_ops=False, want_pieces=True, compress=None, compress_profile=False):
+    def __init__(self, engine, depth=2, fetch=True, want_ops=False, want_pieces=True, compress=None, compress_profile=False,
+                 bam=False):
         self.engines = [engine] + [engine.clone() for _ in range(max(1, depth) - 1)]
         self.depth = len(self.engines)
         self.fetch, self.want_ops, self.want_pieces, self.compress = fetch, want_ops, want_pieces, compress
-        self.compress_profile = compress_profile
+        self.compress_profile, self.bam = compress_profile, bam
         self.bufs = [_HostBuffers(engine.fastq) for _ in self.engines]
         self.hint = {"seq": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0, "gz_err": 0}     # largest batch seen by any slot (pinned allocs are slow)
 
@@ -116,7 +118,7 @@ class BatchPipeline:
         b = Batch(info, seq, None, reads.view(L.READ_DTYPE), pieces.view(L.PIECE_DTYPE),
                   ops.view(np.uint32) if ops is not None else np.zeros(0, dtype=np.uint32) if self.want_ops else None, kind, first)
         b.names = self.compress(b, job)
-        nz = eng.compress_records(b.names)
+        nz = eng.compress_bam(b.names) if self.bam else eng.compress_records(b.names)
         if nz > self.hint["gz"]:
             self.hint["gz"] = nz
         b.gz = eng.fetch_compressed(hb.ensure("gz", max(nz, 1), self.hint["gz"]))

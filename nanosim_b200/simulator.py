@@ -45,6 +45,13 @@ def bgzf_member(text):
             struct.pack("<II", zlib.crc32(text), len(text)))
 
 
+def bam_header():
+    """The BAM header of ``--bam`` files as one BGZF member: magic, the @HD and @PG lines, no reference sequences.  It
+    carries no command line, so the decompressed file depends only on the simulated reads."""
+    text = b"@HD\tVN:1.6\tSO:unknown\n@PG\tID:NanoSim\tPN:NanoSim\tVN:" + VERSION.encode() + b"\n"
+    return bgzf_member(b"BAM\1" + struct.pack("<i", len(text)) + text + struct.pack("<i", 0))
+
+
 def _log(msg):
     sys.stdout.write(strftime("%Y-%m-%d %H:%M:%S") + ": " + msg + "\n")
     sys.stdout.flush()
@@ -248,11 +255,12 @@ def _shard(n, rank, world):
 
 def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min_l, num_threads, fastq,
                median_l=None, sd_l=None, model_ir=False, uracil=False, polya=None, chimeric=False,
-               batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False, gzip_error_profile=False):
-    """gzip: write the reads as BGZF (``.gz``), compressed on the GPU; the error profile stays plain text unless
-    gzip_error_profile (needs gzip): then it is formatted and compressed on the GPU too, ``<out>_aligned_error_profile.gz``,
-    whose first member is the header line.  Under torchrun (world > 1) the per-rank files carry neither the header nor the
-    end-of-file block: merge_rank_files writes them."""
+               batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False, gzip_error_profile=False, bam=False):
+    """gzip: write the reads as BGZF (``.gz``), compressed on the GPU; bam: write them as unaligned BAM (``.bam``, one
+    unmapped record per read), encoded and compressed on the GPU.  The error profile stays plain text unless
+    gzip_error_profile (needs gzip or bam): then it is formatted and compressed on the GPU too,
+    ``<out>_aligned_error_profile.gz``, whose first member is the header line.  Under torchrun (world > 1) the per-rank
+    files carry neither the headers nor the end-of-file block: merge_rank_files writes them."""
     fmt_threads = max(1, min(num_threads, os.cpu_count() or 1))     # host threads of the record formatter
     eng = prof.engine
     meta = mode == "metagenome"
@@ -265,22 +273,25 @@ def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min
                   # the reference's 2-D KDE sample has one row per read of a WORKER (:1072): -t sets its size as it does there
                   kde2d_sample=max(1, (hi_a - lo_a) // max(1, num_threads)),
                   trx_records=prof.n_trx if (trx and prof.ir is not None) else 0)
-    ext = (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
+    ext = ".bam" if bam else (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
     suffix = "" if world == 1 else str(rank)
     want_err = error_profile and not per
-    gz_err = gzip and gzip_error_profile and want_err
-    pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err and not gz_err, compress_profile=gz_err)
+    gz_err = (gzip or bam) and gzip_error_profile and want_err
+    pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err and not gz_err, compress_profile=gz_err, bam=bam)
     totals = {"reads": 0, "bases": 0, "bytes": 0}
     try:
         _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                         gzip, gz_err)
+                         gzip, gz_err, bam)
     finally:
         pipe.close()         # the cloned contexts own device batch buffers and pinned staging
     return totals            # what this rank simulated and wrote (the reference returns nothing)
 
 
 def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                     gzip=False, gz_err=False):
+                     gzip=False, gz_err=False, bam=False):
+    packed = gzip or bam            # the records are compressed on the device: the batches arrive as BGZF members
+    reads_header = bam_header() if bam and world == 1 else b""
+
     def jobs(kind, lo, hi):
         return [(kind, start, min(batch_reads, hi - start)) for start in range(lo, hi, batch_reads)]
 
@@ -292,7 +303,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             view = view[w:]
 
     def put_reads(f, b, names):
-        if not gzip:
+        if not packed:
             f.pos += write_records(f.fd, f.pos, b, names, fastq, n_threads=fmt_threads)
             return
         put_members(f, b.gz)
@@ -302,7 +313,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             f.pos += os.pwrite(f.fd, BGZF_EOF, f.pos)
 
     def end_reads(f):
-        if gzip:
+        if packed:
             end_bgzf(f)
 
     class _Out:
@@ -319,7 +330,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
 
     _log("Start simulation of aligned reads")
     lo, hi = _shard(prof.number_aligned, rank, world)
-    f_reads = _Out(out + "_aligned_reads" + suffix + ext)
+    f_reads = _Out(out + "_aligned_reads" + suffix + ext, reads_header)
     f_err = _Out(out + ("_aligned_error_profile" if world == 1 else "_error_profile" + suffix) + (".gz" if gz_err else ""),
                  b"" if world > 1 else bgzf_member(ERR_HEADER) if gz_err else ERR_HEADER)
     try:
@@ -327,7 +338,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             return name_table(b, prof.ref.names, job[1], perfect=per, metagenome=meta, transcriptome=trx)
 
         def sink_aligned(info, b, job):
-            names = b.names if gzip else aligned_names(b, job)
+            names = b.names if packed else aligned_names(b, job)
             put_reads(f_reads, b, names)
             totals["reads"] += int(info.n_reads)
             totals["bases"] += int(info.total_bases)
@@ -344,7 +355,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             if patch is not None:
                 engine.reemit(*patch)
 
-        pipe.compress = aligned_names if gzip else None
+        pipe.compress = aligned_names if packed else None
         pipe.run(jobs(L.NS_KIND_ALIGNED, lo, hi), sink_aligned, static_assign=meta,
                  after_simulate=retain_introns if (trx and prof.ir is not None and not per) else None)
         end_reads(f_reads)
@@ -358,18 +369,18 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
         _log("Start simulation of random reads")
         lo, hi = _shard(prof.number_unaligned, rank, world)
         pipe.want_ops = pipe.compress_profile = False      # unaligned reads are not logged (:1482-1549)
-        f_un = _Out(out + "_unaligned_reads" + suffix + ext)
+        f_un = _Out(out + "_unaligned_reads" + suffix + ext, reads_header)
         try:
             def unaligned_names(b, job):
                 # the reference's read index keeps counting after the aligned reads (shared total_simulated, :1574)
                 return name_table(b, prof.ref.names, prof.number_aligned + job[1])
 
             def sink_unaligned(info, b, job):
-                put_reads(f_un, b, b.names if gzip else unaligned_names(b, job))
+                put_reads(f_un, b, b.names if packed else unaligned_names(b, job))
                 totals["reads"] += int(info.n_reads)
                 totals["bases"] += int(info.total_bases)
 
-            pipe.compress = unaligned_names if gzip else None
+            pipe.compress = unaligned_names if packed else None
             pipe.run(jobs(L.NS_KIND_UNALIGNED, lo, hi), sink_unaligned, static_assign=meta)
             end_reads(f_un)
         finally:
@@ -377,19 +388,21 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             f_un.close()
 
 
-def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=False):
+def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=False, bam=False):
     """Rank 0: concatenate per-rank sub-files in rank order and delete them (:1626-1639, :1667-1672).  gzip: the reads
-    files are BGZF members without an end-of-file block; the merged file gets it once, at its end.  gzip_error_profile: so
-    are the error-profile files (``_error_profile{r}.gz``); the merged one starts with the header line's member."""
-    ext = (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
-    trailer = BGZF_EOF if gzip else b""
-    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, b"", trailer)]
+    files are BGZF members without an end-of-file block; the merged file gets it once, at its end.  bam: so are the
+    ``.bam`` reads files, and the merged ones start with the BAM header's member.  gzip_error_profile: so are the
+    error-profile files (``_error_profile{r}.gz``); the merged one starts with the header line's member."""
+    ext = ".bam" if bam else (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
+    header = bam_header() if bam else b""
+    trailer = BGZF_EOF if gzip or bam else b""
+    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, header, trailer)]
     if gzip_error_profile:
         jobs.append(("_error_profile%d.gz", "_aligned_error_profile.gz", bgzf_member(ERR_HEADER), BGZF_EOF))
     else:
         jobs.append(("_error_profile%d", "_aligned_error_profile", ERR_HEADER, b""))
     if not per:
-        jobs.append(("_unaligned_reads%d" + ext, "_unaligned_reads" + ext, b"", trailer))
+        jobs.append(("_unaligned_reads%d" + ext, "_unaligned_reads" + ext, header, trailer))
     for pat, dst, header, end in jobs:
         with open(out + dst, "wb") as o:
             o.write(header)
@@ -408,8 +421,11 @@ def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=Fals
 GZIP_HELP = ('Write the reads as BGZF-compressed <out>_aligned_reads.fast{a,q}.gz and <out>_unaligned_reads.fast{a,q}.gz, '
              'compressed on the GPU (gzip, zcat and samtools read them). The error profile stays plain text unless '
              '--gzip_error_profile is given (Default = False)')
-GZIP_ERR_HELP = ('With --gzip: write the error profile as BGZF-compressed <out>_aligned_error_profile.gz, formatted and '
+GZIP_ERR_HELP = ('With --gzip or --bam: write the error profile as BGZF-compressed <out>_aligned_error_profile.gz, formatted and '
                  'compressed on the GPU (Default = False)')
+BAM_HELP = ('Write the reads as unaligned BAM, <out>_aligned_reads.bam and <out>_unaligned_reads.bam (one unmapped record per '
+            'read, as Dorado writes them), encoded and compressed on the GPU. The error profile stays plain text unless '
+            '--gzip_error_profile is given (Default = False)')
 
 
 def _plain_error_profile(args):
@@ -462,6 +478,7 @@ def build_parser():
     g.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
     g.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     g.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
+    g.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     mg = sub.add_parser('metagenome', help="Run the simulator on metagenome mode")
     mg.add_argument('-gl', '--genome_list', help="Reference metagenome list, tsv file, the first column is species/strain "
                     "name, the second column is the reference genome fasta/fastq file directory", required=True)
@@ -496,6 +513,7 @@ def build_parser():
     mg.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
     mg.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     mg.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
+    mg.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     t = sub.add_parser('transcriptome', help="Run the simulator on transcriptome mode")
     t.add_argument('-rt', '--ref_t', help='Input reference transcriptome', required=True)
     t.add_argument('-rg', '--ref_g', help='Input reference genome, required if intron retention simulation is on', default='')
@@ -536,6 +554,7 @@ def build_parser():
     t.add_argument('--device', help='CUDA device index (Default = LOCAL_RANK or 0)', type=int, default=None)
     t.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     t.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
+    t.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     return parser, g, mg, t
 
 
@@ -595,7 +614,7 @@ def main_transcriptome(args, parser_t):
     simulation(prof, "transcriptome", args.output, "transcriptome", args.perfect, args.KmerBias if args.homopolymer else None,
                args.basecaller, max_len, min_len, max(args.num_threads, 1), args.fastq, None, None, model_ir, args.uracil,
                args.polya, batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world,
-               gzip=args.gzip, gzip_error_profile=args.gzip_error_profile)
+               gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
@@ -603,7 +622,7 @@ def main_transcriptome(args, parser_t):
         dist.barrier()
         if rank == 0:
             merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip,
-                             gzip_error_profile=args.gzip_error_profile)
+                             gzip_error_profile=args.gzip_error_profile, bam=args.bam)
         dist.barrier()
     _log("Finished!")
 
@@ -662,7 +681,7 @@ def main_metagenome(args, parser_mg):
         simulation(prof, "metagenome", args.output + "_sample%d" % s_idx, "metagenome", args.perfect, None, None, max_len,
                    min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len, chimeric=args.chimeric,
                    batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world, gzip=args.gzip,
-                   gzip_error_profile=args.gzip_error_profile)
+                   gzip_error_profile=args.gzip_error_profile, bam=args.bam)
         if world > 1:
             import torch.distributed as dist
             if not dist.is_initialized():
@@ -670,7 +689,7 @@ def main_metagenome(args, parser_mg):
             dist.barrier()
             if rank == 0:
                 merge_rank_files(args.output + "_sample%d" % s_idx, args.fastq, args.perfect, world, gzip=args.gzip,
-                                 gzip_error_profile=args.gzip_error_profile)
+                                 gzip_error_profile=args.gzip_error_profile, bam=args.bam)
             dist.barrier()
     _log("Finished!")
 
@@ -693,8 +712,15 @@ def main(argv=None):
     if args.mode is None:
         parser.print_help(sys.stderr)
         sys.exit(1)
-    if args.gzip_error_profile and not args.gzip:
-        sys.stderr.write("\n--gzip_error_profile needs --gzip!\n")
+    usage = None
+    if args.bam and args.gzip:
+        usage = "--bam and --gzip both choose the format of the reads: give one of them"
+    elif args.bam and getattr(args, "uracil", False):
+        usage = "--bam cannot be combined with --uracil: BAM has no code for U"
+    elif args.gzip_error_profile and not (args.gzip or args.bam):
+        usage = "--gzip_error_profile needs --gzip or --bam"
+    if usage:
+        sys.stderr.write("\n" + usage + "!\n")
         {"genome": parser_g, "metagenome": parser_mg, "transcriptome": parser_t}[args.mode].print_help(sys.stderr)
         sys.exit(1)
     # no profile is written with --no_error_profile or --perfect: nothing to compress
@@ -748,7 +774,7 @@ def main(argv=None):
     simulation(prof, args.mode, args.output, args.dna_type, args.perfect, args.KmerBias if args.homopolymer else None,
                None, max_len, min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len,
                chimeric=args.chimeric, batch_reads=args.batch_reads, error_profile=not args.no_error_profile,
-               rank=rank, world=world, gzip=args.gzip, gzip_error_profile=args.gzip_error_profile)
+               rank=rank, world=world, gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
@@ -756,7 +782,7 @@ def main(argv=None):
         dist.barrier()
         if rank == 0:
             merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip,
-                             gzip_error_profile=args.gzip_error_profile)
+                             gzip_error_profile=args.gzip_error_profile, bam=args.bam)
         dist.barrier()
     _log("Finished!")
 
