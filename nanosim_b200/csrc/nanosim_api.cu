@@ -1283,10 +1283,10 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     pa.batch_reversed = batch_reversed;
     pa.abort = d_abort;
     const unsigned plan_tb = 128;
-    // 2 resident blocks per SM rather than 4 (the register limit): the kernel is bound by the latency of its table lookups,
-    // and another context's emit kernel still finds room on every SM (transcripts are short -- 1-2 kb reads, no long tail,
-    // two passes: there the register limit of 4 blocks is used).  NANOSIM_B200_PLAN_BLOCKS_PER_SM overrides the cap.
-    // DESIGN.md §10 has the H100 comparison.
+    // 2 resident blocks per SM rather than 4 (the register limit): the lanes' scattered memory accesses (script stores,
+    // alias loads) share one memory pipeline, which more warps only queue on, and another context's emit kernel still
+    // finds room on every SM (transcripts are short -- 1-2 kb reads, no long tail, two passes: there the register limit
+    // of 4 blocks is used).  NANOSIM_B200_PLAN_BLOCKS_PER_SM overrides the cap.  DESIGN.md §10 has the H100 sweep.
     static const int plan_per_sm_env = env_int("NANOSIM_B200_PLAN_BLOCKS_PER_SM", 0);
     const int plan_per_sm = plan_per_sm_env > 0 ? plan_per_sm_env : (ctx->dcfg.transcriptome ? 4 : 2);
     unsigned plan_blocks = std::min<unsigned>((n + plan_tb - 1) / plan_tb, (unsigned)ctx->sm_count * (unsigned)std::max(1, plan_per_sm));

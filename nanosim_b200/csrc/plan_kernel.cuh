@@ -42,11 +42,18 @@ struct PlanArgs {
 
 enum Phase : int { PH_FETCH = 0, PH_LEN, PH_ATT, PH_PIECE, PH_EVENT, PH_UEVENT, PH_PIECE_END, PH_CHECK, PH_DONE };
 
-template <bool WRITE>
+// VEC (first pass): slots are whole groups of 4 ops (lengths_kernel), 16-byte aligned, and each group goes out as ONE
+// 16-byte store once it is full (finish() writes a partial last group).  The lanes of a warp write to 32 different slots,
+// so a 4-byte store per op costs a memory transaction per op; a group costs one per 4 ops.  A group is written only when it
+// lies wholly inside the slot; `n` keeps counting past `cap` (the read is then flagged and replayed).
+// !VEC (replay): exact, unaligned slots, one 4-byte store per op.
+template <bool VEC>
 struct OpSink {
-    uint32_t* base;       // start of this piece's op slot (WRITE)
-    uint32_t cap;         // slot capacity in ops
+    uint32_t* base;       // start of this piece's op slot
+    uint32_t cap;         // slot capacity in ops (VEC: a multiple of 4)
     uint32_t n;           // ops emitted so far (flushed)
+    uint32_t n0;          // VEC: ops [0, n0) were written by another kernel (gap_kernel) and are not in `grp`
+    uint4 grp;            // VEC: the open group, ops 4 * (n / 4) .. n - 1
     uint32_t pend_type;   // pending (mergeable) op
     uint32_t pend_len;
     uint32_t out_len;     // bases produced by flushed + pending ops
@@ -54,15 +61,38 @@ struct OpSink {
         base = slot;
         cap = capacity;
         n = 0;
+        n0 = 0;
         pend_type = 0xffffffffu;
         pend_len = 0;
         out_len = 0;
     }
-    __device__ __forceinline__ void flush() {
-        if (pend_type != 0xffffffffu && pend_len > 0) {
-            if (WRITE && n < cap) base[n] = (pend_type << 28) | pend_len;
-            ++n;
+    __device__ __forceinline__ void set_word(uint32_t k, uint32_t w) {
+        grp.x = k == 0 ? w : grp.x;
+        grp.y = k == 1 ? w : grp.y;
+        grp.z = k == 2 ? w : grp.z;
+        grp.w = k == 3 ? w : grp.w;
+    }
+    __device__ __forceinline__ void emit(uint32_t w) {
+        if (VEC) {
+            set_word(n & 3u, w);
+            if ((n & 3u) == 3u && n < cap) *reinterpret_cast<uint4*>(base + (n - 3u)) = grp;
+        } else if (n < cap) {
+            base[n] = w;
         }
+        ++n;
+    }
+    // VEC: write the open, partial group (where it is inside the slot)
+    __device__ __forceinline__ void finish() {
+        if (!VEC) return;
+        const uint32_t g = n & ~3u;
+        if (g >= cap) return;
+        const uint32_t w[4] = {grp.x, grp.y, grp.z, grp.w};
+#pragma unroll
+        for (uint32_t k = 0; k < 3; ++k)
+            if (g + k < n && g + k >= n0) base[g + k] = w[k];
+    }
+    __device__ __forceinline__ void flush() {
+        if (pend_type != 0xffffffffu && pend_len > 0) emit((pend_type << 28) | pend_len);
         pend_type = 0xffffffffu;
         pend_len = 0;
     }
@@ -82,20 +112,20 @@ struct OpSink {
     __device__ __forceinline__ void put(uint32_t type, uint32_t len) {
         if (len == 0) return;
         if (type != NS_OP_DEL) out_len += len;
-        if (WRITE && n < cap) base[n] = (type << 28) | len;
-        ++n;
+        emit((type << 28) | len);
     }
     // literal run (polyA): `len` copies of base index `base` with quality state `state`
     __device__ __forceinline__ void put_lit(uint32_t base_idx, uint32_t state, uint32_t len) {
         if (len == 0) return;
         out_len += len;
-        if (WRITE && n < cap) base[n] = (NS_OP_LIT << 28) | (base_idx << 26) | (state << 24) | len;
-        ++n;
+        emit((NS_OP_LIT << 28) | (base_idx << 26) | (state << 24) | len);
     }
     // the reference's e_dict[pos - 0.5] overwrite: a second insertion at the same position replaces the first (:1882)
     __device__ __forceinline__ void replace_last_ins(uint32_t old_len, uint32_t len) {
         out_len = out_len - old_len + len;
-        if (WRITE && n - 1 < cap) base[n - 1] = (NS_OP_INS << 28) | len;
+        const uint32_t i = n - 1, w = (NS_OP_INS << 28) | len;
+        if (VEC && (i & 3u) != 3u) set_word(i & 3u, w);     // still in the open group
+        else if (i < cap) base[i] = w;                      // its group was already written
     }
 };
 
@@ -342,7 +372,7 @@ __global__ void lengths_kernel(DevModel m, DevCfg cfg, uint32_t kind, uint64_t f
                 float e = (float)len * ev_per_base;
                 cap = (uint64_t)(2.0f * (e + 6.0f * ev_cv * sqrtf(e) + 8.0f)) + 4;
             }
-            caps[pf + q] = exact_only ? 0 : cap;
+            caps[pf + q] = exact_only ? 0 : (cap + 3) & ~3ull;          // whole 16-byte groups (OpSink<true>)
         }
     } else if (exact_only) {
         caps[pf] = 0;                                                    // scripted unaligned reads: exact pass only
@@ -399,7 +429,7 @@ __global__ void __launch_bounds__(128, PLAN_MIN_BLOCKS) plan_kernel(const __grid
     uint32_t gap_sw = 0, gap_draw = 0;   // chimeric gap / segment chain: its own stream (a gap's is shared with gap_kernel), draw k = Philox block k + 1
     bool last_op_was_ins_same_pos = false;
     uint32_t last_ins_len = 0;
-    OpSink<true> sink;
+    OpSink<!REPLAY> sink;
     sink.begin(nullptr, 0);
     bool overflow = false;
 
@@ -530,7 +560,7 @@ __global__ void __launch_bounds__(128, PLAN_MIN_BLOCKS) plan_kernel(const __grid
                 gap_draw = 0;
                 if (!REPLAY && attempt == 0 && pm.polya_len == 1u) {
                     pm.polya_len = 0;
-                    sink.n = pm.n_ops;
+                    sink.n = sink.n0 = pm.n_ops;        // no op follows: a gap gets no head or tail
                     sink.out_len = pm.out_len;
                     middle_ref = pm.ref_len;
                     l_new = (int64_t)pm.out_len;
@@ -671,6 +701,7 @@ __global__ void __launch_bounds__(128, PLAN_MIN_BLOCKS) plan_kernel(const __grid
             } else if (!unal_kind && p + 1 == n_pieces && tail > 0) {
                 sink.put(NS_OP_HT, tail);
             }
+            sink.finish();
             if (!REPLAY) {
                 if (sink.n > sink.cap) overflow = true;
                 pm.n_ops = sink.n;
@@ -722,6 +753,7 @@ __global__ void __launch_bounds__(128, PLAN_MIN_BLOCKS) plan_kernel(const __grid
                 }
                 sink.put_lit(0u, 3u, polya_len);
                 sink.put(NS_OP_HT, tail);
+                sink.finish();
                 if (sink.n > sink.cap) overflow = true;
                 pm.pos = ppos;
                 pm.polya_len = polya_len;
