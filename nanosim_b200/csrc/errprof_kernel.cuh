@@ -1,6 +1,6 @@
 // Error-profile rows on the device (ns_compress_error_profile): the bytes host_io.cu:format_error_profile_impl writes for
 // the last aligned batch (after ns_reemit as well), without the header line, laid out in HBM for
-// bgzf_deflate_rows_kernel.  One warp per read.  A read's rows go per mutate_read call -- a segment plus the
+// bgzf_deflate_kernel<BgzfRows>.  One warp per read.  A read's rows go per mutate_read call -- a segment plus the
 // NS_PIECE_CONT pieces that continue it -- and within a call right to left, with Seq_pos counted across the call's
 // pieces.  The rows come from the event scripts (ev_off / ev_n_ops), 32 ops at a time: warp scans give every op its
 // reference and read offsets and every event its row's size and place; the lane of an event writes its row.

@@ -1539,8 +1539,9 @@ static int pack_members(NsContext* ctx, const char* fname, uint32_t n_blocks, De
     return NS_OK;
 }
 
-// staging of n_blocks members of `text` bytes of text; NS_EINVAL when that is too much for one call
-static int stage_members(NsContext* ctx, const char* fname, uint64_t text, uint32_t* n_blocks) {
+// staging of the members of `text` bytes of text, where bgzf_deflate_kernel leaves them; NS_EINVAL when that is too
+// much for one call
+static int stage_members(NsContext* ctx, const char* fname, uint64_t text, BgzfMembers* zm, uint32_t* n_blocks) {
     const uint64_t n_blocks64 = (text + BGZF_BLOCK - 1) / BGZF_BLOCK;
     if (n_blocks64 > 0x7fffffffu) return fail(ctx, NS_EINVAL, "%s: %llu bytes of text is too much for one call", fname,
                                               (unsigned long long)text);
@@ -1549,6 +1550,11 @@ static int stage_members(NsContext* ctx, const char* fname, uint64_t text, uint3
     CK(ctx->z_msize.ensure((size_t)*n_blocks * sizeof(uint64_t)));
     CK(ctx->z_moff.ensure((size_t)*n_blocks * sizeof(uint64_t)));
     CK(ctx->z_trailer.ensure((size_t)*n_blocks * sizeof(uint2)));
+    zm->text_bytes = text;
+    zm->stage = ctx->z_stage.as<uint8_t>();
+    zm->member_size = ctx->z_msize.as<uint64_t>();
+    zm->trailer = ctx->z_trailer.as<uint2>();
+    zm->oversize = (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_OVERSIZE);
     return NS_OK;
 }
 
@@ -1564,10 +1570,21 @@ static int fetch_members(NsContext* ctx, const char* fname, bool have, const Dev
     return NS_OK;
 }
 
+extern "C++" {    // templates cannot have C linkage
+
+// the n_blocks members of the text `src` brings into shared memory
+template <class Source>
+static int deflate_members(NsContext* ctx, const Source& src, const BgzfMembers& zm, uint32_t n_blocks) {
+    const int smem = (int)sizeof(typename Source::Smem);
+    CK(cudaFuncSetAttribute(bgzf_deflate_kernel<Source>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CK(launch(ctx, bgzf_deflate_kernel<Source>, n_blocks, BGZF_THREADS, (size_t)smem, src, zm));
+    return NS_OK;
+}
+
 // ns_compress_records (FASTA/FASTQ text) and ns_compress_bam (BAM records): the last batch's records in that layout as
 // BGZF members in z_out
-static int compress_records(NsContext* ctx, const char* fname, bool bam, const char* names, const uint64_t* name_off,
-                            uint64_t* nbytes) {
+template <class Layout>
+static int compress_records(NsContext* ctx, const char* fname, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
     if (!ctx) return NS_EINVAL;
     if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
     if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
@@ -1582,15 +1599,10 @@ static int compress_records(NsContext* ctx, const char* fname, bool bam, const c
         return NS_OK;
     }
     if (int rc = upload_names(ctx, names, name_off, n)) return rc;
-    uint64_t* totals = ctx->totals.as<uint64_t>();
     const uint32_t fastq = ctx->hcfg.fastq ? 1u : 0u;
-    if (bam)
-        CK(launch(ctx, bam_record_size, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
-                  ctx->z_name_off.as<uint64_t>(), ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>(),
-                  (unsigned long long*)(totals + NS_T_Z_LONG_NAMES)));
-    else
-        CK(launch(ctx, bgzf_record_size, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
-                  ctx->z_name_off.as<uint64_t>(), fastq, ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>()));
+    CK(launch(ctx, record_size_kernel<Layout>, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
+              ctx->z_name_off.as<uint64_t>(), fastq, ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>(),
+              (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_LONG_NAMES)));
     if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->z_rec_off.as<uint64_t>(), n, NS_T_Z_TEXT)) return rc;
     if (int rc = publish_totals_and_wait(ctx)) return rc;
     if (const uint64_t n_long = ctx->h_totals.as<uint64_t>()[NS_T_Z_LONG_NAMES]) {
@@ -1600,26 +1612,20 @@ static int compress_records(NsContext* ctx, const char* fname, bool bam, const c
                     strlen(names + name_off[i]), BAM_MAX_NAME, (unsigned long long)n_long);
     }
     const uint64_t text = ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT];
+    BgzfMembers zm;
     uint32_t n_blocks = 0;
-    if (int rc = stage_members(ctx, fname, text, &n_blocks)) return rc;
-    BgzfArgs za;
-    za.reads = ctx->reads.as<NsReadMeta>();
-    za.seq = ctx->seq.as<uint8_t>();
-    za.qual = fastq ? ctx->qual.as<uint8_t>() : nullptr;
-    za.names = ctx->z_names.as<char>();
-    za.name_off = ctx->z_name_off.as<uint64_t>();
-    za.name_len = ctx->z_name_len.as<uint32_t>();
-    za.rec_off = ctx->z_rec_off.as<uint64_t>();
-    za.n_reads = n;
-    za.fastq = fastq;
-    za.text_bytes = text;
-    za.stage = ctx->z_stage.as<uint8_t>();
-    za.member_size = ctx->z_msize.as<uint64_t>();
-    za.trailer = ctx->z_trailer.as<uint2>();
-    za.oversize = (unsigned long long*)(totals + NS_T_Z_OVERSIZE);
-    void (*deflate)(BgzfArgs) = bam ? bgzf_deflate_kernel<BgzfBamLayout> : bgzf_deflate_kernel<BgzfTextLayout>;
-    CK(cudaFuncSetAttribute(deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BgzfSmem)));
-    CK(launch(ctx, deflate, n_blocks, BGZF_THREADS, sizeof(BgzfSmem), za));
+    if (int rc = stage_members(ctx, fname, text, &zm, &n_blocks)) return rc;
+    BgzfRecords<Layout> src;
+    src.reads = ctx->reads.as<NsReadMeta>();
+    src.seq = ctx->seq.as<uint8_t>();
+    src.qual = fastq ? ctx->qual.as<uint8_t>() : nullptr;
+    src.names = ctx->z_names.as<char>();
+    src.name_off = ctx->z_name_off.as<uint64_t>();
+    src.name_len = ctx->z_name_len.as<uint32_t>();
+    src.rec_off = ctx->z_rec_off.as<uint64_t>();
+    src.n_reads = n;
+    src.fastq = fastq;
+    if (int rc = deflate_members(ctx, src, zm, n_blocks)) return rc;
     uint64_t total = 0;
     if (int rc = pack_members(ctx, fname, n_blocks, ctx->z_out, &total)) return rc;
     ctx->z_bytes = total;
@@ -1628,12 +1634,14 @@ static int compress_records(NsContext* ctx, const char* fname, bool bam, const c
     return NS_OK;
 }
 
+}  // extern "C++"
+
 int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
-    return compress_records(ctx, "ns_compress_records", false, names, name_off, nbytes);
+    return compress_records<BgzfTextLayout>(ctx, "ns_compress_records", names, name_off, nbytes);
 }
 
 int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
-    return compress_records(ctx, "ns_compress_bam", true, names, name_off, nbytes);
+    return compress_records<BgzfBamLayout>(ctx, "ns_compress_bam", names, name_off, nbytes);
 }
 
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap) {
@@ -1684,20 +1692,15 @@ int ns_compress_error_profile(NsContext* ctx, const char* names, const uint64_t*
         *nbytes = 0;
         return NS_OK;
     }
+    BgzfMembers zm;
     uint32_t n_blocks = 0;
-    if (int rc = stage_members(ctx, fname, text, &n_blocks)) return rc;
+    if (int rc = stage_members(ctx, fname, text, &zm, &n_blocks)) return rc;
     CK(ctx->ep_text.ensure((size_t)text));
     ea.text = ctx->ep_text.as<uint8_t>();
     CK(launch(ctx, errprof_write_kernel, warps_grid, 256, 0, ea));
-    BgzfRowsArgs za;
-    za.text = ctx->ep_text.as<uint8_t>();
-    za.text_bytes = text;
-    za.stage = ctx->z_stage.as<uint8_t>();
-    za.member_size = ctx->z_msize.as<uint64_t>();
-    za.trailer = ctx->z_trailer.as<uint2>();
-    za.oversize = (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_OVERSIZE);
-    CK(cudaFuncSetAttribute(bgzf_deflate_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BgzfRowsSmem)));
-    CK(launch(ctx, bgzf_deflate_rows_kernel, n_blocks, BGZF_THREADS, sizeof(BgzfRowsSmem), za));
+    BgzfRows src;
+    src.text = ctx->ep_text.as<uint8_t>();
+    if (int rc = deflate_members(ctx, src, zm, n_blocks)) return rc;
     uint64_t total = 0;
     if (int rc = pack_members(ctx, fname, n_blocks, ctx->ep_out, &total)) return rc;
     ctx->ep_bytes = total;
