@@ -233,6 +233,29 @@ int ns_clone(NsContext* parent, NsContext** out);
 /* --- read_profile() (:244-591): reference + model tables into HBM, once ------------------------------------- */
 int ns_set_reference(NsContext* ctx, const NsReference* ref);
 int ns_set_model(NsContext* ctx, const NsModel* model);
+/* genome --vcf: the haplotype records of a VCF sample (nanosim_b200/variants.py builds these tables).  Haplotype h copies
+ * record hap_chrom[h] of the resident reference with variants var_off[h] .. var_off[h+1]-1 applied, in position order:
+ * the span [var_pos, var_pos + var_ref_len) of that record is replaced by alt[alt_off .. alt_off + alt_len).  Spans of one
+ * haplotype may touch but not overlap.  Host pointers. */
+typedef struct {
+    uint32_t n_hap;
+    const uint32_t* hap_chrom;       /* n_hap */
+    const uint64_t* var_off;         /* n_hap + 1 */
+    uint64_t n_var;
+    const uint64_t* var_pos;         /* n_var, 0-based in the source record */
+    const uint32_t* var_ref_len;
+    const uint64_t* alt_off;
+    const uint32_t* alt_len;
+    const uint8_t* alt;
+    uint64_t alt_bytes;
+    uint64_t* peak_bytes;            /* out, may be NULL: accounted peak -- the sizes of the library's allocations (reference and build) at the build's high
+                                        point, not a device reading */
+} NsVariants;
+/* Builds the haplotypes in HBM from the resident reference and makes them the resident reference, record h being
+ * haplotype h (what ns_set_reference does with them: 2-bit copy, chromosome checks); the haploid bytes are freed.  Call
+ * after ns_set_reference (or ns_bcast_nccl) and before ns_clone; NS_ESTATE on a clone.  Genome references only. */
+int ns_apply_variants(NsContext* ctx, const NsVariants* variants);
+
 int ns_configure(NsContext* ctx, const NsRunConfig* cfg);
 /* metagenome: dict_abun / dict_abun_inflated of the current sample (main() :2497-2514), one value per species in
  * genome-list order; resets the running per-species base counts that assign_species (:758-811) keeps per worker. */

@@ -24,12 +24,18 @@ NS_STATS_WORDS = NS_STATS_COMP_OFF + 4
 
 EXPORTS = ["ns_create", "ns_destroy", "ns_last_error", "ns_clone", "ns_set_abundance", "ns_set_expression", "ns_set_reference", "ns_set_model", "ns_configure",
            "ns_simulate", "ns_fetch", "ns_reemit", "ns_batch_info", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases",
-           "ns_compress_records", "ns_fetch_compressed", "ns_compress_error_profile", "ns_fetch_compressed_error_profile", "ns_compress_bam"]
+           "ns_compress_records", "ns_fetch_compressed", "ns_compress_error_profile", "ns_fetch_compressed_error_profile", "ns_compress_bam", "ns_apply_variants"]
 
 
 class NsReference(C.Structure):
     _fields_ = [("bases", C.c_void_p), ("n_bases", C.c_uint64), ("chrom_off", C.c_void_p), ("n_chrom", C.c_uint32),
                 ("n_species", C.c_uint32), ("chrom_species", C.c_void_p), ("chrom_circular", C.c_void_p)]
+
+
+class NsVariants(C.Structure):
+    _fields_ = [("n_hap", C.c_uint32), ("hap_chrom", C.c_void_p), ("var_off", C.c_void_p), ("n_var", C.c_uint64),
+                ("var_pos", C.c_void_p), ("var_ref_len", C.c_void_p), ("alt_off", C.c_void_p), ("alt_len", C.c_void_p),
+                ("alt", C.c_void_p), ("alt_bytes", C.c_uint64), ("peak_bytes", C.POINTER(C.c_uint64))]
 
 
 class NsKde(C.Structure):
@@ -128,6 +134,8 @@ def lib():
     L.ns_last_error.restype = C.c_char_p
     L.ns_set_reference.argtypes = [P, C.POINTER(NsReference)]
     L.ns_set_reference.restype = C.c_int
+    L.ns_apply_variants.argtypes = [P, C.POINTER(NsVariants)]
+    L.ns_apply_variants.restype = C.c_int
     L.ns_set_model.argtypes = [P, C.POINTER(NsModel)]
     L.ns_set_model.restype = C.c_int
     L.ns_set_abundance.argtypes = [P, P, P, C.c_uint32]

@@ -29,6 +29,7 @@
 #include "hp_kernel.cuh"
 #include "bgzf_kernel.cuh"
 #include "errprof_kernel.cuh"
+#include "haplotype.h"
 #include "host_io.h"
 
 namespace {
@@ -68,6 +69,11 @@ struct DevBuf {
         p = np;
         cap = want;
         return e;
+    }
+    void release() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
     }
     template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
@@ -795,6 +801,82 @@ int ns_set_reference(NsContext* ctx, const NsReference* ref) {
     tab.have_ref = true;
     ctx->have_batch = false;
     ctx->opt_ok[0] = ctx->opt_ok[1] = false;
+    return NS_OK;
+}
+
+int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
+    if (!ctx || !v || !v->hap_chrom || !v->var_off || v->n_hap == 0 ||
+        (v->n_var && (!v->var_pos || !v->var_ref_len || !v->alt_off || !v->alt_len)) || (v->alt_bytes && !v->alt))
+        return fail(ctx, NS_EINVAL, "ns_apply_variants: null argument or no haplotype");
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "ns_apply_variants: a cloned context shares its parent's reference");
+    Tables& tab = *ctx->tables;
+    if (!tab.have_ref) return fail(ctx, NS_ESTATE, "ns_apply_variants: set the reference first (ns_set_reference or ns_bcast_nccl)");
+    if (tab.dref.n_species) return fail(ctx, NS_EINVAL, "ns_apply_variants: a metagenome reference cannot carry variants");
+    const uint32_t n_chrom = tab.dref.n_chrom;
+    const std::vector<uint64_t>& off = tab.h_chrom_off;
+    if (v->var_off[0] != 0 || v->var_off[v->n_hap] != v->n_var)
+        return fail(ctx, NS_EINVAL, "ns_apply_variants: var_off must start at 0 and end at n_var");
+    for (uint32_t h = 0; h < v->n_hap; ++h) {
+        const uint32_t c = v->hap_chrom[h];
+        if (c >= n_chrom) return fail(ctx, NS_EINVAL, "ns_apply_variants: haplotype %u names record %u of %u", h, c, n_chrom);
+        if (v->var_off[h + 1] < v->var_off[h]) return fail(ctx, NS_EINVAL, "ns_apply_variants: var_off decreases at haplotype %u", h);
+        uint64_t end = 0;
+        for (uint64_t j = v->var_off[h]; j < v->var_off[h + 1]; ++j) {
+            if (v->var_pos[j] < end || v->var_pos[j] + v->var_ref_len[j] > off[c + 1] - off[c] || v->alt_off[j] + v->alt_len[j] > v->alt_bytes)
+                return fail(ctx, NS_EINVAL, "ns_apply_variants: variant %llu of haplotype %u overlaps the one before it or lies outside "
+                            "its record or the ALT bytes", (unsigned long long)j, h);
+            end = v->var_pos[j] + v->var_ref_len[j];
+        }
+    }
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    const uint64_t n_seg = 2 * v->n_var + v->n_hap;
+    DevBuf hap_chrom, var_off, var_pos, var_ref_len, alt_off, alt_len, alt, seg_src, seg_len, seg_out, hap_off, out;
+    CK(upload(hap_chrom, v->hap_chrom, (size_t)v->n_hap * 4, st));
+    CK(upload(var_off, v->var_off, (size_t)(v->n_hap + 1) * 8, st));
+    CK(upload(var_pos, v->var_pos, v->n_var * 8, st));
+    CK(upload(var_ref_len, v->var_ref_len, v->n_var * 4, st));
+    CK(upload(alt_off, v->alt_off, v->n_var * 8, st));
+    CK(upload(alt_len, v->alt_len, v->n_var * 4, st));
+    CK(alt.ensure(v->alt_bytes + 16));                              // hap_gather_kernel reads whole words behind the end
+    if (v->alt_bytes) CK(cudaMemcpyAsync(alt.p, v->alt, v->alt_bytes, cudaMemcpyHostToDevice, st));
+    CK(seg_src.ensure(n_seg * 8));
+    CK(seg_len.ensure((n_seg + 1) * 8));
+    CK(seg_out.ensure((n_seg + 1) * 8));
+    CK(hap_off.ensure((size_t)(v->n_hap + 1) * 8));
+    HapArgs a{hap_chrom.as<uint32_t>(), var_off.as<uint64_t>(), var_pos.as<uint64_t>(), var_ref_len.as<uint32_t>(),
+              alt_off.as<uint64_t>(), alt_len.as<uint32_t>(), tab.dref.chrom_off, v->n_hap, n_seg, seg_src.as<uint64_t>(),
+              seg_len.as<uint64_t>()};
+    size_t tmp = 0;
+    CK(hap_layout(a, seg_out.as<uint64_t>(), hap_off.as<uint64_t>(), nullptr, &tmp, st));
+    CK(ctx->scan_tmp.ensure(tmp));
+    CK(hap_layout(a, seg_out.as<uint64_t>(), hap_off.as<uint64_t>(), ctx->scan_tmp.p, &tmp, st));
+    uint64_t n_bases = 0;
+    CK(cudaMemcpyAsync(&n_bases, seg_out.as<uint64_t>() + n_seg, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (n_bases == 0) return fail(ctx, NS_EINVAL, "ns_apply_variants: the haplotypes have no bases");
+    CK(out.ensure(n_bases + 16));
+    CK(hap_gather(tab.dref.bases, alt.as<uint8_t>(), seg_src.as<uint64_t>(), seg_out.as<uint64_t>(), n_seg, n_bases, out.as<uint8_t>(), st));
+    CK(cudaStreamSynchronize(st));
+    // accounted peak (sizes of the library's allocations, not a device reading) at the two high points: the haploid
+    // reference beside the haplotypes, then the new resident copy (ns_set_reference's) beside them; the build's tables
+    // and the scan's scratch space are held throughout
+    const size_t build = hap_chrom.cap + var_off.cap + var_pos.cap + var_ref_len.cap + alt_off.cap + alt_len.cap + alt.cap +
+                         seg_src.cap + seg_len.cap + seg_out.cap + hap_off.cap + out.cap + ctx->scan_tmp.cap;
+    const size_t peak_a = build + tab.ref_bases.cap + tab.ref_off.cap + tab.ref_packed.cap + tab.ref_pk_off.cap + tab.ref_exc.cap;
+    // the haploid bytes and their 2-bit copy go before ns_set_reference allocates the haplotypes' own
+    tab.have_ref = false;
+    tab.ref_bases.release();
+    tab.ref_packed.release();
+    NsReference r{};
+    r.bases = out.as<uint8_t>();                    // device pointers: ns_set_reference copies from them
+    r.n_bases = n_bases;
+    r.chrom_off = hap_off.as<uint64_t>();
+    r.n_chrom = v->n_hap;
+    const int rc = ns_set_reference(ctx, &r);
+    if (rc != NS_OK) return rc;
+    const size_t peak_b = build + tab.ref_bases.cap + tab.ref_off.cap + tab.ref_packed.cap + tab.ref_pk_off.cap + tab.ref_exc.cap;
+    if (v->peak_bytes) *v->peak_bytes = std::max(peak_a, peak_b);
     return NS_OK;
 }
 

@@ -89,6 +89,17 @@ class Engine:
             r = L.NsReference(_ptr(ref.bases), ref.genome_len, _ptr(ref.offsets), len(ref.names), 0, None, None)
         self._check(self._lib.ns_set_reference(self._ctx, C.byref(r)))
 
+    def apply_variants(self, tables):
+        """genome --vcf: replaces the resident reference with the haplotype records of ``tables`` (a
+        variants.HaplotypeTables over it), built in HBM (ns_apply_variants).  Returns the device memory the reference and
+        the build held at the build's peak, in bytes."""
+        t = tables
+        peak = C.c_uint64()
+        v = L.NsVariants(len(t.hap_chrom), _ptr(t.hap_chrom), _ptr(t.var_off), len(t.var_pos), _ptr(t.var_pos), _ptr(t.var_ref_len),
+                         _ptr(t.alt_off), _ptr(t.alt_len), _ptr(t.alt), len(t.alt), C.pointer(peak))
+        self._check(self._lib.ns_apply_variants(self._ctx, C.byref(v)))
+        return int(peak.value)
+
     def set_abundance(self, abun, inflated=None):
         """dict_abun / dict_abun_inflated of one sample, per species in genome-list order (metagenome mode)."""
         a = np.ascontiguousarray(abun, dtype=np.float64)

@@ -68,6 +68,7 @@ class Profile:
         self.number_unaligned = 0
         self.max_chrom = 0
         self.perfect = False
+        self.haplotypes = None      # genome --vcf: variants.HaplotypeTables
 
 
 def _dist_world():
@@ -82,7 +83,8 @@ def _dist_init():
 
 
 class _RemoteReference(PackedReference):
-    """The reference as a rank other than 0 sees it before the broadcast: names and offsets, no bases yet."""
+    """A reference whose bases are in HBM only: names and offsets.  What a rank other than 0 sees before the broadcast,
+    and the haplotype records of ``--vcf``, which are built on the device."""
 
     def __init__(self, names, offsets, raw_names):
         self.names, self.raw_names = list(names), list(raw_names)
@@ -92,27 +94,46 @@ class _RemoteReference(PackedReference):
 
 def read_profile(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                  polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                 device=0, seed=0, ir_files=None, ref_on_host=True):
+                 device=0, seed=0, ir_files=None, ref_on_host=True, vcf=None):
     """read_profile (:244-591).  Under torchrun (WORLD_SIZE > 1) only rank 0 reads the reference files; the other ranks get
     names and offsets through torch.distributed and the bases through ONE NCCL broadcast into their HBM (ns_bcast_nccl).
-    ref_on_host: those ranks also copy the bases back to the host, which only the plain error profile's formatter reads."""
+    ref_on_host: those ranks also copy the bases back to the host, which only the plain error profile's formatter reads.
+    vcf (genome mode): the reads come from the haplotypes of the VCF's first sample.  Rank 0 parses it and hands the
+    tables to the other ranks; every rank builds the haplotypes in its HBM from the haploid reference (ns_apply_variants),
+    and with ref_on_host copies them back to the host."""
     rank, world = _dist_world()
     if world > 1:
         return _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun,
-                                         polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host)
-    return _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
-                               chimeric, homopolymer, fastq, device, seed, ir_files)
+                                         polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host, vcf)
+    prof = _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
+                               chimeric, homopolymer, fastq, device, seed, ir_files, vcf)
+    if prof.haplotypes is not None:
+        _apply_variants(prof, prof.haplotypes, ref_on_host)
+    return prof
+
+
+def _apply_variants(prof, tables, ref_on_host):
+    """Makes the haplotype records of ``tables`` the resident reference of prof.engine (built on the device)."""
+    prof.engine.apply_variants(tables)
+    prof.ref = _RemoteReference(tables.names, tables.offsets, tables.names)
+    if ref_on_host:
+        prof.ref.bases = prof.engine.reference_bases(prof.ref.genome_len)
+    prof.engine.ref = prof.ref
+    for name, n, skipped in zip(tables.names, tables.applied, tables.skipped):
+        _log("%s: %d variants applied, %d records of its chromosome skipped by FILTER" % (name, n, skipped))
+    if tables.skipped_elsewhere:
+        _log("%d records on contigs that are not in the reference skipped by FILTER" % tables.skipped_elsewhere)
 
 
 def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp,
-                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True):
+                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True, vcf=None):
     dist = _dist_init()
     box = [None]
     if rank == 0:
         prof = _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
-                                   chimeric, homopolymer, fastq, device, seed, ir_files)
+                                   chimeric, homopolymer, fastq, device, seed, ir_files, vcf)
         r = prof.ref
-        box[0] = {"names": r.names, "raw": r.raw_names, "offsets": r.offsets,
+        box[0] = {"names": r.names, "raw": r.raw_names, "offsets": r.offsets, "haplotypes": prof.haplotypes,
                   "meta": (r.species, r.chrom_species, r.chrom_circular, r.chrom_keys) if mode == "metagenome" else None,
                   "nccl_id": prof.engine.nccl_unique_id(),
                   "extra": {k: getattr(prof, k) for k in ("samples", "number_list", "expr_chrom", "expr_weights", "polya_flags", "max_chrom",
@@ -149,8 +170,10 @@ def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per
         bind_to_gpu_node(device)
         prof.engine = Engine(device=device, seed=seed)
     prof.engine.bcast_reference(info["nccl_id"], rank, world, 0)          # the one NCCL broadcast of the job
+    if info["haplotypes"] is not None:
+        _apply_variants(prof, info["haplotypes"], ref_on_host)
     if rank != 0:
-        if ref_on_host:
+        if ref_on_host and info["haplotypes"] is None:
             prof.ref.bases = prof.engine.reference_bases(int(prof.ref.offsets[-1]))   # host copy for the error profile's reference column
         prof.engine.ref = prof.ref
         prof.engine.set_model(prof.tables, perfect=per)
@@ -162,7 +185,7 @@ def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per
 
 def _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                         polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                        device=0, seed=0, ir_files=None):
+                        device=0, seed=0, ir_files=None, vcf=None):
     prof = Profile()
     prof.ir = None
     prof.n_trx = 0
@@ -222,6 +245,16 @@ def _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness,
         prof.ref = PackedReference.from_fasta(ref_g)
     if mode != "transcriptome":
         prof.max_chrom = prof.ref.max_chrom
+    if vcf:
+        from .variants import VcfError, read_vcf
+        _log("Read in VCF")
+        try:
+            prof.haplotypes = read_vcf(vcf, prof.ref)
+        except VcfError as e:
+            sys.stderr.write("%s: %s\n" % (vcf, e))
+            sys.exit(1)
+        prof.max_chrom = int(prof.haplotypes.lengths.max())
+        prof.coverage_ref_len = prof.ref.genome_len         # -x counts the haploid reference
     if mode == "genome" and len(prof.ref.names) > 1 and dna_type == "circular":
         sys.stderr.write("Do not choose circular if there is more than one chromosome in the genome!\n")
         sys.exit(1)
@@ -426,6 +459,9 @@ GZIP_ERR_HELP = ('With --gzip or --bam: write the error profile as BGZF-compress
 BAM_HELP = ('Write the reads as unaligned BAM, <out>_aligned_reads.bam and <out>_unaligned_reads.bam (one unmapped record per '
             'read, as Dorado writes them), encoded and compressed on the GPU. The error profile stays plain text unless '
             '--gzip_error_profile is given (Default = False)')
+VCF_HELP = ('Simulate the reads from the haplotypes of the first sample of this VCF (plain or .vcf.gz), built on the GPU from '
+            'the reference: records <chrom>-hap1 and <chrom>-hap2 (one copy for a haploid GT). Only FILTER PASS or . records '
+            'are applied. -x still counts the haploid reference, so -x 30 is about 15x per haplotype')
 
 
 def _plain_error_profile(args):
@@ -479,6 +515,7 @@ def build_parser():
     g.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     g.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     g.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
+    g.add_argument('--vcf', help=VCF_HELP, default=None)
     mg = sub.add_parser('metagenome', help="Run the simulator on metagenome mode")
     mg.add_argument('-gl', '--genome_list', help="Reference metagenome list, tsv file, the first column is species/strain "
                     "name, the second column is the reference genome fasta/fastq file directory", required=True)
@@ -755,6 +792,10 @@ def main(argv=None):
         print("\nPerfect reads cannot be chimeric\n")
         parser_g.print_help(sys.stderr)
         sys.exit(1)
+    if args.vcf and args.dna_type == "circular":
+        sys.stderr.write("\n--vcf cannot be combined with -dna_type circular!\n")
+        parser_g.print_help(sys.stderr)
+        sys.exit(1)
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -766,7 +807,7 @@ def main(argv=None):
 
     prof = read_profile(args.ref_g, number, args.model_prefix, args.perfect, args.mode, args.strandness,
                         dna_type=args.dna_type, chimeric=args.chimeric, homopolymer=args.homopolymer, fastq=args.fastq,
-                        device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args))
+                        device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args), vcf=args.vcf)
     if args.coverage is not None:
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
