@@ -235,8 +235,12 @@ int ns_set_reference(NsContext* ctx, const NsReference* ref);
 int ns_set_model(NsContext* ctx, const NsModel* model);
 /* genome --vcf: the haplotype records of a VCF sample (nanosim_b200/variants.py builds these tables).  Haplotype h copies
  * record hap_chrom[h] of the resident reference with variants var_off[h] .. var_off[h+1]-1 applied, in position order:
- * the span [var_pos, var_pos + var_ref_len) of that record is replaced by alt[alt_off .. alt_off + alt_len).  Spans of one
- * haplotype may touch but not overlap.  Host pointers. */
+ * the span [var_pos, var_pos + var_ref_len) of that record is replaced by the variant's ALT, which alt_kind[j] selects:
+ *   0  alt[alt_off .. alt_off + alt_len) (every variant when alt_kind is NULL);
+ *   1  the source record's own bases [alt_off, alt_off + alt_len), forward (a tandem duplication: var_ref_len 0);
+ *   2  the same bases reverse-complemented (an inversion: alt_off = var_pos, alt_len = var_ref_len).
+ * Spans of one haplotype may touch but not overlap.  NS_EINVAL for a kind above 2, and for an ALT outside the ALT bytes
+ * (kind 0) or outside its source record (kinds 1 and 2).  Host pointers. */
 typedef struct {
     uint32_t n_hap;
     const uint32_t* hap_chrom;       /* n_hap */
@@ -250,6 +254,7 @@ typedef struct {
     uint64_t alt_bytes;
     uint64_t* peak_bytes;            /* out, may be NULL: accounted peak -- the sizes of the library's allocations (reference and build) at the build's high
                                         point, not a device reading */
+    const uint8_t* alt_kind;         /* n_var, or NULL: every variant is kind 0 */
 } NsVariants;
 /* Builds the haplotypes in HBM from the resident reference and makes them the resident reference, record h being
  * haplotype h (what ns_set_reference does with them: 2-bit copy, chromosome checks); the haploid bytes are freed.  Call

@@ -35,7 +35,7 @@ class NsReference(C.Structure):
 class NsVariants(C.Structure):
     _fields_ = [("n_hap", C.c_uint32), ("hap_chrom", C.c_void_p), ("var_off", C.c_void_p), ("n_var", C.c_uint64),
                 ("var_pos", C.c_void_p), ("var_ref_len", C.c_void_p), ("alt_off", C.c_void_p), ("alt_len", C.c_void_p),
-                ("alt", C.c_void_p), ("alt_bytes", C.c_uint64), ("peak_bytes", C.POINTER(C.c_uint64))]
+                ("alt", C.c_void_p), ("alt_bytes", C.c_uint64), ("peak_bytes", C.POINTER(C.c_uint64)), ("alt_kind", C.c_void_p)]
 
 
 class NsKde(C.Structure):

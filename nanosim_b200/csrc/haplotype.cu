@@ -15,7 +15,9 @@ cudaError_t hap_layout(const HapArgs& a, uint64_t* seg_out, uint64_t* hap_off, v
 }
 
 cudaError_t hap_gather(const uint8_t* ref, const uint8_t* alt, const uint64_t* seg_src, const uint64_t* seg_out, uint64_t n_seg,
-                       uint64_t n_bases, uint8_t* out, cudaStream_t st) {
-    hap_gather_kernel<<<(unsigned)((n_bases + 16 * 256 - 1) / (16 * 256)), 256, 0, st>>>(ref, alt, seg_src, seg_out, n_seg, out);
+                       uint64_t n_bases, bool reverse_complement, uint8_t* out, cudaStream_t st) {
+    const unsigned blocks = (unsigned)((n_bases + 16 * 256 - 1) / (16 * 256));
+    if (reverse_complement) hap_gather_kernel<true><<<blocks, 256, 0, st>>>(ref, alt, seg_src, seg_out, n_seg, out);
+    else hap_gather_kernel<false><<<blocks, 256, 0, st>>>(ref, alt, seg_src, seg_out, n_seg, out);
     return cudaGetLastError();
 }

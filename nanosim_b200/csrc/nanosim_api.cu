@@ -814,6 +814,7 @@ int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
     if (tab.dref.n_species) return fail(ctx, NS_EINVAL, "ns_apply_variants: a metagenome reference cannot carry variants");
     const uint32_t n_chrom = tab.dref.n_chrom;
     const std::vector<uint64_t>& off = tab.h_chrom_off;
+    bool any_rc = false;                                            // an inversion: the gather's reverse-complement path
     if (v->var_off[0] != 0 || v->var_off[v->n_hap] != v->n_var)
         return fail(ctx, NS_EINVAL, "ns_apply_variants: var_off must start at 0 and end at n_var");
     for (uint32_t h = 0; h < v->n_hap; ++h) {
@@ -822,22 +823,32 @@ int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
         if (v->var_off[h + 1] < v->var_off[h]) return fail(ctx, NS_EINVAL, "ns_apply_variants: var_off decreases at haplotype %u", h);
         uint64_t end = 0;
         for (uint64_t j = v->var_off[h]; j < v->var_off[h + 1]; ++j) {
-            if (v->var_pos[j] < end || v->var_pos[j] + v->var_ref_len[j] > off[c + 1] - off[c] || v->alt_off[j] + v->alt_len[j] > v->alt_bytes)
+            const uint8_t kind = v->alt_kind ? v->alt_kind[j] : 0;
+            if (kind > 2)
+                return fail(ctx, NS_EINVAL, "ns_apply_variants: variant %llu of haplotype %u has ALT kind %u (0, 1 or 2)", (unsigned long long)j,
+                            h, (unsigned)kind);
+            if (v->var_pos[j] < end || v->var_pos[j] + v->var_ref_len[j] > off[c + 1] - off[c])
                 return fail(ctx, NS_EINVAL, "ns_apply_variants: variant %llu of haplotype %u overlaps the one before it or lies outside "
-                            "its record or the ALT bytes", (unsigned long long)j, h);
+                            "its record", (unsigned long long)j, h);
+            const uint64_t src_bytes = kind ? off[c + 1] - off[c] : v->alt_bytes;      // kinds 1 and 2 read the source record
+            if (v->alt_off[j] > src_bytes || v->alt_len[j] > src_bytes - v->alt_off[j])
+                return fail(ctx, NS_EINVAL, "ns_apply_variants: the ALT of variant %llu of haplotype %u lies outside %s", (unsigned long long)j, h,
+                            kind ? "its source record" : "the ALT bytes");
             end = v->var_pos[j] + v->var_ref_len[j];
+            any_rc |= kind == 2;
         }
     }
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     const uint64_t n_seg = 2 * v->n_var + v->n_hap;
-    DevBuf hap_chrom, var_off, var_pos, var_ref_len, alt_off, alt_len, alt, seg_src, seg_len, seg_out, hap_off, out;
+    DevBuf hap_chrom, var_off, var_pos, var_ref_len, alt_off, alt_len, alt_kind, alt, seg_src, seg_len, seg_out, hap_off, out;
     CK(upload(hap_chrom, v->hap_chrom, (size_t)v->n_hap * 4, st));
     CK(upload(var_off, v->var_off, (size_t)(v->n_hap + 1) * 8, st));
     CK(upload(var_pos, v->var_pos, v->n_var * 8, st));
     CK(upload(var_ref_len, v->var_ref_len, v->n_var * 4, st));
     CK(upload(alt_off, v->alt_off, v->n_var * 8, st));
     CK(upload(alt_len, v->alt_len, v->n_var * 4, st));
+    if (v->alt_kind) CK(upload(alt_kind, v->alt_kind, v->n_var, st));
     CK(alt.ensure(v->alt_bytes + 16));                              // hap_gather_kernel reads whole words behind the end
     if (v->alt_bytes) CK(cudaMemcpyAsync(alt.p, v->alt, v->alt_bytes, cudaMemcpyHostToDevice, st));
     CK(seg_src.ensure(n_seg * 8));
@@ -845,8 +856,8 @@ int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
     CK(seg_out.ensure((n_seg + 1) * 8));
     CK(hap_off.ensure((size_t)(v->n_hap + 1) * 8));
     HapArgs a{hap_chrom.as<uint32_t>(), var_off.as<uint64_t>(), var_pos.as<uint64_t>(), var_ref_len.as<uint32_t>(),
-              alt_off.as<uint64_t>(), alt_len.as<uint32_t>(), tab.dref.chrom_off, v->n_hap, n_seg, seg_src.as<uint64_t>(),
-              seg_len.as<uint64_t>()};
+              alt_off.as<uint64_t>(), alt_len.as<uint32_t>(), v->alt_kind ? alt_kind.as<uint8_t>() : nullptr, tab.dref.chrom_off, v->n_hap,
+              n_seg, seg_src.as<uint64_t>(), seg_len.as<uint64_t>()};
     size_t tmp = 0;
     CK(hap_layout(a, seg_out.as<uint64_t>(), hap_off.as<uint64_t>(), nullptr, &tmp, st));
     CK(ctx->scan_tmp.ensure(tmp));
@@ -856,12 +867,13 @@ int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
     CK(cudaStreamSynchronize(st));
     if (n_bases == 0) return fail(ctx, NS_EINVAL, "ns_apply_variants: the haplotypes have no bases");
     CK(out.ensure(n_bases + 16));
-    CK(hap_gather(tab.dref.bases, alt.as<uint8_t>(), seg_src.as<uint64_t>(), seg_out.as<uint64_t>(), n_seg, n_bases, out.as<uint8_t>(), st));
+    CK(hap_gather(tab.dref.bases, alt.as<uint8_t>(), seg_src.as<uint64_t>(), seg_out.as<uint64_t>(), n_seg, n_bases, any_rc, out.as<uint8_t>(),
+                  st));
     CK(cudaStreamSynchronize(st));
     // accounted peak (sizes of the library's allocations, not a device reading) at the two high points: the haploid
     // reference beside the haplotypes, then the new resident copy (ns_set_reference's) beside them; the build's tables
     // and the scan's scratch space are held throughout
-    const size_t build = hap_chrom.cap + var_off.cap + var_pos.cap + var_ref_len.cap + alt_off.cap + alt_len.cap + alt.cap +
+    const size_t build = hap_chrom.cap + var_off.cap + var_pos.cap + var_ref_len.cap + alt_off.cap + alt_len.cap + alt_kind.cap + alt.cap +
                          seg_src.cap + seg_len.cap + seg_out.cap + hap_off.cap + out.cap + ctx->scan_tmp.cap;
     const size_t peak_a = build + tab.ref_bases.cap + tab.ref_off.cap + tab.ref_packed.cap + tab.ref_pk_off.cap + tab.ref_exc.cap;
     // the haploid bytes and their 2-bit copy go before ns_set_reference allocates the haplotypes' own

@@ -96,7 +96,7 @@ class Engine:
         t = tables
         peak = C.c_uint64()
         v = L.NsVariants(len(t.hap_chrom), _ptr(t.hap_chrom), _ptr(t.var_off), len(t.var_pos), _ptr(t.var_pos), _ptr(t.var_ref_len),
-                         _ptr(t.alt_off), _ptr(t.alt_len), _ptr(t.alt), len(t.alt), C.pointer(peak))
+                         _ptr(t.alt_off), _ptr(t.alt_len), _ptr(t.alt), len(t.alt), C.pointer(peak), _ptr(t.alt_kind))
         self._check(self._lib.ns_apply_variants(self._ctx, C.byref(v)))
         return int(peak.value)
 

@@ -119,8 +119,9 @@ def _apply_variants(prof, tables, ref_on_host):
     if ref_on_host:
         prof.ref.bases = prof.engine.reference_bases(prof.ref.genome_len)
     prof.engine.ref = prof.ref
-    for name, n, skipped in zip(tables.names, tables.applied, tables.skipped):
-        _log("%s: %d variants applied, %d records of its chromosome skipped by FILTER" % (name, n, skipped))
+    for name, n, (n_del, n_inv, n_dup), skipped in zip(tables.names, tables.applied, tables.structural, tables.skipped):
+        _log("%s: %d variants applied (of them from symbolic alleles: %d deletions, %d inversions, %d duplications), %d records of "
+             "its chromosome skipped by FILTER" % (name, n, n_del, n_inv, n_dup, skipped))
     if tables.skipped_elsewhere:
         _log("%d records on contigs that are not in the reference skipped by FILTER" % tables.skipped_elsewhere)
 

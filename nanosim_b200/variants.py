@@ -9,16 +9,29 @@ is a few array operations rather than a Python call.  Semantics (DESIGN §3, "Mo
   order of ``bcftools consensus -H 1`` / ``-H 2``); ``0`` and ``.`` are the reference, ``k`` is ``ALT[k-1]``, ``*`` is
   the reference (a deletion on that haplotype already covers the position);
 * REF must equal the reference bytes (case-insensitively); applied spans of one haplotype may touch but not overlap;
-  symbolic and breakend ALTs are errors; all records of one chromosome have the same ploidy (1 or 2), a chromosome
-  without records gets 2 copies.
+  all records of one chromosome have the same ploidy (1 or 2), a chromosome without records gets 2 copies;
+* the symbolic structural variants ``<DEL>``, ``<INV>``, ``<DUP>`` and ``<DUP:TANDEM>`` are applied; every other
+  symbolic or breakend ALT that a haplotype takes is an error, one that no haplotype takes is not checked.  A record
+  whose allele a haplotype takes as one of those four has exactly one ALT and a one-base REF (the padding base at POS,
+  which stays the FASTA's byte).  Its affected bases are POS+1 .. END (1-based, inclusive), END from INFO ``END=e``
+  (END = e) or ``SVLEN=s`` (END = POS + |s|: VCF 4.3 writes deletions as negative, 4.4 as positive); with both they must
+  agree, and POS < END <= the record's length.  With P = POS and E = END, ``ref[P:E]`` is what changes: ``<DEL>`` gives
+  ``ref[:P] + ref[E:]``, ``<INV>`` ``ref[:P] + rc(ref[P:E]) + ref[E:]`` and ``<DUP>``/``<DUP:TANDEM>``
+  ``ref[:E] + ref[P:E] + ref[E:]`` (one extra copy, in tandem).  ``rc`` reverses and complements A-T, C-G, R-Y, K-M,
+  B-V and D-H in either case, keeping the case; every other byte stays.  For the overlap rule the record's span is
+  ``[POS-1, END)``, the padding base included.  Only these few records are read one by one (their INFO).
 
 Every error is a ``VcfError`` whose message names the line (1-based, header lines included).
 """
 import gzip
+import re
 
 import numpy as np
 
 _PASS = (b"PASS", b".")
+_SYMBOLIC = {b"<DEL>": 1, b"<INV>": 2, b"<DUP>": 3, b"<DUP:TANDEM>": 3}     # the structural variants applied
+_SV_DEL, _SV_INV, _SV_DUP = 1, 2, 3
+_NUMBER = re.compile(rb"[+-]?[0-9]{1,18}")
 _UPPER = np.arange(256, dtype=np.uint8)
 _UPPER[ord("a"):ord("z") + 1] -= 32
 _NOT_SEQUENCE = np.ones(256, dtype=bool)            # an applied ALT is IUPAC nucleotide codes in either case; this rejects
@@ -38,10 +51,14 @@ class HaplotypeTables:
     For haplotype record h (in order: reference records in file order, each with its copies in haplotype order):
     ``hap_chrom[h]`` is its source reference record, ``hap_number[h]`` 1 or 2, and its variants are
     ``var_off[h] .. var_off[h+1]``, in position order: reference span ``[var_pos, var_pos + var_ref_len)`` of that
-    record, replaced by ``alt[alt_off : alt_off + alt_len]``."""
+    record, replaced by what ``alt_kind`` says: 0 ``alt[alt_off : alt_off + alt_len]``, 1 the source record's own bases
+    ``[alt_off, alt_off + alt_len)``, 2 those bases reverse-complemented.  Symbolic alleles are encoded as
+    ``<DEL>``: kind 0 with ``alt_len`` 0 (no other variant has an empty ALT); ``<INV>``: ``var_pos = alt_off = P``,
+    ``var_ref_len = alt_len = E - P``, kind 2; ``<DUP>``: ``var_pos = E``, ``var_ref_len = 0``, ``alt_off = P``,
+    ``alt_len = E - P``, kind 1."""
 
     def __init__(self, names, hap_chrom, hap_number, var_off, var_pos, var_ref_len, alt_off, alt_len, alt, lengths, skipped,
-                 skipped_elsewhere=0):
+                 skipped_elsewhere=0, alt_kind=None):
         self.names = list(names)
         self.hap_chrom = np.ascontiguousarray(hap_chrom, dtype=np.uint32)
         self.hap_number = np.ascontiguousarray(hap_number, dtype=np.uint8)
@@ -54,10 +71,19 @@ class HaplotypeTables:
         self.lengths = np.ascontiguousarray(lengths, dtype=np.int64)    # bases of every haplotype record
         self.skipped = np.ascontiguousarray(skipped, dtype=np.int64)    # records of its chromosome skipped by FILTER
         self.skipped_elsewhere = int(skipped_elsewhere)     # records skipped by FILTER on contigs the reference lacks
+        self.alt_kind = np.ascontiguousarray(np.zeros(len(self.var_pos)) if alt_kind is None else alt_kind, dtype=np.uint8)
 
     @property
     def applied(self):
         return np.diff(self.var_off.astype(np.int64))
+
+    @property
+    def structural(self):
+        """(n_hap, 3): per haplotype record, the deletions, inversions and duplications applied from symbolic alleles."""
+        n = len(self.hap_chrom)
+        h = np.repeat(np.arange(n), self.applied)
+        kinds = ((self.alt_kind == 0) & (self.alt_len == 0), self.alt_kind == 2, self.alt_kind == 1)
+        return np.stack([np.bincount(h[k], minlength=n) for k in kinds], axis=1)
 
     @property
     def offsets(self):
@@ -270,7 +296,14 @@ def _read_records(buf, ref, path, limit):
     order = np.lexsort((rec, key))          # per haplotype record, in file order
     key, rec, a_s, a_n = key[order], rec[order], a_s[order], a_n[order]
 
-    bad_len = a_n == 0
+    # the structural variants applied (a symbolic allele starts with '<'; few alleles do); they have no ALT bytes
+    sv_type = np.zeros(len(rec), dtype=np.int64)
+    for i in np.flatnonzero(buf[np.minimum(a_s, len(buf) - 1)] == ord("<")).tolist():
+        sv_type[i] = _SYMBOLIC.get(bytes(buf[a_s[i]:a_s[i] + a_n[i]]), 0)
+    sv = sv_type > 0
+    a_n = np.where(sv, 0, a_n)
+
+    bad_len = (a_n == 0) & ~sv
     alt_idx, arow = _flat(a_s, a_n)
     bad_byte = np.zeros(len(rec), dtype=bool)
     bad_byte[arow[_NOT_SEQUENCE[buf[alt_idx]]]] = True
@@ -279,9 +312,16 @@ def _read_records(buf, ref, path, limit):
         raise VcfError(line[rec[bad]].min(), "a haplotype takes an ALT allele that is symbolic, a breakend, missing or not a "
                        "nucleotide sequence")
 
+    # span end of every record (0-based, exclusive): END for a structural variant, checked record by record in file order
+    rec_end = pos - 1 + ref_len
+    if sv.any():
+        info_s, info_e = field(7)
+        for r in np.unique(rec[sv]).tolist():
+            rec_end[r] = _sv_end(bytes(buf[info_s[r]:info_e[r]]), int(pos[r]), int(ref_len[r]), int(n_alt[r]), int(clen[r]), int(line[r]))
+
     # overlap: on one haplotype, a span that starts before the previous applied span ends
     v_pos = pos[rec] - 1
-    v_end = v_pos + ref_len[rec]
+    v_end = rec_end[rec]
     same = key[1:] == key[:-1]
     over = same & (v_pos[1:] < v_end[:-1])
     if over.any():
@@ -294,9 +334,44 @@ def _read_records(buf, ref, path, limit):
     hap_number = np.arange(n_hap) - hap_base[hap_chrom] + 1
     counts = np.bincount(key, minlength=n_hap)
     var_off = np.concatenate([[0], np.cumsum(counts)])
-    grow = np.concatenate([[0], np.cumsum(a_n - ref_len[rec])])
+    # the table rows (HaplotypeTables), then the structural variants' own: P = POS and E = END
+    t_pos, t_ref_len, t_alt_len, kind = v_pos, ref_len[rec], a_n, None
+    t_alt_off = np.concatenate([[0], np.cumsum(a_n)[:-1]]) if len(a_n) else a_n
+    if sv.any():
+        P, E = pos[rec], rec_end[rec]
+        t_pos = np.where(sv_type == _SV_DUP, E, np.where(sv, P, v_pos))
+        t_ref_len = np.where(sv_type == _SV_DUP, 0, np.where(sv, E - P, t_ref_len))
+        t_alt_off = np.where(sv_type >= _SV_INV, P, t_alt_off)
+        t_alt_len = np.where(sv_type >= _SV_INV, E - P, a_n)
+        kind = np.select([sv_type == _SV_INV, sv_type == _SV_DUP], [2, 1], 0)
+    grow = np.concatenate([[0], np.cumsum(t_alt_len - t_ref_len)])
     delta = grow[var_off[1:]] - grow[var_off[:-1]]
     lengths = (offs[1:] - offs[:-1])[hap_chrom] + delta
     names = ["%s-hap%d" % (ref.names[c], h) for c, h in zip(hap_chrom, hap_number)]
-    return HaplotypeTables(names, hap_chrom, hap_number, var_off, v_pos, ref_len[rec], np.concatenate([[0], np.cumsum(a_n)[:-1]]) if len(a_n) else [],
-                           a_n, buf[alt_idx], lengths, skipped_chrom[hap_chrom], skipped_elsewhere)
+    return HaplotypeTables(names, hap_chrom, hap_number, var_off, t_pos, t_ref_len, t_alt_off, t_alt_len, buf[alt_idx], lengths,
+                           skipped_chrom[hap_chrom], skipped_elsewhere, kind)
+
+
+def _sv_end(info, pos, ref_len, n_alt, clen, line):
+    """END of a record whose allele a haplotype takes as a structural variant: its span's 0-based exclusive end."""
+    if n_alt > 1:
+        raise VcfError(line, "a symbolic structural variant must be the record's only ALT allele")
+    if ref_len != 1:
+        raise VcfError(line, "the REF of a symbolic structural variant must be one base (the padding base)")
+    value = {}
+    for item in info.split(b";"):
+        k, _, v = item.partition(b"=")
+        if k in (b"END", b"SVLEN") and k not in value:
+            if not _NUMBER.fullmatch(v):
+                raise VcfError(line, "INFO %s is not a number" % k.decode())
+            value[k] = int(v)
+    if not value:
+        raise VcfError(line, "a symbolic structural variant needs END or SVLEN in INFO")
+    end = value.get(b"END", pos + abs(value.get(b"SVLEN", 0)))
+    if b"SVLEN" in value and end != pos + abs(value[b"SVLEN"]):
+        raise VcfError(line, "END (%d) and SVLEN (%d) disagree" % (end, value[b"SVLEN"]))
+    if end <= pos:
+        raise VcfError(line, "END (%d) is not past POS (%d)" % (end, pos))
+    if end > clen:
+        raise VcfError(line, "END (%d) extends past the end of the reference record (%d bases)" % (end, clen))
+    return end
