@@ -394,6 +394,18 @@ int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_
  * ns_fetch_compressed copies them.  NS_EINVAL when a name is longer than 254 bytes (the message names the first such read
  * and its length); names are never truncated. */
 int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
+/* The last aligned batch as MAPPED BAM records: the true alignment of every read to the records of the resident reference,
+ * built on the device from the pieces' emitted scripts and BGZF-compressed like ns_compress_bam.  One record per aligned
+ * segment (two for a segment that crosses a circular record's origin), the read's records adjacent and in the order of
+ * its segments; the one with the longest reference span is primary and stores the whole read with S clips, the others
+ * carry flag 0x800 and store their own bases with H clips.  SEQ/QUAL are in forward-strand order (flag 16 for a reversed
+ * read, stored reverse-complemented), refID is the piece's record, mapq 60, no aux fields but CG:B,I when a CIGAR has more
+ * than 65 535 ops (the CIGAR field then reads <l_seq>S<span>N).  A read with no alignment gets ns_compress_bam's unmapped
+ * record.  The CIGAR rules are in DESIGN.md §3 "Mapped BAM".  Same name layout and 254-byte name limit as ns_compress_bam;
+ * neither header nor end-of-file block.  The members replace those of the last ns_compress_records / ns_compress_bam;
+ * ns_fetch_compressed copies them.  NS_EINVAL when the last batch is unaligned reads or the context is in transcriptome
+ * mode. */
+int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
 /* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' (or ns_compress_bam's)
  * *nbytes. */
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap);

@@ -1,0 +1,353 @@
+// Mapped BAM (ns_compress_bam_mapped): the true alignment of every aligned read of the last batch, built from the pieces'
+// emitted scripts (op_off / n_ops, forward-strand order) as BAM records for bgzf_deflate_kernel<BgzfRecords<BgzfMappedLayout>>.
+// The rules are in DESIGN §3 "Mapped BAM"; tests/test_mapped_bam.py restates them in Python.
+//   pass 1 (aln_count_kernel): per read its records (its alignments, or one unmapped record) and CIGAR words, and which
+//          alignment is primary; CUB scans of both give every read its first record and first CIGAR word
+//   pass 2 (aln_write_kernel): the same walk writes the records' descriptors, CIGAR words and sizes
+// One thread per read: the rules (LIT groups, merging, trimming, the cut at a circular record's origin) are a sequential
+// state machine over the script, and each read's ops are contiguous in HBM.
+#pragma once
+
+// CIGAR operations (SAM/BAM specification §4.2.2: MIDNSHP=X -> 0..8)
+enum : uint32_t { CIG_M = 0, CIG_I = 1, CIG_D = 2, CIG_N = 3, CIG_S = 4, CIG_H = 5 };
+constexpr uint32_t ALN_CUT = 15;                    // the origin of a circular record: one alignment ends, the next starts
+constexpr uint32_t BAM_MAX_CIGAR = 65535;           // n_cigar_op is 16 bits; more ops go into a CG:B,I field
+constexpr uint32_t BAM_MAPQ = 60;
+
+// one mapped record (or, flag 4, the unmapped record ns_compress_bam writes)
+struct BamAln {
+    uint32_t read;                  // slot of the read in the batch
+    uint32_t q0;                    // first stored base, forward-strand offset in the read
+    uint32_t l_seq;                 // stored bases
+    uint32_t ref_id, pos, span;
+    uint32_t n_cig;                 // CIGAR ops with the clips
+    uint16_t bin, flag;
+    uint64_t cig_off;               // first CIGAR word
+};
+
+// reg2bin (specification §5.3) of [beg, end); 4680 past 2^29, which BAI cannot index (CSI recomputes bins)
+__host__ __device__ __forceinline__ uint32_t bam_reg2bin(uint64_t beg, uint64_t end) {
+    if (end > (1ull << 29)) return 4680;
+    --end;
+    if (beg >> 14 == end >> 14) return ((1u << 15) - 1) / 7 + (uint32_t)(beg >> 14);
+    if (beg >> 17 == end >> 17) return ((1u << 12) - 1) / 7 + (uint32_t)(beg >> 17);
+    if (beg >> 20 == end >> 20) return ((1u << 9) - 1) / 7 + (uint32_t)(beg >> 20);
+    if (beg >> 23 == end >> 23) return ((1u << 6) - 1) / 7 + (uint32_t)(beg >> 23);
+    if (beg >> 26 == end >> 26) return ((1u << 3) - 1) / 7 + (uint32_t)(beg >> 26);
+    return 0;
+}
+
+// bytes of a mapped record: the fixed fields, name, CIGAR (kSmN when it does not fit), bases, qualities, CG:B,I
+__host__ __device__ __forceinline__ uint64_t bam_mapped_size(uint32_t nl, const BamAln& a) {
+    const bool cg = a.n_cig > BAM_MAX_CIGAR;
+    return BAM_FIXED + nl + 1 + 4ull * (cg ? 2 : a.n_cig) + (a.l_seq + 1) / 2 + a.l_seq + (cg ? 8 + 4ull * a.n_cig : 0);
+}
+
+// the complement of a 4-bit base code: its bits reversed (A 1 <-> T 8, C 2 <-> G 4, M <-> K, R <-> Y, V <-> B, H <-> D;
+// =, S, W, N fixed)
+__device__ __forceinline__ uint32_t bam_code_comp(uint32_t c) { return __brev(c) >> 28; }
+
+struct BgzfMappedRec {
+    BgzfReadRec rd;                 // the read
+    BamAln a;
+    const uint32_t* cig;
+    uint32_t rev;
+};
+struct BgzfMappedTable {
+    BgzfReadTable reads;
+    const BamAln* aln;
+    const uint32_t* cigar;
+    __device__ __forceinline__ BgzfMappedRec operator[](uint32_t r) const {
+        const BamAln a = aln[r];
+        return BgzfMappedRec{reads[a.read], a, cigar + a.cig_off, reads.reads[a.read].reversed};
+    }
+};
+
+struct BgzfMappedLayout {
+    using Table = BgzfMappedTable;
+    static __device__ __forceinline__ uint8_t byte(uint64_t q, const BgzfMappedRec& rc) {
+        const BamAln& a = rc.a;
+        if (a.flag & 4) return BgzfBamLayout::byte(q, rc.rd);
+        const uint32_t nl = rc.rd.nl, ls = a.l_seq, L = rc.rd.L;
+        const bool cg = a.n_cig > BAM_MAX_CIGAR;
+        const uint32_t nc = cg ? 2 : a.n_cig;
+        if (q < BAM_FIXED) {
+            uint32_t w;
+            switch ((uint32_t)q >> 2) {
+            case 0: w = (uint32_t)bam_mapped_size(nl, a) - 4; break;                        // block_size
+            case 1: w = a.ref_id; break;
+            case 2: w = a.pos; break;
+            case 3: w = (nl + 1) | (BAM_MAPQ << 8) | ((uint32_t)a.bin << 16); break;       // l_read_name, mapq, bin
+            case 4: w = nc | ((uint32_t)a.flag << 16); break;                               // n_cigar_op, flag
+            case 5: w = ls; break;                                                          // l_seq
+            case 8: w = 0; break;                                                           // tlen
+            default: w = 0xffffffffu;                                                       // next_refID, next_pos
+            }
+            return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
+        }
+        q -= BAM_FIXED;
+        if (q < nl) return (uint8_t)rc.rd.nm[q];
+        if (q == nl) return 0;
+        q -= nl + 1;
+        if (q < 4ull * nc) {
+            const uint32_t k = (uint32_t)q >> 2;
+            const uint32_t w = !cg ? rc.cig[k] : k == 0 ? (ls << 4) | CIG_S : (a.span << 4) | CIG_N;
+            return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
+        }
+        q -= 4ull * nc;
+        // stored base b is forward-strand base q0 + b: a reversed read's is the complement of its mirror in the read
+        auto code = [&](uint32_t b) -> uint32_t {
+            const uint32_t f = a.q0 + b;
+            return rc.rev ? bam_code_comp(bam_base_code(rc.rd.sq[L - 1 - f])) : bam_base_code(rc.rd.sq[f]);
+        };
+        const uint64_t n_packed = (ls + 1) / 2;
+        if (q < n_packed) {
+            const uint32_t b = 2 * (uint32_t)q;
+            return (uint8_t)((code(b) << 4) | (b + 1 < ls ? code(b + 1) : 0u));
+        }
+        q -= n_packed;
+        if (q < ls) {
+            const uint32_t f = a.q0 + (uint32_t)q;
+            return rc.rd.fastq ? (uint8_t)(rc.rd.ql[rc.rev ? L - 1 - f : f] - 33) : 0xffu;
+        }
+        q -= ls;
+        if (q < 4) return (uint8_t)"CGBI"[q];
+        const uint32_t k = (uint32_t)(q - 4) >> 2;             // the count, then the words
+        const uint32_t w = k == 0 ? a.n_cig : rc.cig[k - 1];
+        return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
+    }
+};
+
+struct AlnArgs {
+    const NsReadMeta* reads;
+    const NsPieceMeta* pieces;
+    const uint32_t* ops;
+    const uint64_t* chrom_off;
+    const char* names;              // NUL-terminated, at name_off[i]
+    const uint64_t* name_off;
+    uint32_t n_reads;
+    uint32_t* name_len;             // pass 1 writes, pass 2 reads
+    uint64_t* n_rec;                // pass 1: records of every read
+    uint64_t* n_cig;                // pass 1: CIGAR words of every read
+    uint32_t* primary;              // pass 1: the primary alignment's index in the read
+    unsigned long long* long_names; // pass 1: names longer than BAM_MAX_NAME
+    const uint64_t* rec_first;      // pass 2: exclusive prefix sums of n_rec and n_cig
+    const uint64_t* cig_first;
+    BamAln* aln;                    // pass 2 writes
+    uint32_t* cigar;
+    uint64_t* rec_size;
+};
+
+// fn(kind, len) over a segment's script: CIGAR kinds M I D (HT as I: it only stands at a read's edges), a LIT group followed
+// by a DEL as |n - r| I or D and then min(n, r) M, zero lengths dropped, and an ALN_CUT (len 0) before the reference base
+// at offset `cut` and every `period` bases behind it (a circular record's origin, each time the segment passes it; ~0:
+// none), an M or D across one split there
+template <class Fn>
+__device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint32_t n_ops, uint64_t cut, uint64_t period, Fn fn) {
+    uint64_t rf = 0;
+    uint32_t lit = 0;
+    auto put = [&](uint32_t kind, uint32_t len) {
+        if (len == 0) return;
+        if (kind != CIG_I) {
+            while (rf <= cut && rf + len > cut) {
+                const uint32_t a = (uint32_t)(cut - rf);
+                if (a) fn(kind, a);
+                fn(ALN_CUT, 0u);
+                rf += a;
+                len -= a;
+                cut += period;
+            }
+            rf += len;
+        }
+        fn(kind, len);
+    };
+    for (uint32_t j = 0; j < n_ops; ++j) {
+        const uint32_t op = sc[j], ty = NS_OP_TYPE(op), ln = NS_OP_LEN(op);
+        if (ty == NS_OP_LIT) {
+            lit += ln;
+            continue;
+        }
+        if (lit && ty == NS_OP_DEL) {
+            put(lit > ln ? CIG_I : CIG_D, lit > ln ? lit - ln : ln - lit);
+            put(CIG_M, min(lit, ln));
+            lit = 0;
+            continue;
+        }
+        put(CIG_I, lit);
+        lit = 0;
+        put(ty == NS_OP_DEL ? CIG_D : (ty == NS_OP_COPY || ty == NS_OP_MIS) ? CIG_M : CIG_I, ln);
+    }
+    put(CIG_I, lit);
+}
+
+// The alignments of one segment (n_parts of them at most: the cuts split it), its ops starting at read offset q_start: for
+// each, sink.begin(q0, rf0) at its first M, sink.op(kind, len) for its merged ops, sink.end(q1, rf1) after its last M
+// (read offsets in the forward read, reference offsets in the segment).  Ops before the first M and after the last one
+// are outside the alignment: their I is clip, their D moves the start or is dropped.  Two walks per part: the first finds
+// the part's first and last M, the second emits what lies between them.
+template <class Sink>
+__device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, uint64_t cut, uint64_t period, uint32_t n_parts,
+                                            uint32_t q_start, Sink& sink) {
+    for (uint32_t want = 0; want < n_parts; ++want) {
+        uint32_t first = ~0u, last = 0, idx = 0, part = 0;
+        aln_script(sc, n_ops, cut, period, [&](uint32_t kind, uint32_t) {
+            if (kind == ALN_CUT) {
+                ++part;
+            } else if (kind == CIG_M && part == want) {
+                if (first == ~0u) first = idx;
+                last = idx;
+            }
+            ++idx;
+        });
+        if (first == ~0u) continue;
+        idx = 0;
+        uint32_t q = q_start, rf = 0, ck = 0, cl = 0;
+        aln_script(sc, n_ops, cut, period, [&](uint32_t kind, uint32_t len) {
+            if (idx >= first && idx <= last) {
+                if (idx == first) {
+                    sink.begin(q, rf);
+                    ck = kind;
+                    cl = 0;
+                }
+                if (kind == ck) {
+                    cl += len;
+                } else {
+                    sink.op(ck, cl);
+                    ck = kind;
+                    cl = len;
+                }
+                if (idx == last) {
+                    sink.op(ck, cl);
+                    sink.end(q + len, rf + len);
+                }
+            }
+            if (kind != CIG_D) q += len;
+            if (kind != CIG_I) rf += len;
+            ++idx;
+        });
+    }
+}
+
+// every alignment of read r, in the order of its segments: sink.segment(piece, record length) before each segment's
+template <class Sink>
+__device__ __forceinline__ void aln_read(const AlnArgs& a, const NsReadMeta& r, Sink& sink) {
+    for (uint32_t k = 0; k < r.n_pieces; ++k) {
+        const NsPieceMeta pc = a.pieces[r.piece_first + k];
+        if (NS_PIECE_KIND(pc.kind) != NS_PIECE_SEGMENT) continue;
+        const uint64_t clen = a.chrom_off[pc.chrom + 1] - a.chrom_off[pc.chrom];
+        // a segment that runs past its record's end (circular records only) is cut at the origin, as often as it passes it
+        uint64_t cut = ~0ull;
+        uint32_t n_parts = 1;
+        if ((uint64_t)pc.pos + pc.ref_len > clen) {
+            cut = clen > pc.pos ? clen - pc.pos : 0;
+            n_parts = 2 + (uint32_t)((pc.ref_len - 1 - cut) / clen);
+        }
+        sink.segment(pc, clen);
+        aln_segment(a.ops + pc.op_off, pc.n_ops, cut, clen, n_parts, pc.out_rel, sink);
+    }
+}
+
+struct AlnCount {
+    uint32_t L;
+    uint32_t n_aln = 0, prim = 0, best = 0, q0 = 0, rf0 = 0, body = 0;
+    uint64_t words = 0;
+    __device__ void segment(const NsPieceMeta&, uint64_t) {}
+    __device__ void begin(uint32_t q, uint32_t rf) {
+        q0 = q;
+        rf0 = rf;
+        body = 0;
+    }
+    __device__ void op(uint32_t, uint32_t) { ++body; }
+    __device__ void end(uint32_t q1, uint32_t rf1) {
+        words += body + (q0 > 0) + (q1 < L);
+        if (rf1 - rf0 > best) {                                 // the longest span; the first of equal ones
+            best = rf1 - rf0;
+            prim = n_aln;
+        }
+        ++n_aln;
+    }
+};
+
+__global__ void aln_count_kernel(AlnArgs a) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n_reads) return;
+    const char* nm = a.names + a.name_off[i];
+    uint32_t nl = 0;
+    while (nm[nl]) ++nl;
+    a.name_len[i] = nl;
+    if (nl > BAM_MAX_NAME) atomicAdd(a.long_names, 1ull);
+    const NsReadMeta r = a.reads[i];
+    AlnCount c;
+    c.L = r.seq_len;
+    aln_read(a, r, c);
+    a.n_rec[i] = c.n_aln ? c.n_aln : 1;                         // no alignment: the unmapped record
+    a.n_cig[i] = c.words;
+    a.primary[i] = c.prim;
+}
+
+struct AlnWrite {
+    uint32_t i, L, nl, prim, rev;
+    BamAln* rec;                    // the read's records
+    uint32_t* cig;                  // its CIGAR words
+    uint64_t* size;
+    uint64_t cig_off;
+    uint32_t n_aln = 0, w = 0, w0 = 0, q0 = 0, rf0 = 0, chrom = 0, pos = 0;
+    uint64_t clen = 0;
+    __device__ void segment(const NsPieceMeta& pc, uint64_t len) {
+        chrom = pc.chrom;
+        pos = pc.pos;
+        clen = len;
+    }
+    __device__ void begin(uint32_t q, uint32_t rf) {
+        q0 = q;
+        rf0 = rf;
+        w0 = w;
+        if (q > 0) cig[w++] = (q << 4) | (n_aln == prim ? CIG_S : CIG_H);
+    }
+    __device__ void op(uint32_t kind, uint32_t len) { cig[w++] = (len << 4) | kind; }
+    __device__ void end(uint32_t q1, uint32_t rf1) {
+        const bool primary = n_aln == prim;
+        if (q1 < L) cig[w++] = ((L - q1) << 4) | (primary ? CIG_S : CIG_H);
+        BamAln b;
+        b.read = i;
+        b.q0 = primary ? 0 : q0;
+        b.l_seq = primary ? L : q1 - q0;
+        b.ref_id = chrom;
+        const uint64_t p = ((uint64_t)pos + rf0) % clen;       // a part behind a circular record's origin starts past it
+        b.pos = (uint32_t)p;
+        b.span = rf1 - rf0;
+        b.n_cig = w - w0;
+        b.bin = (uint16_t)bam_reg2bin(p, p + b.span);
+        b.flag = (uint16_t)((rev ? 16u : 0u) | (primary ? 0u : 0x800u));
+        b.cig_off = cig_off + w0;
+        rec[n_aln] = b;
+        size[n_aln] = bam_mapped_size(nl, b);
+        ++n_aln;
+    }
+};
+
+__global__ void aln_write_kernel(AlnArgs a) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n_reads) return;
+    const NsReadMeta r = a.reads[i];
+    const uint64_t r0 = a.rec_first[i];
+    AlnWrite s;
+    s.i = i;
+    s.L = r.seq_len;
+    s.nl = a.name_len[i];
+    s.prim = a.primary[i];
+    s.rev = r.reversed;
+    s.rec = a.aln + r0;
+    s.cig_off = a.cig_first[i];
+    s.cig = a.cigar + s.cig_off;
+    s.size = a.rec_size + r0;
+    aln_read(a, r, s);
+    if (s.n_aln == 0) {                                         // the unmapped record of ns_compress_bam
+        BamAln b{};
+        b.read = i;
+        b.l_seq = r.seq_len;
+        b.flag = 4;
+        a.aln[r0] = b;
+        a.rec_size[r0] = BgzfBamLayout::size(s.nl, r.seq_len, 0);
+    }
+}

@@ -5,6 +5,7 @@
 // brings the block's text into shared memory and cuts it into tokens:
 //   BgzfRecords<BgzfTextLayout>  ns_compress_records: the last batch's FASTA/FASTQ text, as ns_format_records lays it out
 //   BgzfRecords<BgzfBamLayout>   ns_compress_bam: the last batch's BAM records
+//   BgzfRecords<BgzfMappedLayout> ns_compress_bam_mapped: the last aligned batch's mapped BAM records (aln_kernel.cuh)
 //   BgzfRows                     ns_compress_error_profile: the error profile's rows, flat in HBM
 //
 // Records are literals only: simulated bases and qualities leave LZ77 almost nothing to find.  Such a member is the
@@ -181,27 +182,51 @@ __device__ __forceinline__ void bgzf_or_bits(uint32_t* out, uint64_t& pos, uint3
 // records: one per read of the last batch, in a layout's bytes
 // ---------------------------------------------------------------------------------------------------------------------
 
+// one read's record as the text and BAM layouts see it: its name (nl bytes), its bases and qualities (L each; ql null
+// without --fastq)
+struct BgzfReadRec {
+    const char* nm;
+    const uint8_t* sq;
+    const uint8_t* ql;
+    uint32_t nl, L, fastq;
+};
+// the records of the text and BAM layouts: one per read of the batch
+struct BgzfReadTable {
+    const NsReadMeta* reads;
+    const uint8_t* seq;
+    const uint8_t* qual;
+    const char* names;
+    const uint64_t* name_off;
+    const uint32_t* name_len;
+    uint32_t fastq;
+    __device__ __forceinline__ BgzfReadRec operator[](uint32_t r) const {
+        const NsReadMeta rm = reads[r];
+        return BgzfReadRec{names + name_off[r], seq + rm.seq_off, fastq ? qual + rm.seq_off : nullptr, name_len[r], rm.seq_len, fastq};
+    }
+};
+
 // FASTA/FASTQ text (host_io.cu:format_records_impl): '>' name '\n' seq '\n', FASTQ '@' name '\n' seq '\n' '+' '\n' qual '\n'
 struct BgzfTextLayout {
+    using Table = BgzfReadTable;
     static constexpr uint32_t max_name = 0;                     // names of any length
     static __device__ __forceinline__ uint64_t size(uint32_t nl, uint64_t L, uint32_t fastq) {
         return fastq ? 1 + nl + 1 + L + 1 + 2 + L + 1 : 1 + nl + 1 + L + 1;
     }
-    // byte q of a record (name at `nm`, nl bytes; bases and qualities at `sq` / `ql`, L each)
-    static __device__ __forceinline__ uint8_t byte(uint64_t q, uint32_t fastq, const char* nm, uint32_t nl, const uint8_t* sq,
-                                                   const uint8_t* ql, uint32_t L) {
+    // byte q of a record
+    static __device__ __forceinline__ uint8_t byte(uint64_t q, const BgzfReadRec& rc) {
+        const uint32_t nl = rc.nl, L = rc.L, fastq = rc.fastq;
         if (q == 0) return fastq ? '@' : '>';
-        if (q <= nl) return (uint8_t)nm[q - 1];
+        if (q <= nl) return (uint8_t)rc.nm[q - 1];
         q -= nl + 1;
         if (q == 0) return '\n';
         q -= 1;
-        if (q < L) return sq[q];
+        if (q < L) return rc.sq[q];
         q -= L;
         if (q == 0 || !fastq) return '\n';
         if (q == 1) return '+';
         if (q == 2) return '\n';
         q -= 3;
-        return q < L ? ql[q] : '\n';
+        return q < L ? rc.ql[q] : '\n';
     }
 };
 
@@ -236,13 +261,14 @@ __device__ __forceinline__ uint32_t bam_base_code(uint8_t c) {
 }
 
 struct BgzfBamLayout {
+    using Table = BgzfReadTable;
     static constexpr uint32_t max_name = BAM_MAX_NAME;          // a longer name fails the call
     static __device__ __forceinline__ uint64_t size(uint32_t nl, uint64_t L, uint32_t) {
         return BAM_FIXED + nl + 1 + (L + 1) / 2 + L;
     }
-    // byte q of a read's BAM record, arguments as for BgzfTextLayout::byte
-    static __device__ __forceinline__ uint8_t byte(uint64_t q, uint32_t fastq, const char* nm, uint32_t nl, const uint8_t* sq,
-                                                   const uint8_t* ql, uint32_t L) {
+    // byte q of a read's BAM record
+    static __device__ __forceinline__ uint8_t byte(uint64_t q, const BgzfReadRec& rc) {
+        const uint32_t nl = rc.nl, L = rc.L;
         if (q < BAM_FIXED) {
             uint32_t w;
             switch ((uint32_t)q >> 2) {
@@ -256,16 +282,16 @@ struct BgzfBamLayout {
             return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
         }
         q -= BAM_FIXED;
-        if (q < nl) return (uint8_t)nm[q];
+        if (q < nl) return (uint8_t)rc.nm[q];
         if (q == nl) return 0;
         q -= nl + 1;
         const uint64_t n_packed = (L + 1) / 2;
         if (q < n_packed) {
             const uint64_t b = 2 * q;
-            return (uint8_t)((bam_base_code(sq[b]) << 4) | (b + 1 < L ? bam_base_code(sq[b + 1]) : 0u));
+            return (uint8_t)((bam_base_code(rc.sq[b]) << 4) | (b + 1 < L ? bam_base_code(rc.sq[b + 1]) : 0u));
         }
         q -= n_packed;
-        return fastq ? (uint8_t)(ql[q] - 33) : 0xffu;
+        return rc.fastq ? (uint8_t)(rc.ql[q] - 33) : 0xffu;
     }
 };
 
@@ -285,39 +311,30 @@ __global__ void record_size_kernel(const NsReadMeta* __restrict__ reads, uint32_
     size[i] = Layout::size(nl, reads[i].seq_len, fastq);
 }
 
-// bgzf_deflate_kernel's source of records in `Layout`, every byte a literal
+// bgzf_deflate_kernel's source of records in `Layout`, every byte a literal.  Record r is tab[r] (Layout::Table), its
+// bytes Layout::byte(q, tab[r]).
 template <class Layout>
 struct BgzfRecords {
     static constexpr int NLL = BGZF_SYMS, ND = 2;
     using Smem = BgzfSmem<NLL, ND>;
-    const NsReadMeta* reads;
-    const uint8_t* seq;
-    const uint8_t* qual;
-    const char* names;
-    const uint64_t* name_off;
-    const uint32_t* name_len;
+    typename Layout::Table tab;
     const uint64_t* rec_off;        // exclusive prefix sum of the record sizes
-    uint32_t n_reads;
-    uint32_t fastq;
+    uint32_t n_recs;
 
     // gather this thread's span [lo, hi) of the block at t0
     __device__ __forceinline__ void load(Smem& s, uint64_t t0, uint64_t text_bytes, uint32_t, uint32_t lo, uint32_t hi) {
         if (lo >= hi) return;
         uint64_t p = t0 + lo;
-        uint32_t rl = 0, rh = n_reads;                          // last record with rec_off <= p
+        uint32_t rl = 0, rh = n_recs;                           // last record with rec_off <= p
         while (rh - rl > 1) {
             const uint32_t mid = (rl + rh) >> 1;
             if (rec_off[mid] <= p) rl = mid; else rh = mid;
         }
         uint32_t k = lo;
         for (uint32_t r = rl; k < hi; ++r) {                    // the records this span overlaps
-            const uint64_t r0 = rec_off[r], r1 = r + 1 < n_reads ? rec_off[r + 1] : text_bytes;
-            const NsReadMeta rm = reads[r];
-            const char* nm = names + name_off[r];
-            const uint32_t nl = name_len[r];
-            const uint8_t* sq = seq + rm.seq_off;
-            const uint8_t* ql = fastq ? qual + rm.seq_off : nullptr;
-            for (; k < hi && p < r1; ++k, ++p) s.text[k] = Layout::byte(p - r0, fastq, nm, nl, sq, ql, rm.seq_len);
+            const uint64_t r0 = rec_off[r], r1 = r + 1 < n_recs ? rec_off[r + 1] : text_bytes;
+            const auto rc = tab[r];
+            for (; k < hi && p < r1; ++k, ++p) s.text[k] = Layout::byte(p - r0, rc);
         }
     }
     // thread t's tokens start at its byte span

@@ -29,6 +29,7 @@
 #include "hp_kernel.cuh"
 #include "bgzf_kernel.cuh"
 #include "errprof_kernel.cuh"
+#include "aln_kernel.cuh"
 #include "haplotype.h"
 #include "host_io.h"
 
@@ -171,6 +172,9 @@ struct NsContext {
     DevBuf ep_text, ep_out;
     uint64_t ep_bytes = 0;
     bool have_ep = false;
+    // ns_compress_bam_mapped: per read its record and CIGAR-word counts (2n) and their offsets (2n), its primary alignment;
+    // the records' descriptors and CIGAR words.  Its members go to z_out.
+    DevBuf m_cnt, m_first, m_prim, m_aln, m_cig;
     // Batches of one job have near-identical sizes: once a batch of a kind has run with host-sized buffers, the next ones
     // are submitted in one go (no host round trip between the first and the last kernel) against those capacities; a
     // kernel checks them on the device and a batch that does not fit is simply run again the sized way.
@@ -1664,6 +1668,19 @@ static int fetch_members(NsContext* ctx, const char* fname, bool have, const Dev
     return NS_OK;
 }
 
+// the last batch's reads with the names upload_names left on the device
+static BgzfReadTable read_table(NsContext* ctx) {
+    BgzfReadTable t;
+    t.fastq = ctx->hcfg.fastq ? 1u : 0u;
+    t.reads = ctx->reads.as<NsReadMeta>();
+    t.seq = ctx->seq.as<uint8_t>();
+    t.qual = t.fastq ? ctx->qual.as<uint8_t>() : nullptr;
+    t.names = ctx->z_names.as<char>();
+    t.name_off = ctx->z_name_off.as<uint64_t>();
+    t.name_len = ctx->z_name_len.as<uint32_t>();
+    return t;
+}
+
 extern "C++" {    // templates cannot have C linkage
 
 // the n_blocks members of the text `src` brings into shared memory
@@ -1710,15 +1727,9 @@ static int compress_records(NsContext* ctx, const char* fname, const char* names
     uint32_t n_blocks = 0;
     if (int rc = stage_members(ctx, fname, text, &zm, &n_blocks)) return rc;
     BgzfRecords<Layout> src;
-    src.reads = ctx->reads.as<NsReadMeta>();
-    src.seq = ctx->seq.as<uint8_t>();
-    src.qual = fastq ? ctx->qual.as<uint8_t>() : nullptr;
-    src.names = ctx->z_names.as<char>();
-    src.name_off = ctx->z_name_off.as<uint64_t>();
-    src.name_len = ctx->z_name_len.as<uint32_t>();
+    src.tab = read_table(ctx);
     src.rec_off = ctx->z_rec_off.as<uint64_t>();
-    src.n_reads = n;
-    src.fastq = fastq;
+    src.n_recs = n;
     if (int rc = deflate_members(ctx, src, zm, n_blocks)) return rc;
     uint64_t total = 0;
     if (int rc = pack_members(ctx, fname, n_blocks, ctx->z_out, &total)) return rc;
@@ -1736,6 +1747,87 @@ int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_
 
 int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
     return compress_records<BgzfBamLayout>(ctx, "ns_compress_bam", names, name_off, nbytes);
+}
+
+int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    static const char* fname = "ns_compress_bam_mapped";
+    if (!ctx) return NS_EINVAL;
+    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
+    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
+    if (ctx->last_kind != NS_KIND_ALIGNED) return fail(ctx, NS_EINVAL, "%s: the last batch is unaligned reads, which have no alignment", fname);
+    if (ctx->hcfg.mode == 2)
+        return fail(ctx, NS_EINVAL, "%s: transcriptome reads are not written as mapped records", fname);
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t n = ctx->last.n_reads;
+    ctx->have_z = false;
+    ctx->z_bytes = 0;
+    if (n == 0) {
+        ctx->have_z = true;
+        *nbytes = 0;
+        return NS_OK;
+    }
+    if (int rc = upload_names(ctx, names, name_off, n)) return rc;
+    CK(ctx->m_cnt.ensure((size_t)2 * n * sizeof(uint64_t)));
+    CK(ctx->m_first.ensure((size_t)2 * n * sizeof(uint64_t)));
+    CK(ctx->m_prim.ensure((size_t)n * sizeof(uint32_t)));
+    uint64_t* totals = ctx->totals.as<uint64_t>();
+    AlnArgs aa{};
+    aa.reads = ctx->reads.as<NsReadMeta>();
+    aa.pieces = ctx->pieces.as<NsPieceMeta>();
+    aa.ops = ctx->ops.as<uint32_t>();
+    aa.chrom_off = ctx->tables->dref.chrom_off;
+    aa.names = ctx->z_names.as<char>();
+    aa.name_off = ctx->z_name_off.as<uint64_t>();
+    aa.n_reads = n;
+    aa.name_len = ctx->z_name_len.as<uint32_t>();
+    aa.n_rec = ctx->m_cnt.as<uint64_t>();
+    aa.n_cig = aa.n_rec + n;
+    aa.primary = ctx->m_prim.as<uint32_t>();
+    aa.long_names = (unsigned long long*)(totals + NS_T_Z_LONG_NAMES);
+    const unsigned grid = (n + 255) / 256;
+    CK(launch(ctx, aln_count_kernel, grid, 256, 0, aa));
+    // the record and CIGAR-word totals borrow the text and member-bytes slots, which the later scans overwrite
+    uint64_t* rec_first = ctx->m_first.as<uint64_t>();
+    if (int rc = scan_total(ctx, aa.n_rec, rec_first, n, NS_T_Z_TEXT)) return rc;
+    if (int rc = scan_total(ctx, aa.n_cig, rec_first + n, n, NS_T_Z_BYTES)) return rc;
+    if (int rc = publish_totals_and_wait(ctx)) return rc;
+    const uint64_t* h = ctx->h_totals.as<uint64_t>();
+    if (const uint64_t n_long = h[NS_T_Z_LONG_NAMES]) {
+        uint32_t i = 0;                                         // the first such name, for the message
+        while (i + 1 < n && strlen(names + name_off[i]) <= BAM_MAX_NAME) ++i;
+        return fail(ctx, NS_EINVAL, "%s: read %u has a name of %zu bytes, more than the %u BAM holds (%llu such reads)", fname, i,
+                    strlen(names + name_off[i]), BAM_MAX_NAME, (unsigned long long)n_long);
+    }
+    const uint64_t n_rec = h[NS_T_Z_TEXT], n_words = h[NS_T_Z_BYTES];
+    if (n_rec > 0xffffffffu) return fail(ctx, NS_EINVAL, "%s: %llu records are too many for one call", fname, (unsigned long long)n_rec);
+    CK(ctx->m_aln.ensure((size_t)n_rec * sizeof(BamAln)));
+    CK(ctx->m_cig.ensure((size_t)std::max<uint64_t>(n_words, 1) * sizeof(uint32_t)));
+    CK(ctx->scan_in.ensure((size_t)n_rec * sizeof(uint64_t)));
+    CK(ctx->z_rec_off.ensure((size_t)n_rec * sizeof(uint64_t)));
+    aa.rec_first = rec_first;
+    aa.cig_first = rec_first + n;
+    aa.aln = ctx->m_aln.as<BamAln>();
+    aa.cigar = ctx->m_cig.as<uint32_t>();
+    aa.rec_size = ctx->scan_in.as<uint64_t>();
+    CK(launch(ctx, aln_write_kernel, grid, 256, 0, aa));
+    if (int rc = scan_total(ctx, aa.rec_size, ctx->z_rec_off.as<uint64_t>(), (uint32_t)n_rec, NS_T_Z_TEXT)) return rc;
+    if (int rc = publish_totals_and_wait(ctx)) return rc;
+    BgzfMembers zm;
+    uint32_t n_blocks = 0;
+    if (int rc = stage_members(ctx, fname, h[NS_T_Z_TEXT], &zm, &n_blocks)) return rc;
+    BgzfRecords<BgzfMappedLayout> src;
+    src.tab.reads = read_table(ctx);
+    src.tab.aln = aa.aln;
+    src.tab.cigar = aa.cigar;
+    src.rec_off = ctx->z_rec_off.as<uint64_t>();
+    src.n_recs = (uint32_t)n_rec;
+    if (int rc = deflate_members(ctx, src, zm, n_blocks)) return rc;
+    uint64_t total = 0;
+    if (int rc = pack_members(ctx, fname, n_blocks, ctx->z_out, &total)) return rc;
+    ctx->z_bytes = total;
+    ctx->have_z = true;
+    *nbytes = total;
+    return NS_OK;
 }
 
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap) {

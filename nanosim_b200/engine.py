@@ -283,8 +283,23 @@ class Engine:
         self._z_bytes = int(n.value)
         return self._z_bytes
 
+    def compress_bam_mapped(self, names):
+        """The last aligned batch as mapped BAM records, the true alignment of every read (``names`` as for compress_bam),
+        as BGZF members built on the device and kept there (ns_compress_bam_mapped); they replace those of the last
+        compress_records() / compress_bam().  Returns their size in bytes; neither the BAM header nor the end-of-file
+        block."""
+        from .records import _name_blob
+        blob, offs = _name_blob(names)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        if len(offs) != int(self.info.n_reads):
+            raise ValueError("compress_bam_mapped: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
+        n = C.c_uint64()
+        self._check(self._lib.ns_compress_bam_mapped(self._ctx, blob, _ptr(offs), C.byref(n)))
+        self._z_bytes = int(n.value)
+        return self._z_bytes
+
     def fetch_compressed(self, out=None):
-        """The members of the last compress_records() or compress_bam() -> uint8 array (into ``out`` when given: a
+        """The members of the last compress_records(), compress_bam() or compress_bam_mapped() -> uint8 array (into ``out`` when given: a
         uint8 array, pinned memory recommended, at least that large)."""
         if out is None:
             out = np.empty(self._z_bytes, dtype=np.uint8)

@@ -171,7 +171,7 @@ class MetaReference(PackedReference):
 
     @staticmethod
     def from_genome_list(genome_list, dna_type_list=None):
-        genomes = []
+        genomes, raw_names = [], []
         with open(genome_list) as f:
             for line in f.readlines():
                 if not line.strip():
@@ -183,6 +183,7 @@ class MetaReference(PackedReference):
                 one = PackedReference.from_fasta(path)
                 recs = [(k, one.bases[int(one.offsets[i]):int(one.offsets[i + 1])]) for i, k in enumerate(one.names)]
                 genomes.append((fields[0], recs))
+                raw_names += one.raw_names
         types = {}
         known = {MetaReference.species_key(g[0]) for g in genomes}
         if dna_type_list:
@@ -195,7 +196,9 @@ class MetaReference(PackedReference):
                     if sp not in known:
                         raise KeyError("You didn't provide a reference genome for " + sp)
                     types.setdefault(sp, {})[normalise_name(fields[1])] = fields[2].strip("\n")
-        return MetaReference.from_genomes(genomes, types)
+        m = MetaReference.from_genomes(genomes, types)
+        m.raw_names = raw_names              # FASTA headers up to the first blank: the names a mapped BAM gives the records
+        return m
 
 
 def read_abundance(path, species):

@@ -33,6 +33,7 @@ from .model import build_alias
 VERSION = "3.2.2-b200"
 
 # BGZF end-of-file marker: an empty member (SAM/BAM format specification §4.1.2), once at the end of every .gz file
+BGZF_HEADER_BLOCK = 56 << 10     # header bytes per member: zlib's output for them stays below the 64 KiB BGZF allows
 BGZF_EOF = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")
 ERR_HEADER = b"Seq_name\tSeq_pos\terror_type\terror_length\tref_base\tseq_base\n"      # first line of the error profile (:1634)
 
@@ -45,11 +46,39 @@ def bgzf_member(text):
             struct.pack("<II", zlib.crc32(text), len(text)))
 
 
-def bam_header():
-    """The BAM header of ``--bam`` files as one BGZF member: magic, the @HD and @PG lines, no reference sequences.  It
-    carries no command line, so the decompressed file depends only on the simulated reads."""
-    text = b"@HD\tVN:1.6\tSO:unknown\n@PG\tID:NanoSim\tPN:NanoSim\tVN:" + VERSION.encode() + b"\n"
-    return bgzf_member(b"BAM\1" + struct.pack("<i", len(text)) + text + struct.pack("<i", 0))
+def bam_header(refs=None):
+    """The BAM header of ``--bam`` files: magic, the @HD and @PG lines, no reference sequences, as one BGZF member.  It
+    carries no command line, so the decompressed file depends only on the simulated reads.  refs (``--mapped_bam``): the
+    reference records as (name, length, circular), which get one @SQ line each (``TP:circular`` on circular ones) and the
+    binary reference list; that header is cut into members of at most BGZF_HEADER_BLOCK bytes."""
+    refs = refs or []
+    sq = b"".join(b"@SQ\tSN:%s\tLN:%d%s\n" % (n.encode(), ln, b"\tTP:circular" if c else b"") for n, ln, c in refs)
+    text = b"@HD\tVN:1.6\tSO:unknown\n" + sq + b"@PG\tID:NanoSim\tPN:NanoSim\tVN:" + VERSION.encode() + b"\n"
+    raw = b"BAM\1" + struct.pack("<i", len(text)) + text + struct.pack("<i", len(refs))
+    raw += b"".join(struct.pack("<i", len(n.encode()) + 1) + n.encode() + b"\0" + struct.pack("<i", ln) for n, ln, _ in refs)
+    return b"".join(bgzf_member(raw[k:k + BGZF_HEADER_BLOCK]) for k in range(0, len(raw), BGZF_HEADER_BLOCK))
+
+
+def bam_refs(ref, circular=False):
+    """The reference records of a mapped BAM header, as bam_header takes them: name (the FASTA header up to the first blank,
+    or a --vcf haplotype's name), length and whether the record is circular (``-dna_type circular``, or the metagenome's
+    DNA type list).  A name given to two records, and a record longer than BAM's int32 l_ref holds, are ValueErrors that
+    name the record."""
+    names, lengths = list(ref.raw_names), [int(x) for x in ref.lengths]
+    for i, ln in enumerate(lengths):
+        if ln > 0x7fffffff:
+            raise ValueError("reference record %d (%s) has %d bases, more than the %d a BAM header can state"
+                             % (i, ref.names[i], ln, 0x7fffffff))
+    circ = getattr(ref, "chrom_circular", None)
+    circ = [bool(c) for c in circ] if circ is not None else [bool(circular)] * len(names)
+    seen = {}
+    for i, n in enumerate(names):
+        if n in seen:
+            j = seen[n]
+            raise ValueError("reference records %d (%s) and %d (%s) have the same name %s: a mapped BAM cannot tell them apart"
+                             % (j, ref.names[j], i, ref.names[i], n))
+        seen[n] = i
+    return list(zip(names, lengths, circ))
 
 
 def _log(msg):
@@ -289,9 +318,11 @@ def _shard(n, rank, world):
 
 def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min_l, num_threads, fastq,
                median_l=None, sd_l=None, model_ir=False, uracil=False, polya=None, chimeric=False,
-               batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False, gzip_error_profile=False, bam=False):
+               batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False, gzip_error_profile=False, bam=False,
+               mapped_refs=None):
     """gzip: write the reads as BGZF (``.gz``), compressed on the GPU; bam: write them as unaligned BAM (``.bam``, one
-    unmapped record per read), encoded and compressed on the GPU.  The error profile stays plain text unless
+    unmapped record per read), encoded and compressed on the GPU.  mapped_refs (with bam; bam_refs' list): the aligned
+    reads are written as mapped records, their true alignments to those records (``--mapped_bam``).  The error profile stays plain text unless
     gzip_error_profile (needs gzip or bam): then it is formatted and compressed on the GPU too,
     ``<out>_aligned_error_profile.gz``, whose first member is the header line.  Under torchrun (world > 1) the per-rank
     files carry neither the headers nor the end-of-file block: merge_rank_files writes them."""
@@ -311,20 +342,22 @@ def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min
     suffix = "" if world == 1 else str(rank)
     want_err = error_profile and not per
     gz_err = (gzip or bam) and gzip_error_profile and want_err
-    pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err and not gz_err, compress_profile=gz_err, bam=bam)
+    pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err and not gz_err, compress_profile=gz_err, bam=bam,
+                         mapped_bam=mapped_refs is not None)
     totals = {"reads": 0, "bases": 0, "bytes": 0}
     try:
         _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                         gzip, gz_err, bam)
+                         gzip, gz_err, bam, mapped_refs)
     finally:
         pipe.close()         # the cloned contexts own device batch buffers and pinned staging
     return totals            # what this rank simulated and wrote (the reference returns nothing)
 
 
 def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                     gzip=False, gz_err=False, bam=False):
+                     gzip=False, gz_err=False, bam=False, mapped_refs=None):
     packed = gzip or bam            # the records are compressed on the device: the batches arrive as BGZF members
     reads_header = bam_header() if bam and world == 1 else b""
+    aligned_header = bam_header(mapped_refs) if mapped_refs is not None and world == 1 else reads_header
 
     def jobs(kind, lo, hi):
         return [(kind, start, min(batch_reads, hi - start)) for start in range(lo, hi, batch_reads)]
@@ -364,7 +397,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
 
     _log("Start simulation of aligned reads")
     lo, hi = _shard(prof.number_aligned, rank, world)
-    f_reads = _Out(out + "_aligned_reads" + suffix + ext, reads_header)
+    f_reads = _Out(out + "_aligned_reads" + suffix + ext, aligned_header)
     f_err = _Out(out + ("_aligned_error_profile" if world == 1 else "_error_profile" + suffix) + (".gz" if gz_err else ""),
                  b"" if world > 1 else bgzf_member(ERR_HEADER) if gz_err else ERR_HEADER)
     try:
@@ -422,15 +455,17 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             f_un.close()
 
 
-def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=False, bam=False):
+def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=False, bam=False, mapped_refs=None):
     """Rank 0: concatenate per-rank sub-files in rank order and delete them (:1626-1639, :1667-1672).  gzip: the reads
     files are BGZF members without an end-of-file block; the merged file gets it once, at its end.  bam: so are the
-    ``.bam`` reads files, and the merged ones start with the BAM header's member.  gzip_error_profile: so are the
-    error-profile files (``_error_profile{r}.gz``); the merged one starts with the header line's member."""
+    ``.bam`` reads files, and the merged ones start with the BAM header's members (with mapped_refs' @SQ lines for the
+    aligned reads).  gzip_error_profile: so are the error-profile files (``_error_profile{r}.gz``); the merged one starts
+    with the header line's member."""
     ext = ".bam" if bam else (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
     header = bam_header() if bam else b""
     trailer = BGZF_EOF if gzip or bam else b""
-    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, header, trailer)]
+    aligned_header = bam_header(mapped_refs) if bam and mapped_refs is not None else header
+    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, aligned_header, trailer)]
     if gzip_error_profile:
         jobs.append(("_error_profile%d.gz", "_aligned_error_profile.gz", bgzf_member(ERR_HEADER), BGZF_EOF))
     else:
@@ -460,6 +495,9 @@ GZIP_ERR_HELP = ('With --gzip or --bam: write the error profile as BGZF-compress
 BAM_HELP = ('Write the reads as unaligned BAM, <out>_aligned_reads.bam and <out>_unaligned_reads.bam (one unmapped record per '
             'read, as Dorado writes them), encoded and compressed on the GPU. The error profile stays plain text unless '
             '--gzip_error_profile is given (Default = False)')
+MAPPED_BAM_HELP = ('With --bam: write <out>_aligned_reads.bam as mapped records, the true alignment of every aligned read to the '
+                   'reference records (one record per segment, supplementary ones for chimeric reads, CIGAR from the simulated '
+                   'errors), built on the GPU. <out>_unaligned_reads.bam is unchanged (Default = False)')
 VCF_HELP = ('Simulate the reads from the haplotypes of the first sample of this VCF (plain or .vcf.gz), built on the GPU from '
             'the reference: records <chrom>-hap1 and <chrom>-hap2 (one copy for a haploid GT). Only FILTER PASS or . records '
             'are applied. -x still counts the haploid reference, so -x 30 is about 15x per haplotype')
@@ -516,6 +554,7 @@ def build_parser():
     g.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     g.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     g.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
+    g.add_argument('--mapped_bam', help=MAPPED_BAM_HELP, action='store_true', default=False)
     g.add_argument('--vcf', help=VCF_HELP, default=None)
     mg = sub.add_parser('metagenome', help="Run the simulator on metagenome mode")
     mg.add_argument('-gl', '--genome_list', help="Reference metagenome list, tsv file, the first column is species/strain "
@@ -552,6 +591,7 @@ def build_parser():
     mg.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     mg.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     mg.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
+    mg.add_argument('--mapped_bam', help=MAPPED_BAM_HELP, action='store_true', default=False)
     t = sub.add_parser('transcriptome', help="Run the simulator on transcriptome mode")
     t.add_argument('-rt', '--ref_t', help='Input reference transcriptome', required=True)
     t.add_argument('-rg', '--ref_g', help='Input reference genome, required if intron retention simulation is on', default='')
@@ -593,6 +633,7 @@ def build_parser():
     t.add_argument('--gzip', help=GZIP_HELP, action='store_true', default=False)
     t.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     t.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
+    t.add_argument('--mapped_bam', help=argparse.SUPPRESS, action='store_true', default=False)     # a usage error here
     return parser, g, mg, t
 
 
@@ -704,6 +745,7 @@ def main_metagenome(args, parser_mg):
     prof = read_profile(args.genome_list, [], args.model_prefix, args.perfect, "metagenome", args.strandness,
                         dna_type=args.dna_type_list, abun=args.abun, chimeric=args.chimeric, homopolymer=args.homopolymer,
                         fastq=args.fastq, device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args))
+    mapped_refs = _mapped_refs(args, prof, False)
     rnd = random.Random(args.seed)
     L_ = prof.ref.lengths
     total_len = [int(L_[prof.ref.chrom_species == i].sum()) for i in range(len(prof.ref.species))]
@@ -719,7 +761,7 @@ def main_metagenome(args, parser_mg):
         simulation(prof, "metagenome", args.output + "_sample%d" % s_idx, "metagenome", args.perfect, None, None, max_len,
                    min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len, chimeric=args.chimeric,
                    batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world, gzip=args.gzip,
-                   gzip_error_profile=args.gzip_error_profile, bam=args.bam)
+                   gzip_error_profile=args.gzip_error_profile, bam=args.bam, mapped_refs=mapped_refs)
         if world > 1:
             import torch.distributed as dist
             if not dist.is_initialized():
@@ -727,7 +769,7 @@ def main_metagenome(args, parser_mg):
             dist.barrier()
             if rank == 0:
                 merge_rank_files(args.output + "_sample%d" % s_idx, args.fastq, args.perfect, world, gzip=args.gzip,
-                                 gzip_error_profile=args.gzip_error_profile, bam=args.bam)
+                                 gzip_error_profile=args.gzip_error_profile, bam=args.bam, mapped_refs=mapped_refs)
             dist.barrier()
     _log("Finished!")
 
@@ -744,6 +786,17 @@ def coverage_to_reads(prof, cm, coverage):
     return int(ref_len / mean * coverage)
 
 
+def _mapped_refs(args, prof, circular):
+    """--mapped_bam: bam_refs of the resident reference, None without the flag; a repeated name is a usage error."""
+    if not args.mapped_bam:
+        return None
+    try:
+        return bam_refs(prof.ref, circular)
+    except ValueError as e:
+        sys.stderr.write("\n--mapped_bam: %s!\n" % e)
+        sys.exit(1)
+
+
 def main(argv=None):
     parser, parser_g, parser_mg, parser_t = build_parser()
     args = parser.parse_args(argv)
@@ -757,6 +810,10 @@ def main(argv=None):
         usage = "--bam cannot be combined with --uracil: BAM has no code for U"
     elif args.gzip_error_profile and not (args.gzip or args.bam):
         usage = "--gzip_error_profile needs --gzip or --bam"
+    elif args.mapped_bam and args.mode == "transcriptome":
+        usage = "--mapped_bam is not available in transcriptome mode: reads that retain an intron lie on the genome"
+    elif args.mapped_bam and not args.bam:
+        usage = "--mapped_bam needs --bam"
     if usage:
         sys.stderr.write("\n" + usage + "!\n")
         {"genome": parser_g, "metagenome": parser_mg, "transcriptome": parser_t}[args.mode].print_help(sys.stderr)
@@ -813,10 +870,12 @@ def main(argv=None):
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
     max_len = min(max_len, prof.max_chrom)
+    mapped_refs = _mapped_refs(args, prof, args.dna_type == "circular")
     simulation(prof, args.mode, args.output, args.dna_type, args.perfect, args.KmerBias if args.homopolymer else None,
                None, max_len, min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len,
                chimeric=args.chimeric, batch_reads=args.batch_reads, error_profile=not args.no_error_profile,
-               rank=rank, world=world, gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam)
+               rank=rank, world=world, gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam,
+               mapped_refs=mapped_refs)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
@@ -824,7 +883,7 @@ def main(argv=None):
         dist.barrier()
         if rank == 0:
             merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip,
-                             gzip_error_profile=args.gzip_error_profile, bam=args.bam)
+                             gzip_error_profile=args.gzip_error_profile, bam=args.bam, mapped_refs=mapped_refs)
         dist.barrier()
     _log("Finished!")
 

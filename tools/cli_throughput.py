@@ -4,7 +4,9 @@ reference, writing into /dev/shm when it exists.  Bases are counted from the rea
 every ns_compress_records call is reported too, and with --gzip_error_profile that of every ns_compress_error_profile call
 (both calls end in a device synchronise) and the profile's compressed / plain ratio, next to zlib levels 1 and 6 on the
 text of its first 1024 members (decompressed and compressed again on the CPU after the run).  With --bam every
-ns_compress_bam call is timed, and the bases of a ``.bam`` file are the sum of its records' l_seq (read after the run)."""
+ns_compress_bam call is timed, and the bases of a ``.bam`` file are the sum of its records' l_seq (read after the run; the
+primary records only, so that --mapped_bam's supplementary records are not counted twice).  With --mapped_bam every
+ns_compress_bam_mapped call is timed."""
 import os, shutil, struct, sys, time, tempfile, zlib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -29,7 +31,7 @@ def text_bytes(path):
 
 
 def bam_bases(path):
-    """Bases of a .bam reads file: the sum of its records' l_seq, inflating one BGZF member at a time."""
+    """Bases of a .bam reads file: the sum of its primary records' l_seq, inflating one BGZF member at a time."""
     total, buf, pos, header = 0, b"", 0, True
     with open(path, "rb") as f:
         while True:
@@ -39,14 +41,22 @@ def bam_bases(path):
             size = struct.unpack("<H", h[16:18])[0] + 1
             buf = buf[pos:] + zlib.decompress(f.read(size - 18)[:-8], -15)
             pos = 0
-            if header and len(buf) >= 8:
-                l_text = struct.unpack_from("<i", buf, 4)[0]
-                pos, header = 8 + l_text + 4, False          # magic, l_text, text, n_ref = 0
+            if header and len(buf) >= 8 and len(buf) >= 12 + struct.unpack_from("<i", buf, 4)[0]:
+                pos = 12 + struct.unpack_from("<i", buf, 4)[0]       # magic, l_text, text, n_ref, then the reference list
+                n_ref = struct.unpack_from("<i", buf, pos - 4)[0]
+                while n_ref and pos + 4 <= len(buf) and pos + 8 + struct.unpack_from("<i", buf, pos)[0] <= len(buf):
+                    pos += 8 + struct.unpack_from("<i", buf, pos)[0]
+                    n_ref -= 1
+                if n_ref:                                               # the list goes on in the next member
+                    pos = 0
+                    continue
+                header = False
             while not header and pos + 24 <= len(buf):
                 block = struct.unpack_from("<i", buf, pos)[0]
                 if pos + 4 + block > len(buf):
                     break
-                total += struct.unpack_from("<i", buf, pos + 20)[0]
+                if not struct.unpack_from("<H", buf, pos + 18)[0] & 0x800:
+                    total += struct.unpack_from("<i", buf, pos + 20)[0]
                 pos += 4 + block
 
 
@@ -66,7 +76,7 @@ def profile_sample(path, n_members=1024):
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 300000
 extra = sys.argv[2:]
-timings = {"ns_compress_records": [], "ns_compress_bam": [], "ns_compress_error_profile": []}
+timings = {"ns_compress_records": [], "ns_compress_bam": [], "ns_compress_bam_mapped": [], "ns_compress_error_profile": []}
 
 
 def timed(fn, key):
@@ -81,6 +91,7 @@ def timed(fn, key):
 
 Engine.compress_records = timed(Engine.compress_records, "ns_compress_records")
 Engine.compress_bam = timed(Engine.compress_bam, "ns_compress_bam")
+Engine.compress_bam_mapped = timed(Engine.compress_bam_mapped, "ns_compress_bam_mapped")
 Engine.compress_error_profile = timed(Engine.compress_error_profile, "ns_compress_error_profile")
 tmp = tempfile.mkdtemp(prefix="cli_tp_", dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
 try:
