@@ -260,6 +260,15 @@ typedef struct {
  * haplotype h (what ns_set_reference does with them: 2-bit copy, chromosome checks); the haploid bytes are freed.  Call
  * after ns_set_reference (or ns_bcast_nccl) and before ns_clone; NS_ESTATE on a clone.  Genome references only. */
 int ns_apply_variants(NsContext* ctx, const NsVariants* variants);
+/* Keeps, with the tables the context and its clones share, the lift of the resident haplotype records onto the haploid
+ * records they were built from, so that ns_compress_bam_mapped writes lifted records (DESIGN §3 "Lifted mapped BAM").
+ * `variants` are the tables ns_apply_variants was given; they get its checks, and NS_EINVAL (naming the haplotype) when
+ * their haplotypes do not have the resident records' lengths.  One segment per stretch and per ALT (ns_apply_variants'
+ * segmentation), built on the device.  A haplotype's HP value is its place among the haplotypes of its source record
+ * (1, 2).  peak_bytes, when given, receives the device bytes the lift keeps.  Call after ns_apply_variants and before
+ * ns_clone; NS_ESTATE on a clone or when the resident reference is not ns_apply_variants' haplotypes.  A later
+ * ns_set_reference or ns_apply_variants drops the lift. */
+int ns_set_lift(NsContext* ctx, const NsVariants* variants);
 
 int ns_configure(NsContext* ctx, const NsRunConfig* cfg);
 /* metagenome: dict_abun / dict_abun_inflated of the current sample (main() :2497-2514), one value per species in
@@ -403,8 +412,11 @@ int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off,
  * than 65 535 ops (the CIGAR field then reads <l_seq>S<span>N).  A read with no alignment gets ns_compress_bam's unmapped
  * record.  The CIGAR rules are in DESIGN.md §3 "Mapped BAM".  Same name layout and 254-byte name limit as ns_compress_bam;
  * neither header nor end-of-file block.  The members replace those of the last ns_compress_records / ns_compress_bam;
- * ns_fetch_compressed copies them.  NS_EINVAL when the last batch is unaligned reads or the context is in transcriptome
- * mode. */
+ * ns_fetch_compressed copies them.  When the context's tables carry a lift (ns_set_lift), the records are lifted onto the
+ * haploid reference: refID is the haplotype's source record, POS is on it, a part inside an <INV> is a record on the
+ * other strand, and every mapped record has HP:C:<1 or 2> as its first aux field (DESIGN.md §3 "Lifted mapped BAM").
+ * NS_EINVAL when the last batch is unaligned reads, the context is in transcriptome mode, or a lift meets a circular
+ * configuration. */
 int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
 /* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' (or ns_compress_bam's)
  * *nbytes. */

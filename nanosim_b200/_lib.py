@@ -25,7 +25,7 @@ NS_STATS_WORDS = NS_STATS_COMP_OFF + 4
 EXPORTS = ["ns_create", "ns_destroy", "ns_last_error", "ns_clone", "ns_set_abundance", "ns_set_expression", "ns_set_reference", "ns_set_model", "ns_configure",
            "ns_simulate", "ns_fetch", "ns_reemit", "ns_batch_info", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases",
            "ns_compress_records", "ns_fetch_compressed", "ns_compress_error_profile", "ns_fetch_compressed_error_profile", "ns_compress_bam", "ns_apply_variants",
-           "ns_compress_bam_mapped"]
+           "ns_compress_bam_mapped", "ns_set_lift"]
 
 
 class NsReference(C.Structure):
@@ -137,6 +137,8 @@ def lib():
     L.ns_set_reference.restype = C.c_int
     L.ns_apply_variants.argtypes = [P, C.POINTER(NsVariants)]
     L.ns_apply_variants.restype = C.c_int
+    L.ns_set_lift.argtypes = [P, C.POINTER(NsVariants)]
+    L.ns_set_lift.restype = C.c_int
     L.ns_set_model.argtypes = [P, C.POINTER(NsModel)]
     L.ns_set_model.restype = C.c_int
     L.ns_set_abundance.argtypes = [P, P, P, C.c_uint32]

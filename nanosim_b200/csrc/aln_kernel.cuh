@@ -6,7 +6,11 @@
 //   pass 2 (aln_write_kernel): the same walk writes the records' descriptors, CIGAR words and sizes
 // One thread per read: the rules (LIT groups, merging, trimming, the cut at a circular record's origin) are a sequential
 // state machine over the script, and each read's ops are contiguous in HBM.
+// kLift (ns_set_lift, DESIGN §3 "Lifted mapped BAM"): the same walk composes every op with the haplotype record's lift
+// segments on the way, so the records are against the haploid reference the VCF describes.
 #pragma once
+
+#include "haplotype.h"
 
 // CIGAR operations (SAM/BAM specification §4.2.2: MIDNSHP=X -> 0..8)
 enum : uint32_t { CIG_M = 0, CIG_I = 1, CIG_D = 2, CIG_N = 3, CIG_S = 4, CIG_H = 5 };
@@ -37,10 +41,14 @@ __host__ __device__ __forceinline__ uint32_t bam_reg2bin(uint64_t beg, uint64_t 
     return 0;
 }
 
-// bytes of a mapped record: the fixed fields, name, CIGAR (kSmN when it does not fit), bases, qualities, CG:B,I
-__host__ __device__ __forceinline__ uint64_t bam_mapped_size(uint32_t nl, const BamAln& a) {
+// A lifted record keeps its HP value (1 or 2) in BamAln::flag's bits 12-15, above the BAM flag bits
+constexpr uint32_t BAM_FLAG_BITS = 0xfff, BAM_HP_SHIFT = 12;
+
+// bytes of a mapped record: the fixed fields, name, CIGAR (kSmN when it does not fit), bases, qualities, hp (4: a lifted
+// record's HP:C field), CG:B,I
+__host__ __device__ __forceinline__ uint64_t bam_mapped_size(uint32_t nl, const BamAln& a, uint32_t hp = 0) {
     const bool cg = a.n_cig > BAM_MAX_CIGAR;
-    return BAM_FIXED + nl + 1 + 4ull * (cg ? 2 : a.n_cig) + (a.l_seq + 1) / 2 + a.l_seq + (cg ? 8 + 4ull * a.n_cig : 0);
+    return BAM_FIXED + nl + 1 + 4ull * (cg ? 2 : a.n_cig) + (a.l_seq + 1) / 2 + a.l_seq + hp + (cg ? 8 + 4ull * a.n_cig : 0);
 }
 
 // the complement of a 4-bit base code: its bits reversed (A 1 <-> T 8, C 2 <-> G 4, M <-> K, R <-> Y, V <-> B, H <-> D;
@@ -59,12 +67,15 @@ struct BgzfMappedTable {
     const uint32_t* cigar;
     __device__ __forceinline__ BgzfMappedRec operator[](uint32_t r) const {
         const BamAln a = aln[r];
-        return BgzfMappedRec{reads[a.read], a, cigar + a.cig_off, reads.reads[a.read].reversed};
+        return BgzfMappedRec{reads[a.read], a, cigar + a.cig_off, a.flag & 16u};       // the record's strand
     }
 };
 
-struct BgzfMappedLayout {
+// kLift: a mapped record also has the HP:C field of its haplotype (BamAln::flag >> BAM_HP_SHIFT) as its first aux field
+template <bool kLift>
+struct BgzfMappedLayoutOf {
     using Table = BgzfMappedTable;
+    static constexpr uint32_t hp = kLift ? 4 : 0;
     static __device__ __forceinline__ uint8_t byte(uint64_t q, const BgzfMappedRec& rc) {
         const BamAln& a = rc.a;
         if (a.flag & 4) return BgzfBamLayout::byte(q, rc.rd);
@@ -74,11 +85,11 @@ struct BgzfMappedLayout {
         if (q < BAM_FIXED) {
             uint32_t w;
             switch ((uint32_t)q >> 2) {
-            case 0: w = (uint32_t)bam_mapped_size(nl, a) - 4; break;                        // block_size
+            case 0: w = (uint32_t)bam_mapped_size(nl, a, hp) - 4; break;                    // block_size
             case 1: w = a.ref_id; break;
             case 2: w = a.pos; break;
             case 3: w = (nl + 1) | (BAM_MAPQ << 8) | ((uint32_t)a.bin << 16); break;       // l_read_name, mapq, bin
-            case 4: w = nc | ((uint32_t)a.flag << 16); break;                               // n_cigar_op, flag
+            case 4: w = nc | ((uint32_t)(kLift ? a.flag & BAM_FLAG_BITS : a.flag) << 16); break;   // n_cigar_op, flag
             case 5: w = ls; break;                                                          // l_seq
             case 8: w = 0; break;                                                           // tlen
             default: w = 0xffffffffu;                                                       // next_refID, next_pos
@@ -111,12 +122,99 @@ struct BgzfMappedLayout {
             return rc.rd.fastq ? (uint8_t)(rc.rd.ql[rc.rev ? L - 1 - f : f] - 33) : 0xffu;
         }
         q -= ls;
+        if (kLift) {
+            if (q < 3) return (uint8_t)"HPC"[q];
+            if (q == 3) return (uint8_t)(a.flag >> BAM_HP_SHIFT);
+            q -= 4;
+        }
         if (q < 4) return (uint8_t)"CGBI"[q];
         const uint32_t k = (uint32_t)(q - 4) >> 2;             // the count, then the words
         const uint32_t w = k == 0 ? a.n_cig : rc.cig[k - 1];
         return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
     }
 };
+struct BgzfMappedLayout : BgzfMappedLayoutOf<false> {};
+struct BgzfLiftedLayout : BgzfMappedLayoutOf<true> {};
+
+// ns_set_lift's table in HBM: haplotype record h's segments are seg[first[h] .. first[h + 1]) in haplotype order, their
+// kinds kind[...]; hap_chrom[h] its source record and hap_number[h] its HP value
+struct AlnLift {
+    const HapLift* seg;
+    const uint8_t* kind;
+    const uint64_t* first;
+    const uint32_t* hap_chrom;
+    const uint8_t* hap_number;
+};
+
+// Where the lift walk stands: haplotype base t of segment s (s_last: the record's last segment); d_done once the
+// reference-only bases of s are emitted.  Before each M or D it hands to fn: at, the reference coordinate of its first
+// base (inv = false), or one past it in reference order (inv = true: inside an <INV>, the bases run backwards).
+struct LiftWalk {
+    const HapLift* seg;
+    const uint8_t* kind;
+    uint64_t s, s_last;
+    uint32_t t;
+    bool d_done, inv;
+    uint32_t at;
+};
+
+// Past the end of segment s: its reference-only bases (a sequence ALT with ref_len > hap_len: a deletion) as D, then the
+// next segment, with an ALN_CUT where the reference stops advancing forward (into a <DUP> copy, into or out of an <INV>)
+template <class Fn>
+__device__ __forceinline__ void lift_advance(LiftWalk& w, Fn& fn) {
+    for (;;) {
+        const HapLift g = w.seg[w.s];
+        if (w.t < g.hap_len) return;
+        const uint8_t k = w.kind[w.s];
+        if (k == HAP_LIFT_SEQ && g.ref_len > g.hap_len && !w.d_done) {
+            w.d_done = true;
+            w.at = g.ref0 + g.hap_len;
+            w.inv = false;
+            fn(CIG_D, g.ref_len - g.hap_len);
+        }
+        if (w.s == w.s_last) return;
+        ++w.s;
+        w.t = 0;
+        w.d_done = false;
+        if (k == HAP_LIFT_INV || w.kind[w.s] != HAP_LIFT_SEQ) fn(ALN_CUT, 0u);
+    }
+}
+
+// A read op (M, I or D over the haplotype) composed with the lift: I stays I; M and D over 1:1 bases stay M and D; over
+// the inserted bases of a sequence ALT an M becomes I and a D vanishes
+template <class Fn>
+__device__ __forceinline__ void lift_put(LiftWalk& w, uint32_t kind, uint32_t len, Fn& fn) {
+    if (kind == CIG_I) {
+        fn(CIG_I, len);
+        return;
+    }
+    while (len) {
+        const HapLift g = w.seg[w.s];
+        const uint8_t k = w.kind[w.s];
+        uint32_t n = len, out = kind;
+        w.inv = k == HAP_LIFT_INV;
+        if (w.t >= g.hap_len) {                                 // past the record's last base: no segment of a linear record
+            w.at = g.ref0 + g.ref_len;                          // gets here; 1:1 so that the walk ends
+            w.inv = false;
+        } else if (w.inv) {
+            n = min(len, g.hap_len - w.t);
+            w.at = g.ref0 + g.ref_len - w.t;
+        } else {
+            const uint32_t m = k == HAP_LIFT_SEQ ? min(g.hap_len, g.ref_len) : g.hap_len;        // the 1:1 bases
+            if (w.t < m) {
+                n = min(len, m - w.t);
+                w.at = g.ref0 + w.t;
+            } else {
+                n = min(len, g.hap_len - w.t);
+                out = kind == CIG_M ? CIG_I : ~0u;
+            }
+        }
+        if (out != ~0u) fn(out, n);
+        w.t += n;
+        len -= n;
+        lift_advance(w, fn);
+    }
+}
 
 struct AlnArgs {
     const NsReadMeta* reads;
@@ -136,18 +234,25 @@ struct AlnArgs {
     BamAln* aln;                    // pass 2 writes
     uint32_t* cigar;
     uint64_t* rec_size;
+    AlnLift lift;                   // kLift only
 };
 
 // fn(kind, len) over a segment's script: CIGAR kinds M I D (HT as I: it only stands at a read's edges), a LIT group followed
 // by a DEL as |n - r| I or D and then min(n, r) M, zero lengths dropped, and an ALN_CUT (len 0) before the reference base
 // at offset `cut` and every `period` bases behind it (a circular record's origin, each time the segment passes it; ~0:
 // none), an M or D across one split there
-template <class Fn>
-__device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint32_t n_ops, uint64_t cut, uint64_t period, Fn fn) {
+// kLift: every op goes through lift_put on walk w instead (no circular record: cut is ~0)
+template <bool kLift, class Fn>
+__device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint32_t n_ops, uint64_t cut, uint64_t period, LiftWalk& w,
+                                           Fn fn) {
     uint64_t rf = 0;
     uint32_t lit = 0;
     auto put = [&](uint32_t kind, uint32_t len) {
         if (len == 0) return;
+        if constexpr (kLift) {
+            lift_put(w, kind, len, fn);
+            return;
+        }
         if (kind != CIG_I) {
             while (rf <= cut && rf + len > cut) {
                 const uint32_t a = (uint32_t)(cut - rf);
@@ -184,13 +289,16 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
 // each, sink.begin(q0, rf0) at its first M, sink.op(kind, len) for its merged ops, sink.end(q1, rf1) after its last M
 // (read offsets in the forward read, reference offsets in the segment).  Ops before the first M and after the last one
 // are outside the alignment: their I is clip, their D moves the start or is dropped.  Two walks per part: the first finds
-// the part's first and last M, the second emits what lies between them.
-template <class Sink>
+// the part's first and last M, the second emits what lies between them.  kLift: every walk starts from `start`, the first
+// one counts the parts (n_parts = 1 on entry), and sink.place(at, inv) follows sink.begin with the lift's position of the
+// first M.
+template <bool kLift, class Sink>
 __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, uint64_t cut, uint64_t period, uint32_t n_parts,
-                                            uint32_t q_start, Sink& sink) {
+                                            uint32_t q_start, const LiftWalk& start, Sink& sink) {
     for (uint32_t want = 0; want < n_parts; ++want) {
         uint32_t first = ~0u, last = 0, idx = 0, part = 0;
-        aln_script(sc, n_ops, cut, period, [&](uint32_t kind, uint32_t) {
+        LiftWalk w = start;
+        aln_script<kLift>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t) {
             if (kind == ALN_CUT) {
                 ++part;
             } else if (kind == CIG_M && part == want) {
@@ -199,13 +307,16 @@ __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, 
             }
             ++idx;
         });
+        if constexpr (kLift) n_parts = part + 1;
         if (first == ~0u) continue;
         idx = 0;
         uint32_t q = q_start, rf = 0, ck = 0, cl = 0;
-        aln_script(sc, n_ops, cut, period, [&](uint32_t kind, uint32_t len) {
+        w = start;
+        aln_script<kLift>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t len) {
             if (idx >= first && idx <= last) {
                 if (idx == first) {
                     sink.begin(q, rf);
+                    if constexpr (kLift) sink.place(w.at, w.inv);
                     ck = kind;
                     cl = 0;
                 }
@@ -228,8 +339,10 @@ __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, 
     }
 }
 
-// every alignment of read r, in the order of its segments: sink.segment(piece, record length) before each segment's
-template <class Sink>
+// every alignment of read r, in the order of its segments: sink.segment(piece, record length) before each segment's.
+// kLift: the walk of a segment starts in the lift segment holding its first haplotype base, the last of its record's
+// segments that starts at or before it (binary search).
+template <bool kLift, class Sink>
 __device__ __forceinline__ void aln_read(const AlnArgs& a, const NsReadMeta& r, Sink& sink) {
     for (uint32_t k = 0; k < r.n_pieces; ++k) {
         const NsPieceMeta pc = a.pieces[r.piece_first + k];
@@ -238,12 +351,24 @@ __device__ __forceinline__ void aln_read(const AlnArgs& a, const NsReadMeta& r, 
         // a segment that runs past its record's end (circular records only) is cut at the origin, as often as it passes it
         uint64_t cut = ~0ull;
         uint32_t n_parts = 1;
-        if ((uint64_t)pc.pos + pc.ref_len > clen) {
+        LiftWalk w{};
+        if constexpr (kLift) {
+            uint64_t lo = a.lift.first[pc.chrom], hi = a.lift.first[pc.chrom + 1];
+            w.s_last = hi - 1;
+            while (hi - lo > 1) {
+                const uint64_t mid = (lo + hi) >> 1;
+                if (a.lift.seg[mid].hap0 <= pc.pos) lo = mid; else hi = mid;
+            }
+            w.seg = a.lift.seg;
+            w.kind = a.lift.kind;
+            w.s = lo;
+            w.t = pc.pos - a.lift.seg[lo].hap0;
+        } else if ((uint64_t)pc.pos + pc.ref_len > clen) {
             cut = clen > pc.pos ? clen - pc.pos : 0;
             n_parts = 2 + (uint32_t)((pc.ref_len - 1 - cut) / clen);
         }
         sink.segment(pc, clen);
-        aln_segment(a.ops + pc.op_off, pc.n_ops, cut, clen, n_parts, pc.out_rel, sink);
+        aln_segment<kLift>(a.ops + pc.op_off, pc.n_ops, cut, clen, n_parts, pc.out_rel, w, sink);
     }
 }
 
@@ -257,6 +382,7 @@ struct AlnCount {
         rf0 = rf;
         body = 0;
     }
+    __device__ void place(uint32_t, bool) {}
     __device__ void op(uint32_t, uint32_t) { ++body; }
     __device__ void end(uint32_t q1, uint32_t rf1) {
         words += body + (q0 > 0) + (q1 < L);
@@ -268,6 +394,7 @@ struct AlnCount {
     }
 };
 
+template <bool kLift>
 __global__ void aln_count_kernel(AlnArgs a) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n_reads) return;
@@ -279,19 +406,24 @@ __global__ void aln_count_kernel(AlnArgs a) {
     const NsReadMeta r = a.reads[i];
     AlnCount c;
     c.L = r.seq_len;
-    aln_read(a, r, c);
+    aln_read<kLift>(a, r, c);
     a.n_rec[i] = c.n_aln ? c.n_aln : 1;                         // no alignment: the unmapped record
     a.n_cig[i] = c.words;
     a.primary[i] = c.prim;
 }
 
+// kLift: refID is the haplotype's source record and POS the lifted one; a part inside an <INV> is a record on the other
+// strand, its CIGAR words (written in haplotype order) reversed in place and its stored bases mirrored
+template <bool kLift>
 struct AlnWrite {
     uint32_t i, L, nl, prim, rev;
     BamAln* rec;                    // the read's records
     uint32_t* cig;                  // its CIGAR words
     uint64_t* size;
     uint64_t cig_off;
-    uint32_t n_aln = 0, w = 0, w0 = 0, q0 = 0, rf0 = 0, chrom = 0, pos = 0;
+    AlnLift lift;
+    uint32_t n_aln = 0, w = 0, w0 = 0, q0 = 0, rf0 = 0, chrom = 0, pos = 0, at = 0;
+    bool inv = false;
     uint64_t clen = 0;
     __device__ void segment(const NsPieceMeta& pc, uint64_t len) {
         chrom = pc.chrom;
@@ -304,6 +436,10 @@ struct AlnWrite {
         w0 = w;
         if (q > 0) cig[w++] = (q << 4) | (n_aln == prim ? CIG_S : CIG_H);
     }
+    __device__ void place(uint32_t a, bool in) {
+        at = a;
+        inv = in;
+    }
     __device__ void op(uint32_t kind, uint32_t len) { cig[w++] = (len << 4) | kind; }
     __device__ void end(uint32_t q1, uint32_t rf1) {
         const bool primary = n_aln == prim;
@@ -313,25 +449,42 @@ struct AlnWrite {
         b.q0 = primary ? 0 : q0;
         b.l_seq = primary ? L : q1 - q0;
         b.ref_id = chrom;
-        const uint64_t p = ((uint64_t)pos + rf0) % clen;       // a part behind a circular record's origin starts past it
-        b.pos = (uint32_t)p;
         b.span = rf1 - rf0;
         b.n_cig = w - w0;
+        uint64_t p;
+        if constexpr (kLift) {
+            b.ref_id = lift.hap_chrom[chrom];
+            p = inv ? at - b.span : at;
+            if (inv) {
+                if (!primary) b.q0 = L - q1;
+                for (uint32_t x = w0, y = w - 1; x < y; ++x, --y) {
+                    const uint32_t c = cig[x];
+                    cig[x] = cig[y];
+                    cig[y] = c;
+                }
+            }
+        } else {
+            p = ((uint64_t)pos + rf0) % clen;                   // a part behind a circular record's origin starts past it
+        }
+        b.pos = (uint32_t)p;
         b.bin = (uint16_t)bam_reg2bin(p, p + b.span);
-        b.flag = (uint16_t)((rev ? 16u : 0u) | (primary ? 0u : 0x800u));
+        b.flag = (uint16_t)(((rev ^ (uint32_t)inv) ? 16u : 0u) | (primary ? 0u : 0x800u));
+        if constexpr (kLift) b.flag |= (uint16_t)(lift.hap_number[chrom] << BAM_HP_SHIFT);
         b.cig_off = cig_off + w0;
         rec[n_aln] = b;
-        size[n_aln] = bam_mapped_size(nl, b);
+        size[n_aln] = bam_mapped_size(nl, b, kLift ? 4 : 0);
         ++n_aln;
     }
 };
 
+template <bool kLift>
 __global__ void aln_write_kernel(AlnArgs a) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n_reads) return;
     const NsReadMeta r = a.reads[i];
     const uint64_t r0 = a.rec_first[i];
-    AlnWrite s;
+    AlnWrite<kLift> s;
+    s.lift = a.lift;
     s.i = i;
     s.L = r.seq_len;
     s.nl = a.name_len[i];
@@ -341,7 +494,7 @@ __global__ void aln_write_kernel(AlnArgs a) {
     s.cig_off = a.cig_first[i];
     s.cig = a.cigar + s.cig_off;
     s.size = a.rec_size + r0;
-    aln_read(a, r, s);
+    aln_read<kLift>(a, r, s);
     if (s.n_aln == 0) {                                         // the unmapped record of ns_compress_bam
         BamAln b{};
         b.read = i;

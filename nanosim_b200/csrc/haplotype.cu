@@ -21,3 +21,8 @@ cudaError_t hap_gather(const uint8_t* ref, const uint8_t* alt, const uint64_t* s
     else hap_gather_kernel<false><<<blocks, 256, 0, st>>>(ref, alt, seg_src, seg_out, n_seg, out);
     return cudaGetLastError();
 }
+
+cudaError_t hap_lift(const HapArgs& a, const uint64_t* seg_out, const uint64_t* hap_off, HapLift* lift, uint8_t* kind, cudaStream_t st) {
+    hap_lift_kernel<<<(unsigned)((a.n_seg + 255) / 256), 256, 0, st>>>(a, seg_out, hap_off, lift, kind);
+    return cudaGetLastError();
+}

@@ -23,6 +23,15 @@ struct HapArgs {
     uint64_t* seg_len;                  // n_seg + 1 (the last one 0: the scan's total lands behind the segments)
 };
 
+// One segment of a haplotype record as ns_set_lift keeps it: haplotype bases [hap0, hap0 + hap_len) of the record and
+// the reference span [ref0, ref0 + ref_len) of its source record, with the segment's kind (HapLiftKind) beside it
+struct HapLift {
+    uint32_t hap0, hap_len, ref0, ref_len;
+};
+// the kind of a segment: a stretch between variants or a sequence ALT (min(hap_len, ref_len) bases 1:1, then the rest
+// inserted or deleted), a <DUP> copy (1:1 onto [ref0, ref0 + ref_len) again), an <INV> (1:1, reversed); = alt_kind
+enum : uint8_t { HAP_LIFT_SEQ = 0, HAP_LIFT_DUP = 1, HAP_LIFT_INV = 2 };
+
 // Segments, their output offsets seg_out[0 .. n_seg] (seg_out[n_seg] = the haplotypes' bytes) and the haplotype records'
 // offsets hap_off[0 .. n_hap], on `st`.  With tmp == nullptr only *tmp_bytes is set (the scan's scratch space).
 cudaError_t hap_layout(const HapArgs& a, uint64_t* seg_out, uint64_t* hap_off, void* tmp, size_t* tmp_bytes, cudaStream_t st);
@@ -30,3 +39,5 @@ cudaError_t hap_layout(const HapArgs& a, uint64_t* seg_out, uint64_t* hap_off, v
 // is HAP_SRC_RC (an ALT of kind 2).
 cudaError_t hap_gather(const uint8_t* ref, const uint8_t* alt, const uint64_t* seg_src, const uint64_t* seg_out, uint64_t n_seg,
                        uint64_t n_bases, bool reverse_complement, uint8_t* out, cudaStream_t st);
+// Every segment's HapLift and kind (n_seg of each) from the arrays hap_layout left, on `st`.
+cudaError_t hap_lift(const HapArgs& a, const uint64_t* seg_out, const uint64_t* hap_off, HapLift* lift, uint8_t* kind, cudaStream_t st);

@@ -7,6 +7,7 @@
 //   (CUB exclusive sum over the lengths: every segment's offset in the output, and the total)
 //   hap_offsets_kernel:  the haplotype records' offsets (chrom_off of the new reference)
 //   hap_gather_kernel:   one thread per 16-byte unit of the output; see there
+//   hap_lift_kernel:     (ns_set_lift, after hap_segments_kernel and the scan) one thread per segment, its HapLift
 // Included only by haplotype.cu, which launches them: a translation unit of their own, so the host code that drives them
 // leaves the code generated for nanosim_api.cu's kernels as it is.
 #pragma once
@@ -15,6 +16,16 @@
 
 __device__ __forceinline__ uint64_t hap_seg_first(const uint64_t* var_off, uint32_t h) { return 2 * var_off[h] + h; }
 
+// the haplotype of segment s: the last h with seg_first(h) <= s
+__device__ __forceinline__ uint32_t hap_of_segment(const HapArgs& a, uint64_t s) {
+    uint32_t lo = 0, hi = a.n_hap;
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (hap_seg_first(a.var_off, mid) <= s) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 __global__ void hap_segments_kernel(HapArgs a) {
     const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (s > a.n_seg) return;
@@ -22,11 +33,7 @@ __global__ void hap_segments_kernel(HapArgs a) {
         a.seg_len[s] = 0;
         return;
     }
-    uint32_t lo = 0, hi = a.n_hap;      // haplotype of this segment: last h with seg_first(h) <= s
-    while (hi - lo > 1) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (hap_seg_first(a.var_off, mid) <= s) lo = mid; else hi = mid;
-    }
+    const uint32_t lo = hap_of_segment(a, s);
     const uint64_t local = s - hap_seg_first(a.var_off, lo);
     const uint64_t j = a.var_off[lo] + local / 2;
     const uint32_t c = a.hap_chrom[lo];
@@ -41,6 +48,32 @@ __global__ void hap_segments_kernel(HapArgs a) {
     const uint64_t end = j < a.var_off[lo + 1] ? a.var_pos[j] : a.chrom_off[c + 1] - a.chrom_off[c];
     a.seg_src[s] = a.chrom_off[c] + begin;
     a.seg_len[s] = end - begin;
+}
+
+// ns_set_lift: segment s as a HapLift (offsets in its haplotype record and in the source record) and its kind.  A stretch
+// maps onto its own source span; an ALT onto [var_pos, var_pos + var_ref_len), except a <DUP> copy (kind 1), whose
+// reference span is the source span [alt_off, alt_off + alt_len) it repeats.  (An <INV> has var_pos = alt_off.)
+__global__ void hap_lift_kernel(HapArgs a, const uint64_t* __restrict__ seg_out, const uint64_t* __restrict__ hap_off,
+                                HapLift* __restrict__ lift, uint8_t* __restrict__ kind) {
+    const uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= a.n_seg) return;
+    const uint32_t h = hap_of_segment(a, s);
+    const uint64_t local = s - hap_seg_first(a.var_off, h);
+    const uint64_t j = a.var_off[h] + local / 2;
+    HapLift g;
+    g.hap0 = (uint32_t)(seg_out[s] - hap_off[h]);
+    g.hap_len = (uint32_t)a.seg_len[s];
+    uint8_t k = HAP_LIFT_SEQ;
+    if (local & 1) {
+        k = a.alt_kind ? a.alt_kind[j] : 0;
+        g.ref0 = (uint32_t)(k == HAP_LIFT_DUP ? a.alt_off[j] : a.var_pos[j]);
+        g.ref_len = k == HAP_LIFT_DUP ? a.alt_len[j] : a.var_ref_len[j];
+    } else {
+        g.ref0 = (uint32_t)(a.seg_src[s] - a.chrom_off[a.hap_chrom[h]]);
+        g.ref_len = g.hap_len;
+    }
+    lift[s] = g;
+    kind[s] = k;
 }
 
 // hap_off[h] = output offset of haplotype h's first segment; hap_off[n_hap] = the total

@@ -123,6 +123,11 @@ struct Tables {
     DevRef dref{};                  // without the transcript-length table: that one is per context (NsContext::trx)
     DevModel dmodel{};
     NsModel hmodel{};
+    // ns_apply_variants: the record offsets of the haploid reference the haplotypes were built from (empty before)
+    std::vector<uint64_t> h_haploid_off;
+    // ns_set_lift: the lift table of the resident haplotype records (aln_kernel.cuh's AlnLift)
+    DevBuf lift_seg, lift_kind, lift_first, lift_chrom, lift_hp;
+    bool have_lift = false;
 };
 
 // transcript lengths ascending + their record indices (ns_configure, transcriptome mode); a clone that configures another
@@ -803,69 +808,96 @@ int ns_set_reference(NsContext* ctx, const NsReference* ref) {
         tab.dref.species_chrom_off = tab.ref_sp_off.as<uint32_t>();
     }
     tab.have_ref = true;
+    tab.h_haploid_off.clear();
+    tab.have_lift = false;
+    for (DevBuf* b : {&tab.lift_seg, &tab.lift_kind, &tab.lift_first, &tab.lift_chrom, &tab.lift_hp}) b->release();
     ctx->have_batch = false;
     ctx->opt_ok[0] = ctx->opt_ok[1] = false;
     return NS_OK;
 }
 
-int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
-    if (!ctx || !v || !v->hap_chrom || !v->var_off || v->n_hap == 0 ||
-        (v->n_var && (!v->var_pos || !v->var_ref_len || !v->alt_off || !v->alt_len)) || (v->alt_bytes && !v->alt))
-        return fail(ctx, NS_EINVAL, "ns_apply_variants: null argument or no haplotype");
-    if (ctx->clone) return fail(ctx, NS_ESTATE, "ns_apply_variants: a cloned context shares its parent's reference");
-    Tables& tab = *ctx->tables;
-    if (!tab.have_ref) return fail(ctx, NS_ESTATE, "ns_apply_variants: set the reference first (ns_set_reference or ns_bcast_nccl)");
-    if (tab.dref.n_species) return fail(ctx, NS_EINVAL, "ns_apply_variants: a metagenome reference cannot carry variants");
-    const uint32_t n_chrom = tab.dref.n_chrom;
-    const std::vector<uint64_t>& off = tab.h_chrom_off;
-    bool any_rc = false;                                            // an inversion: the gather's reverse-complement path
+// The checks ns_apply_variants and ns_set_lift make on the tables, against the haploid records' offsets `off`: *any_rc
+// tells whether some variant is an inversion
+static bool variants_given(const NsVariants* v) {
+    return v && v->hap_chrom && v->var_off && v->n_hap != 0 && (!v->n_var || (v->var_pos && v->var_ref_len && v->alt_off && v->alt_len)) &&
+           (!v->alt_bytes || v->alt);
+}
+static int check_variants(NsContext* ctx, const char* fname, const NsVariants* v, const std::vector<uint64_t>& off, bool* any_rc) {
+    const uint32_t n_chrom = (uint32_t)(off.size() - 1);
+    *any_rc = false;
     if (v->var_off[0] != 0 || v->var_off[v->n_hap] != v->n_var)
-        return fail(ctx, NS_EINVAL, "ns_apply_variants: var_off must start at 0 and end at n_var");
+        return fail(ctx, NS_EINVAL, "%s: var_off must start at 0 and end at n_var", fname);
     for (uint32_t h = 0; h < v->n_hap; ++h) {
         const uint32_t c = v->hap_chrom[h];
-        if (c >= n_chrom) return fail(ctx, NS_EINVAL, "ns_apply_variants: haplotype %u names record %u of %u", h, c, n_chrom);
-        if (v->var_off[h + 1] < v->var_off[h]) return fail(ctx, NS_EINVAL, "ns_apply_variants: var_off decreases at haplotype %u", h);
+        if (c >= n_chrom) return fail(ctx, NS_EINVAL, "%s: haplotype %u names record %u of %u", fname, h, c, n_chrom);
+        if (v->var_off[h + 1] < v->var_off[h]) return fail(ctx, NS_EINVAL, "%s: var_off decreases at haplotype %u", fname, h);
         uint64_t end = 0;
         for (uint64_t j = v->var_off[h]; j < v->var_off[h + 1]; ++j) {
             const uint8_t kind = v->alt_kind ? v->alt_kind[j] : 0;
             if (kind > 2)
-                return fail(ctx, NS_EINVAL, "ns_apply_variants: variant %llu of haplotype %u has ALT kind %u (0, 1 or 2)", (unsigned long long)j,
-                            h, (unsigned)kind);
+                return fail(ctx, NS_EINVAL, "%s: variant %llu of haplotype %u has ALT kind %u (0, 1 or 2)", fname, (unsigned long long)j, h,
+                            (unsigned)kind);
             if (v->var_pos[j] < end || v->var_pos[j] + v->var_ref_len[j] > off[c + 1] - off[c])
-                return fail(ctx, NS_EINVAL, "ns_apply_variants: variant %llu of haplotype %u overlaps the one before it or lies outside "
-                            "its record", (unsigned long long)j, h);
+                return fail(ctx, NS_EINVAL, "%s: variant %llu of haplotype %u overlaps the one before it or lies outside its record", fname,
+                            (unsigned long long)j, h);
             const uint64_t src_bytes = kind ? off[c + 1] - off[c] : v->alt_bytes;      // kinds 1 and 2 read the source record
             if (v->alt_off[j] > src_bytes || v->alt_len[j] > src_bytes - v->alt_off[j])
-                return fail(ctx, NS_EINVAL, "ns_apply_variants: the ALT of variant %llu of haplotype %u lies outside %s", (unsigned long long)j, h,
+                return fail(ctx, NS_EINVAL, "%s: the ALT of variant %llu of haplotype %u lies outside %s", fname, (unsigned long long)j, h,
                             kind ? "its source record" : "the ALT bytes");
             end = v->var_pos[j] + v->var_ref_len[j];
-            any_rc |= kind == 2;
+            *any_rc |= kind == 2;
         }
     }
+    return NS_OK;
+}
+
+// The tables' uploads and hap_layout's segments (sources, lengths, output offsets) and record offsets, on the context's
+// stream; the haploid records' offsets on the device are chrom_off.  ns_apply_variants and ns_set_lift share them.
+struct VariantLayout {
+    DevBuf hap_chrom, var_off, var_pos, var_ref_len, alt_off, alt_len, alt_kind, seg_src, seg_len, seg_out, hap_off;
+    HapArgs args{};
+    size_t bytes() const {
+        return hap_chrom.cap + var_off.cap + var_pos.cap + var_ref_len.cap + alt_off.cap + alt_len.cap + alt_kind.cap + seg_src.cap +
+               seg_len.cap + seg_out.cap + hap_off.cap;
+    }
+};
+static cudaError_t variant_layout(NsContext* ctx, const NsVariants* v, const uint64_t* chrom_off, VariantLayout& L) {
+    cudaStream_t st = ctx->stream;
+    const uint64_t n_seg = 2 * v->n_var + v->n_hap;
+    cudaError_t e = cudaSuccess;
+    auto ok = [&](cudaError_t x) { return (e = x) == cudaSuccess; };
+    if (!ok(upload(L.hap_chrom, v->hap_chrom, (size_t)v->n_hap * 4, st)) || !ok(upload(L.var_off, v->var_off, (size_t)(v->n_hap + 1) * 8, st)) ||
+        !ok(upload(L.var_pos, v->var_pos, v->n_var * 8, st)) || !ok(upload(L.var_ref_len, v->var_ref_len, v->n_var * 4, st)) ||
+        !ok(upload(L.alt_off, v->alt_off, v->n_var * 8, st)) || !ok(upload(L.alt_len, v->alt_len, v->n_var * 4, st)) ||
+        (v->alt_kind && !ok(upload(L.alt_kind, v->alt_kind, v->n_var, st))) || !ok(L.seg_src.ensure(n_seg * 8)) ||
+        !ok(L.seg_len.ensure((n_seg + 1) * 8)) || !ok(L.seg_out.ensure((n_seg + 1) * 8)) || !ok(L.hap_off.ensure((size_t)(v->n_hap + 1) * 8)))
+        return e;
+    L.args = HapArgs{L.hap_chrom.as<uint32_t>(), L.var_off.as<uint64_t>(), L.var_pos.as<uint64_t>(), L.var_ref_len.as<uint32_t>(),
+                     L.alt_off.as<uint64_t>(), L.alt_len.as<uint32_t>(), v->alt_kind ? L.alt_kind.as<uint8_t>() : nullptr, chrom_off, v->n_hap,
+                     n_seg, L.seg_src.as<uint64_t>(), L.seg_len.as<uint64_t>()};
+    size_t tmp = 0;
+    if (!ok(hap_layout(L.args, L.seg_out.as<uint64_t>(), L.hap_off.as<uint64_t>(), nullptr, &tmp, st)) || !ok(ctx->scan_tmp.ensure(tmp)))
+        return e;
+    return hap_layout(L.args, L.seg_out.as<uint64_t>(), L.hap_off.as<uint64_t>(), ctx->scan_tmp.p, &tmp, st);
+}
+
+int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
+    if (!ctx || !variants_given(v)) return fail(ctx, NS_EINVAL, "ns_apply_variants: null argument or no haplotype");
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "ns_apply_variants: a cloned context shares its parent's reference");
+    Tables& tab = *ctx->tables;
+    if (!tab.have_ref) return fail(ctx, NS_ESTATE, "ns_apply_variants: set the reference first (ns_set_reference or ns_bcast_nccl)");
+    if (tab.dref.n_species) return fail(ctx, NS_EINVAL, "ns_apply_variants: a metagenome reference cannot carry variants");
+    bool any_rc = false;                                            // an inversion: the gather's reverse-complement path
+    if (int rc = check_variants(ctx, "ns_apply_variants", v, tab.h_chrom_off, &any_rc)) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     const uint64_t n_seg = 2 * v->n_var + v->n_hap;
-    DevBuf hap_chrom, var_off, var_pos, var_ref_len, alt_off, alt_len, alt_kind, alt, seg_src, seg_len, seg_out, hap_off, out;
-    CK(upload(hap_chrom, v->hap_chrom, (size_t)v->n_hap * 4, st));
-    CK(upload(var_off, v->var_off, (size_t)(v->n_hap + 1) * 8, st));
-    CK(upload(var_pos, v->var_pos, v->n_var * 8, st));
-    CK(upload(var_ref_len, v->var_ref_len, v->n_var * 4, st));
-    CK(upload(alt_off, v->alt_off, v->n_var * 8, st));
-    CK(upload(alt_len, v->alt_len, v->n_var * 4, st));
-    if (v->alt_kind) CK(upload(alt_kind, v->alt_kind, v->n_var, st));
+    DevBuf alt, out;
+    VariantLayout lay;
+    CK(variant_layout(ctx, v, tab.dref.chrom_off, lay));
     CK(alt.ensure(v->alt_bytes + 16));                              // hap_gather_kernel reads whole words behind the end
     if (v->alt_bytes) CK(cudaMemcpyAsync(alt.p, v->alt, v->alt_bytes, cudaMemcpyHostToDevice, st));
-    CK(seg_src.ensure(n_seg * 8));
-    CK(seg_len.ensure((n_seg + 1) * 8));
-    CK(seg_out.ensure((n_seg + 1) * 8));
-    CK(hap_off.ensure((size_t)(v->n_hap + 1) * 8));
-    HapArgs a{hap_chrom.as<uint32_t>(), var_off.as<uint64_t>(), var_pos.as<uint64_t>(), var_ref_len.as<uint32_t>(),
-              alt_off.as<uint64_t>(), alt_len.as<uint32_t>(), v->alt_kind ? alt_kind.as<uint8_t>() : nullptr, tab.dref.chrom_off, v->n_hap,
-              n_seg, seg_src.as<uint64_t>(), seg_len.as<uint64_t>()};
-    size_t tmp = 0;
-    CK(hap_layout(a, seg_out.as<uint64_t>(), hap_off.as<uint64_t>(), nullptr, &tmp, st));
-    CK(ctx->scan_tmp.ensure(tmp));
-    CK(hap_layout(a, seg_out.as<uint64_t>(), hap_off.as<uint64_t>(), ctx->scan_tmp.p, &tmp, st));
+    const DevBuf &seg_src = lay.seg_src, &seg_out = lay.seg_out, &hap_off = lay.hap_off;
     uint64_t n_bases = 0;
     CK(cudaMemcpyAsync(&n_bases, seg_out.as<uint64_t>() + n_seg, 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -877,13 +909,13 @@ int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
     // accounted peak (sizes of the library's allocations, not a device reading) at the two high points: the haploid
     // reference beside the haplotypes, then the new resident copy (ns_set_reference's) beside them; the build's tables
     // and the scan's scratch space are held throughout
-    const size_t build = hap_chrom.cap + var_off.cap + var_pos.cap + var_ref_len.cap + alt_off.cap + alt_len.cap + alt_kind.cap + alt.cap +
-                         seg_src.cap + seg_len.cap + seg_out.cap + hap_off.cap + out.cap + ctx->scan_tmp.cap;
+    const size_t build = lay.bytes() + alt.cap + out.cap + ctx->scan_tmp.cap;
     const size_t peak_a = build + tab.ref_bases.cap + tab.ref_off.cap + tab.ref_packed.cap + tab.ref_pk_off.cap + tab.ref_exc.cap;
     // the haploid bytes and their 2-bit copy go before ns_set_reference allocates the haplotypes' own
     tab.have_ref = false;
     tab.ref_bases.release();
     tab.ref_packed.release();
+    std::vector<uint64_t> haploid_off = tab.h_chrom_off;
     NsReference r{};
     r.bases = out.as<uint8_t>();                    // device pointers: ns_set_reference copies from them
     r.n_bases = n_bases;
@@ -891,8 +923,56 @@ int ns_apply_variants(NsContext* ctx, const NsVariants* v) {
     r.n_chrom = v->n_hap;
     const int rc = ns_set_reference(ctx, &r);
     if (rc != NS_OK) return rc;
+    tab.h_haploid_off = std::move(haploid_off);
     const size_t peak_b = build + tab.ref_bases.cap + tab.ref_off.cap + tab.ref_packed.cap + tab.ref_pk_off.cap + tab.ref_exc.cap;
     if (v->peak_bytes) *v->peak_bytes = std::max(peak_a, peak_b);
+    return NS_OK;
+}
+
+int ns_set_lift(NsContext* ctx, const NsVariants* v) {
+    static const char* fname = "ns_set_lift";
+    if (!ctx || !variants_given(v)) return fail(ctx, NS_EINVAL, "%s: null argument or no haplotype", fname);
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "%s: a cloned context shares its parent's tables", fname);
+    Tables& tab = *ctx->tables;
+    if (!tab.have_ref || tab.h_haploid_off.empty())
+        return fail(ctx, NS_ESTATE, "%s: the resident reference is not the haplotypes of ns_apply_variants", fname);
+    bool any_rc = false;
+    if (int rc = check_variants(ctx, fname, v, tab.h_haploid_off, &any_rc)) return rc;
+    const std::vector<uint64_t>& off = tab.h_haploid_off;
+    if (v->n_hap != tab.dref.n_chrom)
+        return fail(ctx, NS_EINVAL, "%s: %u haplotypes for %u resident haplotype records", fname, v->n_hap, tab.dref.n_chrom);
+    std::vector<uint64_t> first(v->n_hap + 1);                      // hap_seg_first: each record's first segment
+    std::vector<uint8_t> hp(v->n_hap);                              // the haplotype's place among those of its source record
+    for (uint32_t h = 0; h < v->n_hap; ++h) {
+        const uint32_t c = v->hap_chrom[h];
+        int64_t len = (int64_t)(off[c + 1] - off[c]);
+        for (uint64_t j = v->var_off[h]; j < v->var_off[h + 1]; ++j) len += (int64_t)v->alt_len[j] - (int64_t)v->var_ref_len[j];
+        const uint64_t resident = tab.h_chrom_off[h + 1] - tab.h_chrom_off[h];
+        if ((uint64_t)len != resident)
+            return fail(ctx, NS_EINVAL, "%s: haplotype %u has %lld bases by these tables, the resident record %u has %llu", fname, h,
+                        (long long)len, h, (unsigned long long)resident);
+        first[h] = 2 * v->var_off[h] + h;
+        hp[h] = (uint8_t)(h > 0 && v->hap_chrom[h - 1] == c ? hp[h - 1] + 1 : 1);
+    }
+    first[v->n_hap] = 2 * v->n_var + v->n_hap;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    tab.have_lift = false;
+    DevBuf haploid;
+    VariantLayout lay;
+    CK(upload(haploid, off.data(), off.size() * 8, st));
+    CK(variant_layout(ctx, v, haploid.as<uint64_t>(), lay));
+    const uint64_t n_seg = lay.args.n_seg;
+    CK(tab.lift_seg.ensure(n_seg * sizeof(HapLift)));
+    CK(tab.lift_kind.ensure(n_seg));
+    CK(hap_lift(lay.args, lay.seg_out.as<uint64_t>(), lay.hap_off.as<uint64_t>(), tab.lift_seg.as<HapLift>(), tab.lift_kind.as<uint8_t>(), st));
+    CK(upload(tab.lift_first, first.data(), first.size() * 8, st));
+    CK(upload(tab.lift_chrom, v->hap_chrom, (size_t)v->n_hap * 4, st));
+    CK(upload(tab.lift_hp, hp.data(), hp.size(), st));
+    CK(cudaStreamSynchronize(st));
+    tab.have_lift = true;
+    if (v->peak_bytes)
+        *v->peak_bytes = tab.lift_seg.cap + tab.lift_kind.cap + tab.lift_first.cap + tab.lift_chrom.cap + tab.lift_hp.cap;
     return NS_OK;
 }
 
@@ -1757,6 +1837,9 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     if (ctx->last_kind != NS_KIND_ALIGNED) return fail(ctx, NS_EINVAL, "%s: the last batch is unaligned reads, which have no alignment", fname);
     if (ctx->hcfg.mode == 2)
         return fail(ctx, NS_EINVAL, "%s: transcriptome reads are not written as mapped records", fname);
+    const Tables& tab = *ctx->tables;
+    const bool lift = tab.have_lift;
+    if (lift && ctx->hcfg.circular) return fail(ctx, NS_EINVAL, "%s: lifted records need linear haplotype records", fname);
     CK(cudaSetDevice(ctx->device));
     const uint32_t n = ctx->last.n_reads;
     ctx->have_z = false;
@@ -1784,8 +1867,11 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     aa.n_cig = aa.n_rec + n;
     aa.primary = ctx->m_prim.as<uint32_t>();
     aa.long_names = (unsigned long long*)(totals + NS_T_Z_LONG_NAMES);
+    if (lift)
+        aa.lift = AlnLift{tab.lift_seg.as<HapLift>(), tab.lift_kind.as<uint8_t>(), tab.lift_first.as<uint64_t>(), tab.lift_chrom.as<uint32_t>(),
+                          tab.lift_hp.as<uint8_t>()};
     const unsigned grid = (n + 255) / 256;
-    CK(launch(ctx, aln_count_kernel, grid, 256, 0, aa));
+    CK(launch(ctx, lift ? aln_count_kernel<true> : aln_count_kernel<false>, grid, 256, 0, aa));
     // the record and CIGAR-word totals borrow the text and member-bytes slots, which the later scans overwrite
     uint64_t* rec_first = ctx->m_first.as<uint64_t>();
     if (int rc = scan_total(ctx, aa.n_rec, rec_first, n, NS_T_Z_TEXT)) return rc;
@@ -1809,7 +1895,7 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     aa.aln = ctx->m_aln.as<BamAln>();
     aa.cigar = ctx->m_cig.as<uint32_t>();
     aa.rec_size = ctx->scan_in.as<uint64_t>();
-    CK(launch(ctx, aln_write_kernel, grid, 256, 0, aa));
+    CK(launch(ctx, lift ? aln_write_kernel<true> : aln_write_kernel<false>, grid, 256, 0, aa));
     if (int rc = scan_total(ctx, aa.rec_size, ctx->z_rec_off.as<uint64_t>(), (uint32_t)n_rec, NS_T_Z_TEXT)) return rc;
     if (int rc = publish_totals_and_wait(ctx)) return rc;
     BgzfMembers zm;
@@ -1821,7 +1907,15 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     src.tab.cigar = aa.cigar;
     src.rec_off = ctx->z_rec_off.as<uint64_t>();
     src.n_recs = (uint32_t)n_rec;
-    if (int rc = deflate_members(ctx, src, zm, n_blocks)) return rc;
+    if (lift) {
+        BgzfRecords<BgzfLiftedLayout> lifted;
+        lifted.tab = src.tab;
+        lifted.rec_off = src.rec_off;
+        lifted.n_recs = src.n_recs;
+        if (int rc = deflate_members(ctx, lifted, zm, n_blocks)) return rc;
+    } else if (int rc = deflate_members(ctx, src, zm, n_blocks)) {
+        return rc;
+    }
     uint64_t total = 0;
     if (int rc = pack_members(ctx, fname, n_blocks, ctx->z_out, &total)) return rc;
     ctx->z_bytes = total;

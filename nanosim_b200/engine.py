@@ -15,6 +15,12 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+def _variants(t, out):
+    """NsVariants over the arrays of a variants.HaplotypeTables; out (c_uint64) receives peak_bytes."""
+    return L.NsVariants(len(t.hap_chrom), _ptr(t.hap_chrom), _ptr(t.var_off), len(t.var_pos), _ptr(t.var_pos), _ptr(t.var_ref_len),
+                        _ptr(t.alt_off), _ptr(t.alt_len), _ptr(t.alt), len(t.alt), C.pointer(out), _ptr(t.alt_kind))
+
+
 class Batch:
     """Host copy of one simulated batch."""
 
@@ -93,12 +99,17 @@ class Engine:
         """genome --vcf: replaces the resident reference with the haplotype records of ``tables`` (a
         variants.HaplotypeTables over it), built in HBM (ns_apply_variants).  Returns the device memory the reference and
         the build held at the build's peak, in bytes."""
-        t = tables
         peak = C.c_uint64()
-        v = L.NsVariants(len(t.hap_chrom), _ptr(t.hap_chrom), _ptr(t.var_off), len(t.var_pos), _ptr(t.var_pos), _ptr(t.var_ref_len),
-                         _ptr(t.alt_off), _ptr(t.alt_len), _ptr(t.alt), len(t.alt), C.pointer(peak), _ptr(t.alt_kind))
-        self._check(self._lib.ns_apply_variants(self._ctx, C.byref(v)))
+        self._check(self._lib.ns_apply_variants(self._ctx, C.byref(_variants(tables, peak))))
         return int(peak.value)
+
+    def set_lift(self, tables):
+        """genome --vcf --lift_mapped_bam: after apply_variants(tables), keeps the lift of the haplotype records onto the
+        haploid reference (ns_set_lift), so that compress_bam_mapped() writes the reads' alignments to the haploid
+        records.  Call before clone().  Returns the device bytes the lift keeps."""
+        n = C.c_uint64()
+        self._check(self._lib.ns_set_lift(self._ctx, C.byref(_variants(tables, n))))
+        return int(n.value)
 
     def set_abundance(self, abun, inflated=None):
         """dict_abun / dict_abun_inflated of one sample, per species in genome-list order (metagenome mode)."""
@@ -286,8 +297,8 @@ class Engine:
     def compress_bam_mapped(self, names):
         """The last aligned batch as mapped BAM records, the true alignment of every read (``names`` as for compress_bam),
         as BGZF members built on the device and kept there (ns_compress_bam_mapped); they replace those of the last
-        compress_records() / compress_bam().  Returns their size in bytes; neither the BAM header nor the end-of-file
-        block."""
+        compress_records() / compress_bam().  After set_lift() the records are lifted onto the haploid reference.  Returns
+        their size in bytes; neither the BAM header nor the end-of-file block."""
         from .records import _name_blob
         blob, offs = _name_blob(names)
         offs = np.ascontiguousarray(offs, dtype=np.uint64)

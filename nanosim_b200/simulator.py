@@ -98,6 +98,7 @@ class Profile:
         self.max_chrom = 0
         self.perfect = False
         self.haplotypes = None      # genome --vcf: variants.HaplotypeTables
+        self.haploid = None         # genome --vcf: names and offsets of the haploid reference records
 
 
 def _dist_world():
@@ -123,27 +124,33 @@ class _RemoteReference(PackedReference):
 
 def read_profile(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                  polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                 device=0, seed=0, ir_files=None, ref_on_host=True, vcf=None):
+                 device=0, seed=0, ir_files=None, ref_on_host=True, vcf=None, lift=False):
     """read_profile (:244-591).  Under torchrun (WORLD_SIZE > 1) only rank 0 reads the reference files; the other ranks get
     names and offsets through torch.distributed and the bases through ONE NCCL broadcast into their HBM (ns_bcast_nccl).
     ref_on_host: those ranks also copy the bases back to the host, which only the plain error profile's formatter reads.
     vcf (genome mode): the reads come from the haplotypes of the VCF's first sample.  Rank 0 parses it and hands the
     tables to the other ranks; every rank builds the haplotypes in its HBM from the haploid reference (ns_apply_variants),
-    and with ref_on_host copies them back to the host."""
+    and with ref_on_host copies them back to the host.  lift (``--lift_mapped_bam``): every rank also keeps the lift of the
+    haplotypes onto the haploid records (ns_set_lift), so that mapped BAM records are against those."""
     rank, world = _dist_world()
     if world > 1:
         return _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun,
-                                         polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host, vcf)
+                                         polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host, vcf,
+                                         lift)
     prof = _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
                                chimeric, homopolymer, fastq, device, seed, ir_files, vcf)
     if prof.haplotypes is not None:
-        _apply_variants(prof, prof.haplotypes, ref_on_host)
+        _apply_variants(prof, prof.haplotypes, ref_on_host, lift)
     return prof
 
 
-def _apply_variants(prof, tables, ref_on_host):
-    """Makes the haplotype records of ``tables`` the resident reference of prof.engine (built on the device)."""
+def _apply_variants(prof, tables, ref_on_host, lift=False):
+    """Makes the haplotype records of ``tables`` the resident reference of prof.engine (built on the device); the haploid
+    records' names and offsets stay in prof.haploid.  lift: ns_set_lift with the same tables."""
+    prof.haploid = _RemoteReference(prof.ref.names, prof.ref.offsets, prof.ref.raw_names)
     prof.engine.apply_variants(tables)
+    if lift:
+        prof.engine.set_lift(tables)
     prof.ref = _RemoteReference(tables.names, tables.offsets, tables.names)
     if ref_on_host:
         prof.ref.bases = prof.engine.reference_bases(prof.ref.genome_len)
@@ -156,7 +163,7 @@ def _apply_variants(prof, tables, ref_on_host):
 
 
 def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp,
-                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True, vcf=None):
+                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True, vcf=None, lift=False):
     dist = _dist_init()
     box = [None]
     if rank == 0:
@@ -201,7 +208,7 @@ def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per
         prof.engine = Engine(device=device, seed=seed)
     prof.engine.bcast_reference(info["nccl_id"], rank, world, 0)          # the one NCCL broadcast of the job
     if info["haplotypes"] is not None:
-        _apply_variants(prof, info["haplotypes"], ref_on_host)
+        _apply_variants(prof, info["haplotypes"], ref_on_host, lift)
     if rank != 0:
         if ref_on_host and info["haplotypes"] is None:
             prof.ref.bases = prof.engine.reference_bases(int(prof.ref.offsets[-1]))   # host copy for the error profile's reference column
@@ -501,6 +508,10 @@ MAPPED_BAM_HELP = ('With --bam: write <out>_aligned_reads.bam as mapped records,
 VCF_HELP = ('Simulate the reads from the haplotypes of the first sample of this VCF (plain or .vcf.gz), built on the GPU from '
             'the reference: records <chrom>-hap1 and <chrom>-hap2 (one copy for a haploid GT). Only FILTER PASS or . records '
             'are applied. -x still counts the haploid reference, so -x 30 is about 15x per haplotype')
+LIFT_HELP = ('With --vcf and --mapped_bam: write the true alignments in <out>_aligned_reads.bam against the -rg records (as '
+             'an aligner or a VCF names them) instead of the haplotype records: variants become CIGAR operations, <INV> and '
+             '<DUP> split alignments, and every record has HP:C:1 or HP:C:2 for its haplotype. Read names and the error '
+             'profile stay in haplotype coordinates (Default = False)')
 
 
 def _plain_error_profile(args):
@@ -556,6 +567,7 @@ def build_parser():
     g.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     g.add_argument('--mapped_bam', help=MAPPED_BAM_HELP, action='store_true', default=False)
     g.add_argument('--vcf', help=VCF_HELP, default=None)
+    g.add_argument('--lift_mapped_bam', help=LIFT_HELP, action='store_true', default=False)
     mg = sub.add_parser('metagenome', help="Run the simulator on metagenome mode")
     mg.add_argument('-gl', '--genome_list', help="Reference metagenome list, tsv file, the first column is species/strain "
                     "name, the second column is the reference genome fasta/fastq file directory", required=True)
@@ -787,11 +799,12 @@ def coverage_to_reads(prof, cm, coverage):
 
 
 def _mapped_refs(args, prof, circular):
-    """--mapped_bam: bam_refs of the resident reference, None without the flag; a repeated name is a usage error."""
+    """--mapped_bam: bam_refs of the resident reference (of the haploid one with --lift_mapped_bam), None without the flag;
+    a repeated name is a usage error."""
     if not args.mapped_bam:
         return None
     try:
-        return bam_refs(prof.ref, circular)
+        return bam_refs(prof.haploid if getattr(args, "lift_mapped_bam", False) else prof.ref, circular)
     except ValueError as e:
         sys.stderr.write("\n--mapped_bam: %s!\n" % e)
         sys.exit(1)
@@ -814,6 +827,10 @@ def main(argv=None):
         usage = "--mapped_bam is not available in transcriptome mode: reads that retain an intron lie on the genome"
     elif args.mapped_bam and not args.bam:
         usage = "--mapped_bam needs --bam"
+    elif getattr(args, "lift_mapped_bam", False) and not args.vcf:
+        usage = "--lift_mapped_bam needs --vcf"
+    elif getattr(args, "lift_mapped_bam", False) and not args.mapped_bam:
+        usage = "--lift_mapped_bam needs --mapped_bam"
     if usage:
         sys.stderr.write("\n" + usage + "!\n")
         {"genome": parser_g, "metagenome": parser_mg, "transcriptome": parser_t}[args.mode].print_help(sys.stderr)
@@ -865,7 +882,8 @@ def main(argv=None):
 
     prof = read_profile(args.ref_g, number, args.model_prefix, args.perfect, args.mode, args.strandness,
                         dna_type=args.dna_type, chimeric=args.chimeric, homopolymer=args.homopolymer, fastq=args.fastq,
-                        device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args), vcf=args.vcf)
+                        device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args), vcf=args.vcf,
+                        lift=args.lift_mapped_bam)
     if args.coverage is not None:
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
