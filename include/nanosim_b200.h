@@ -270,6 +270,34 @@ int ns_apply_variants(NsContext* ctx, const NsVariants* variants);
  * ns_set_reference or ns_apply_variants drops the lift. */
 int ns_set_lift(NsContext* ctx, const NsVariants* variants);
 
+/* transcriptome --spliced_bam: where the transcripts lie on the genome, so that ns_compress_bam_mapped writes every read's
+ * true spliced alignment to the genome records (DESIGN.md §3 "Spliced mapped BAM").  Transcript t (resident record t,
+ * t < n_trx) has exons exon_off[t] .. exon_off[t+1]-1 in TRANSCRIPT order (descending on the minus strand), each bases
+ * [exon_start, exon_start + exon_len) of genome record exon_chrom (0 = the first genome record); none = the transcript has
+ * no map and its reads get ns_compress_bam's unmapped record.  minus[t]: the transcript's bases are the exons' read
+ * backwards and complemented.  genome_len: the genome records' lengths.  genome_first: the resident index of genome record
+ * 0 when the genome is resident behind the transcripts (intron retention: NsRunConfig.trx_records, the records reads that
+ * retain an intron lie on), NS_SPLICE_NO_GENOME when it is not.  Host pointers; the table (16 bytes per exon) is kept with
+ * the tables the context and its clones share.  NS_EINVAL (naming the transcript) when an exon leaves its genome record
+ * or is empty, the exons of a transcript lie on two records, are not monotone in transcript order or overlap, or do not
+ * add up to the transcript's resident length, and when the genome records are not the resident ones behind the
+ * transcripts.  peak_bytes, when given, receives the device bytes the map keeps.  Call before ns_clone; NS_ESTATE on a
+ * clone.  A later ns_set_reference drops the map. */
+#define NS_SPLICE_NO_GENOME 0xffffffffu
+typedef struct {
+    uint32_t n_trx;
+    const uint64_t* exon_off;        /* n_trx + 1 */
+    const uint32_t* exon_chrom;      /* exon_off[n_trx] each */
+    const uint32_t* exon_start;
+    const uint32_t* exon_len;
+    const uint8_t* minus;            /* n_trx */
+    uint32_t n_genome;
+    const uint64_t* genome_len;      /* n_genome */
+    uint32_t genome_first;
+    uint64_t* peak_bytes;            /* out, may be NULL */
+} NsSplice;
+int ns_set_splice(NsContext* ctx, const NsSplice* splice);
+
 int ns_configure(NsContext* ctx, const NsRunConfig* cfg);
 /* metagenome: dict_abun / dict_abun_inflated of the current sample (main() :2497-2514), one value per species in
  * genome-list order; resets the running per-species base counts that assign_species (:758-811) keeps per worker. */
@@ -415,8 +443,11 @@ int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off,
  * ns_fetch_compressed copies them.  When the context's tables carry a lift (ns_set_lift), the records are lifted onto the
  * haploid reference: refID is the haplotype's source record, POS is on it, a part inside an <INV> is a record on the
  * other strand, and every mapped record has HP:C:<1 or 2> as its first aux field (DESIGN.md §3 "Lifted mapped BAM").
- * NS_EINVAL when the last batch is unaligned reads, the context is in transcriptome mode, or a lift meets a circular
- * configuration. */
+ * In transcriptome mode the records are spliced onto the genome records of the context's splice map (ns_set_splice):
+ * refID is the genome record, an intron the read skips is an N, a minus-strand transcript's read is a record on the other
+ * strand, and every mapped record has XS:A:<+ or -> (the transcript's strand) as its first aux field (DESIGN.md §3
+ * "Spliced mapped BAM").  NS_EINVAL when the last batch is unaligned reads, the context is in transcriptome mode without
+ * a splice map (or with one whose records are not the run's), or a lift meets a circular configuration. */
 int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
 /* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' (or ns_compress_bam's)
  * *nbytes. */

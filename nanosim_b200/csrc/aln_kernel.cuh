@@ -6,11 +6,19 @@
 //   pass 2 (aln_write_kernel): the same walk writes the records' descriptors, CIGAR words and sizes
 // One thread per read: the rules (LIT groups, merging, trimming, the cut at a circular record's origin) are a sequential
 // state machine over the script, and each read's ops are contiguous in HBM.
-// kLift (ns_set_lift, DESIGN §3 "Lifted mapped BAM"): the same walk composes every op with the haplotype record's lift
+// ALN_LIFT (ns_set_lift, DESIGN §3 "Lifted mapped BAM"): the same walk composes every op with the haplotype record's lift
 // segments on the way, so the records are against the haploid reference the VCF describes.
+// ALN_SPLICE (ns_set_splice, DESIGN §3 "Spliced mapped BAM"): transcriptome reads, the walk composed with the transcript's
+// exons (or, for a read that retains an intron, with its chain of genome pieces), so the records are against the genome
+// with an N for every intron the read skips.
 #pragma once
 
+#include <type_traits>
+
 #include "haplotype.h"
+
+// which walk an aln kernel instantiation runs
+enum AlnMode : int { ALN_PLAIN = 0, ALN_LIFT = 1, ALN_SPLICE = 2 };
 
 // CIGAR operations (SAM/BAM specification §4.2.2: MIDNSHP=X -> 0..8)
 enum : uint32_t { CIG_M = 0, CIG_I = 1, CIG_D = 2, CIG_N = 3, CIG_S = 4, CIG_H = 5 };
@@ -41,11 +49,12 @@ __host__ __device__ __forceinline__ uint32_t bam_reg2bin(uint64_t beg, uint64_t 
     return 0;
 }
 
-// A lifted record keeps its HP value (1 or 2) in BamAln::flag's bits 12-15, above the BAM flag bits
+// A lifted record keeps its HP value (1 or 2) in BamAln::flag's bits 12-15, above the BAM flag bits; a spliced one its
+// transcript's strand there (0 +, 1 -)
 constexpr uint32_t BAM_FLAG_BITS = 0xfff, BAM_HP_SHIFT = 12;
 
 // bytes of a mapped record: the fixed fields, name, CIGAR (kSmN when it does not fit), bases, qualities, hp (4: a lifted
-// record's HP:C field), CG:B,I
+// record's HP:C field or a spliced one's XS:A field), CG:B,I
 __host__ __device__ __forceinline__ uint64_t bam_mapped_size(uint32_t nl, const BamAln& a, uint32_t hp = 0) {
     const bool cg = a.n_cig > BAM_MAX_CIGAR;
     return BAM_FIXED + nl + 1 + 4ull * (cg ? 2 : a.n_cig) + (a.l_seq + 1) / 2 + a.l_seq + hp + (cg ? 8 + 4ull * a.n_cig : 0);
@@ -71,11 +80,12 @@ struct BgzfMappedTable {
     }
 };
 
-// kLift: a mapped record also has the HP:C field of its haplotype (BamAln::flag >> BAM_HP_SHIFT) as its first aux field
-template <bool kLift>
+// ALN_LIFT: a mapped record also has the HP:C field of its haplotype (BamAln::flag >> BAM_HP_SHIFT) as its first aux
+// field; ALN_SPLICE: the XS:A field of its transcript's strand
+template <AlnMode kMode>
 struct BgzfMappedLayoutOf {
     using Table = BgzfMappedTable;
-    static constexpr uint32_t hp = kLift ? 4 : 0;
+    static constexpr uint32_t hp = kMode != ALN_PLAIN ? 4 : 0;
     static __device__ __forceinline__ uint8_t byte(uint64_t q, const BgzfMappedRec& rc) {
         const BamAln& a = rc.a;
         if (a.flag & 4) return BgzfBamLayout::byte(q, rc.rd);
@@ -89,7 +99,7 @@ struct BgzfMappedLayoutOf {
             case 1: w = a.ref_id; break;
             case 2: w = a.pos; break;
             case 3: w = (nl + 1) | (BAM_MAPQ << 8) | ((uint32_t)a.bin << 16); break;       // l_read_name, mapq, bin
-            case 4: w = nc | ((uint32_t)(kLift ? a.flag & BAM_FLAG_BITS : a.flag) << 16); break;   // n_cigar_op, flag
+            case 4: w = nc | ((uint32_t)(kMode != ALN_PLAIN ? a.flag & BAM_FLAG_BITS : a.flag) << 16); break;   // n_cigar_op, flag
             case 5: w = ls; break;                                                          // l_seq
             case 8: w = 0; break;                                                           // tlen
             default: w = 0xffffffffu;                                                       // next_refID, next_pos
@@ -122,9 +132,14 @@ struct BgzfMappedLayoutOf {
             return rc.rd.fastq ? (uint8_t)(rc.rd.ql[rc.rev ? L - 1 - f : f] - 33) : 0xffu;
         }
         q -= ls;
-        if (kLift) {
+        if (kMode == ALN_LIFT) {
             if (q < 3) return (uint8_t)"HPC"[q];
             if (q == 3) return (uint8_t)(a.flag >> BAM_HP_SHIFT);
+            q -= 4;
+        }
+        if (kMode == ALN_SPLICE) {
+            if (q < 3) return (uint8_t)"XSA"[q];
+            if (q == 3) return (uint8_t)(a.flag >> BAM_HP_SHIFT ? '-' : '+');
             q -= 4;
         }
         if (q < 4) return (uint8_t)"CGBI"[q];
@@ -133,8 +148,9 @@ struct BgzfMappedLayoutOf {
         return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
     }
 };
-struct BgzfMappedLayout : BgzfMappedLayoutOf<false> {};
-struct BgzfLiftedLayout : BgzfMappedLayoutOf<true> {};
+struct BgzfMappedLayout : BgzfMappedLayoutOf<ALN_PLAIN> {};
+struct BgzfLiftedLayout : BgzfMappedLayoutOf<ALN_LIFT> {};
+struct BgzfSplicedLayout : BgzfMappedLayoutOf<ALN_SPLICE> {};
 
 // ns_set_lift's table in HBM: haplotype record h's segments are seg[first[h] .. first[h + 1]) in haplotype order, their
 // kinds kind[...]; hap_chrom[h] its source record and hap_number[h] its HP value
@@ -216,6 +232,80 @@ __device__ __forceinline__ void lift_put(LiftWalk& w, uint32_t kind, uint32_t le
     }
 }
 
+// ns_set_splice's table in HBM: transcript t's exons are exon[first[t] .. first[t + 1]) in transcript order (none: no
+// map), minus[t] its strand; genome_first the resident index of genome record 0 (the chains' pieces lie on those records)
+struct SpliceExon {
+    uint32_t chrom, start, len;     // genome record (0 = the first -rg record), first base on it, bases
+    uint32_t cum;                   // transcript offset of its first base in transcript order
+};
+struct AlnSplice {
+    const SpliceExon* exon;
+    const uint64_t* first;
+    const uint8_t* minus;
+    uint32_t n_trx, genome_first;
+};
+
+// Where the splice walk stands: offset t in interval k of n_iv (a transcript's exons, or a chain's genome pieces), which is
+// bases [start, start + len) of genome record chrom, walked backwards when inv (minus strand).  The ops walked are those of
+// src[0], src[2], ... (n_src pieces: one transcript piece, or a chain's segments with their gap pieces between them).
+// Before each M or D: at, the genome coordinate of its first base (inv = false) or one past it (inv = true).
+struct SpliceWalk {
+    const SpliceExon* exon;         // the transcript's exons; nullptr: the intervals are the chain's pieces
+    const NsPieceMeta* src;
+    const uint32_t* ops;
+    uint32_t n_src, n_iv, k, t, genome_first;
+    uint32_t chrom, start, len, at;
+    bool inv;
+};
+
+__device__ __forceinline__ void splice_interval(const SpliceWalk& w, uint32_t k, uint32_t& chrom, uint32_t& start, uint32_t& len) {
+    if (w.exon) {
+        const SpliceExon e = w.exon[k];
+        chrom = e.chrom;
+        start = e.start;
+        len = e.len;
+    } else {
+        const NsPieceMeta& pc = w.src[2 * k];
+        chrom = pc.chrom - w.genome_first;
+        start = pc.pos;
+        len = pc.ref_len;
+    }
+}
+
+// A read op (M, I or D over the transcript, or over the chain's pieces back to back) composed with the intervals: I stays
+// I; an M or D that reaches the next interval's first base first emits the distance to it in the walk's direction as N
+// (nothing when it is 0: an exon and the retained intron beside it), or an ALN_CUT when that interval is on another record
+// or does not lie further on
+template <class Fn>
+__device__ __forceinline__ void splice_put(SpliceWalk& w, uint32_t kind, uint32_t len, Fn& fn) {
+    if (kind == CIG_I) {
+        fn(CIG_I, len);
+        return;
+    }
+    while (len) {
+        if (w.t >= w.len && w.k + 1 < w.n_iv) {
+            uint32_t c, s, l;
+            splice_interval(w, w.k + 1, c, s, l);
+            const int64_t gap = w.inv ? (int64_t)w.start - ((int64_t)s + l) : (int64_t)s - ((int64_t)w.start + w.len);
+            if (c != w.chrom || gap < 0) fn(ALN_CUT, 0u);
+            else if (gap) fn(CIG_N, (uint32_t)gap);
+            ++w.k;
+            w.t = 0;
+            w.chrom = c;
+            w.start = s;
+            w.len = l;
+        }
+        const uint32_t n = w.t < w.len ? min(len, w.len - w.t) : len;     // past the last interval (no valid map gets here)
+        w.at = w.inv ? w.start + w.len - w.t : w.start + w.t;
+        fn(kind, n);
+        w.t += n;
+        len -= n;
+    }
+}
+
+template <AlnMode kMode>
+using AlnWalk = std::conditional_t<kMode == ALN_SPLICE, SpliceWalk, LiftWalk>;
+
 struct AlnArgs {
     const NsReadMeta* reads;
     const NsPieceMeta* pieces;
@@ -234,23 +324,28 @@ struct AlnArgs {
     BamAln* aln;                    // pass 2 writes
     uint32_t* cigar;
     uint64_t* rec_size;
-    AlnLift lift;                   // kLift only
+    AlnLift lift;                   // ALN_LIFT only
+    AlnSplice splice;               // ALN_SPLICE only
 };
 
 // fn(kind, len) over a segment's script: CIGAR kinds M I D (HT as I: it only stands at a read's edges), a LIT group followed
 // by a DEL as |n - r| I or D and then min(n, r) M, zero lengths dropped, and an ALN_CUT (len 0) before the reference base
 // at offset `cut` and every `period` bases behind it (a circular record's origin, each time the segment passes it; ~0:
 // none), an M or D across one split there
-// kLift: every op goes through lift_put on walk w instead (no circular record: cut is ~0)
-template <bool kLift, class Fn>
-__device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint32_t n_ops, uint64_t cut, uint64_t period, LiftWalk& w,
+// ALN_LIFT: every op goes through lift_put on walk w instead (no circular record: cut is ~0)
+// ALN_SPLICE: the scripts of w's n_src pieces back to back (sc, n_ops unused), every op through splice_put
+template <AlnMode kMode, class Walk, class Fn>
+__device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint32_t n_ops, uint64_t cut, uint64_t period, Walk& w,
                                            Fn fn) {
     uint64_t rf = 0;
     uint32_t lit = 0;
     auto put = [&](uint32_t kind, uint32_t len) {
         if (len == 0) return;
-        if constexpr (kLift) {
+        if constexpr (kMode == ALN_LIFT) {
             lift_put(w, kind, len, fn);
+            return;
+        } else if constexpr (kMode == ALN_SPLICE) {
+            splice_put(w, kind, len, fn);
             return;
         }
         if (kind != CIG_I) {
@@ -266,21 +361,29 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
         }
         fn(kind, len);
     };
-    for (uint32_t j = 0; j < n_ops; ++j) {
-        const uint32_t op = sc[j], ty = NS_OP_TYPE(op), ln = NS_OP_LEN(op);
-        if (ty == NS_OP_LIT) {
-            lit += ln;
-            continue;
+    uint32_t n_src = 1;
+    if constexpr (kMode == ALN_SPLICE) n_src = w.n_src;
+    for (uint32_t p = 0; p < n_src; ++p) {
+        if constexpr (kMode == ALN_SPLICE) {
+            sc = w.ops + w.src[2 * p].op_off;
+            n_ops = w.src[2 * p].n_ops;
         }
-        if (lit && ty == NS_OP_DEL) {
-            put(lit > ln ? CIG_I : CIG_D, lit > ln ? lit - ln : ln - lit);
-            put(CIG_M, min(lit, ln));
+        for (uint32_t j = 0; j < n_ops; ++j) {
+            const uint32_t op = sc[j], ty = NS_OP_TYPE(op), ln = NS_OP_LEN(op);
+            if (ty == NS_OP_LIT) {
+                lit += ln;
+                continue;
+            }
+            if (lit && ty == NS_OP_DEL) {
+                put(lit > ln ? CIG_I : CIG_D, lit > ln ? lit - ln : ln - lit);
+                put(CIG_M, min(lit, ln));
+                lit = 0;
+                continue;
+            }
+            put(CIG_I, lit);
             lit = 0;
-            continue;
+            put(ty == NS_OP_DEL ? CIG_D : (ty == NS_OP_COPY || ty == NS_OP_MIS) ? CIG_M : CIG_I, ln);
         }
-        put(CIG_I, lit);
-        lit = 0;
-        put(ty == NS_OP_DEL ? CIG_D : (ty == NS_OP_COPY || ty == NS_OP_MIS) ? CIG_M : CIG_I, ln);
     }
     put(CIG_I, lit);
 }
@@ -288,17 +391,17 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
 // The alignments of one segment (n_parts of them at most: the cuts split it), its ops starting at read offset q_start: for
 // each, sink.begin(q0, rf0) at its first M, sink.op(kind, len) for its merged ops, sink.end(q1, rf1) after its last M
 // (read offsets in the forward read, reference offsets in the segment).  Ops before the first M and after the last one
-// are outside the alignment: their I is clip, their D moves the start or is dropped.  Two walks per part: the first finds
-// the part's first and last M, the second emits what lies between them.  kLift: every walk starts from `start`, the first
-// one counts the parts (n_parts = 1 on entry), and sink.place(at, inv) follows sink.begin with the lift's position of the
-// first M.
-template <bool kLift, class Sink>
+// are outside the alignment: their I is clip, their D (or N) moves the start or is dropped.  Two walks per part: the first
+// finds the part's first and last M, the second emits what lies between them.  ALN_LIFT, ALN_SPLICE: every walk starts from
+// `start`, the first one counts the parts (n_parts = 1 on entry), and sink.place(w) follows sink.begin with the walk as it
+// stands at the first M (its position there).
+template <AlnMode kMode, class Sink>
 __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, uint64_t cut, uint64_t period, uint32_t n_parts,
-                                            uint32_t q_start, const LiftWalk& start, Sink& sink) {
+                                            uint32_t q_start, const AlnWalk<kMode>& start, Sink& sink) {
     for (uint32_t want = 0; want < n_parts; ++want) {
         uint32_t first = ~0u, last = 0, idx = 0, part = 0;
-        LiftWalk w = start;
-        aln_script<kLift>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t) {
+        AlnWalk<kMode> w = start;
+        aln_script<kMode>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t) {
             if (kind == ALN_CUT) {
                 ++part;
             } else if (kind == CIG_M && part == want) {
@@ -307,16 +410,16 @@ __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, 
             }
             ++idx;
         });
-        if constexpr (kLift) n_parts = part + 1;
+        if constexpr (kMode != ALN_PLAIN) n_parts = part + 1;
         if (first == ~0u) continue;
         idx = 0;
         uint32_t q = q_start, rf = 0, ck = 0, cl = 0;
         w = start;
-        aln_script<kLift>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t len) {
+        aln_script<kMode>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t len) {
             if (idx >= first && idx <= last) {
                 if (idx == first) {
                     sink.begin(q, rf);
-                    if constexpr (kLift) sink.place(w.at, w.inv);
+                    if constexpr (kMode != ALN_PLAIN) sink.place(w);
                     ck = kind;
                     cl = 0;
                 }
@@ -332,43 +435,83 @@ __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, 
                     sink.end(q + len, rf + len);
                 }
             }
-            if (kind != CIG_D) q += len;
+            if (kind != CIG_D && (kMode != ALN_SPLICE || kind != CIG_N)) q += len;     // an N (splice walk) takes no read bases
             if (kind != CIG_I) rf += len;
             ++idx;
         });
     }
 }
 
-// every alignment of read r, in the order of its segments: sink.segment(piece, record length) before each segment's.
-// kLift: the walk of a segment starts in the lift segment holding its first haplotype base, the last of its record's
-// segments that starts at or before it (binary search).
-template <bool kLift, class Sink>
-__device__ __forceinline__ void aln_read(const AlnArgs& a, const NsReadMeta& r, Sink& sink) {
-    for (uint32_t k = 0; k < r.n_pieces; ++k) {
-        const NsPieceMeta pc = a.pieces[r.piece_first + k];
-        if (NS_PIECE_KIND(pc.kind) != NS_PIECE_SEGMENT) continue;
-        const uint64_t clen = a.chrom_off[pc.chrom + 1] - a.chrom_off[pc.chrom];
-        // a segment that runs past its record's end (circular records only) is cut at the origin, as often as it passes it
-        uint64_t cut = ~0ull;
-        uint32_t n_parts = 1;
-        LiftWalk w{};
-        if constexpr (kLift) {
-            uint64_t lo = a.lift.first[pc.chrom], hi = a.lift.first[pc.chrom + 1];
-            w.s_last = hi - 1;
-            while (hi - lo > 1) {
-                const uint64_t mid = (lo + hi) >> 1;
-                if (a.lift.seg[mid].hap0 <= pc.pos) lo = mid; else hi = mid;
-            }
-            w.seg = a.lift.seg;
-            w.kind = a.lift.kind;
-            w.s = lo;
-            w.t = pc.pos - a.lift.seg[lo].hap0;
-        } else if ((uint64_t)pc.pos + pc.ref_len > clen) {
-            cut = clen > pc.pos ? clen - pc.pos : 0;
-            n_parts = 2 + (uint32_t)((pc.ref_len - 1 - cut) / clen);
+// ALN_SPLICE: read r's one alignment walk.  A read laid out on the genome (NS_PIECE_GENOME, it retains an intron) walks its
+// chain of genome pieces; any other read its transcript piece over the transcript's exons, starting in the exon that holds
+// its first base (binary search over the exons' transcript offsets).  A transcript without a map gives no alignment.
+template <class Sink>
+__device__ __forceinline__ void aln_read_spliced(const AlnArgs& a, const NsReadMeta& r, Sink& sink) {
+    if (r.n_pieces == 0) return;
+    const NsPieceMeta pc = a.pieces[r.piece_first];
+    if (NS_PIECE_KIND(pc.kind) != NS_PIECE_SEGMENT) return;
+    SpliceWalk w{};
+    w.src = a.pieces + r.piece_first;
+    w.ops = a.ops;
+    w.genome_first = a.splice.genome_first;
+    if (pc.kind & NS_PIECE_GENOME) {
+        w.n_src = w.n_iv = (r.n_pieces + 1u) / 2u;
+        w.inv = (pc.kind & NS_PIECE_REF_REV) != 0;
+    } else {
+        if (pc.chrom >= a.splice.n_trx) return;
+        uint64_t lo = a.splice.first[pc.chrom], hi = a.splice.first[pc.chrom + 1];
+        if (lo == hi) return;
+        w.exon = a.splice.exon + lo;
+        w.n_src = 1;
+        w.n_iv = (uint32_t)(hi - lo);
+        const uint64_t e0 = lo;
+        while (hi - lo > 1) {
+            const uint64_t mid = (lo + hi) >> 1;
+            if (a.splice.exon[mid].cum <= pc.pos) lo = mid; else hi = mid;
         }
-        sink.segment(pc, clen);
-        aln_segment<kLift>(a.ops + pc.op_off, pc.n_ops, cut, clen, n_parts, pc.out_rel, w, sink);
+        w.k = (uint32_t)(lo - e0);
+        w.t = pc.pos - a.splice.exon[lo].cum;
+        w.inv = a.splice.minus[pc.chrom] != 0;
+    }
+    splice_interval(w, w.k, w.chrom, w.start, w.len);
+    sink.segment(pc, 0);
+    aln_segment<ALN_SPLICE>(nullptr, 0, ~0ull, 0, 1, pc.out_rel, w, sink);
+}
+
+// every alignment of read r, in the order of its segments: sink.segment(piece, record length) before each segment's.
+// ALN_LIFT: the walk of a segment starts in the lift segment holding its first haplotype base, the last of its record's
+// segments that starts at or before it (binary search).
+template <AlnMode kMode, class Sink>
+__device__ __forceinline__ void aln_read(const AlnArgs& a, const NsReadMeta& r, Sink& sink) {
+    if constexpr (kMode == ALN_SPLICE) {
+        aln_read_spliced(a, r, sink);
+    } else {
+        for (uint32_t k = 0; k < r.n_pieces; ++k) {
+            const NsPieceMeta pc = a.pieces[r.piece_first + k];
+            if (NS_PIECE_KIND(pc.kind) != NS_PIECE_SEGMENT) continue;
+            const uint64_t clen = a.chrom_off[pc.chrom + 1] - a.chrom_off[pc.chrom];
+            // a segment that runs past its record's end (circular records only) is cut at the origin, as often as it passes it
+            uint64_t cut = ~0ull;
+            uint32_t n_parts = 1;
+            LiftWalk w{};
+            if constexpr (kMode == ALN_LIFT) {
+                uint64_t lo = a.lift.first[pc.chrom], hi = a.lift.first[pc.chrom + 1];
+                w.s_last = hi - 1;
+                while (hi - lo > 1) {
+                    const uint64_t mid = (lo + hi) >> 1;
+                    if (a.lift.seg[mid].hap0 <= pc.pos) lo = mid; else hi = mid;
+                }
+                w.seg = a.lift.seg;
+                w.kind = a.lift.kind;
+                w.s = lo;
+                w.t = pc.pos - a.lift.seg[lo].hap0;
+            } else if ((uint64_t)pc.pos + pc.ref_len > clen) {
+                cut = clen > pc.pos ? clen - pc.pos : 0;
+                n_parts = 2 + (uint32_t)((pc.ref_len - 1 - cut) / clen);
+            }
+            sink.segment(pc, clen);
+            aln_segment<kMode>(a.ops + pc.op_off, pc.n_ops, cut, clen, n_parts, pc.out_rel, w, sink);
+        }
     }
 }
 
@@ -382,7 +525,8 @@ struct AlnCount {
         rf0 = rf;
         body = 0;
     }
-    __device__ void place(uint32_t, bool) {}
+    template <class Walk>
+    __device__ void place(const Walk&) {}
     __device__ void op(uint32_t, uint32_t) { ++body; }
     __device__ void end(uint32_t q1, uint32_t rf1) {
         words += body + (q0 > 0) + (q1 < L);
@@ -394,7 +538,7 @@ struct AlnCount {
     }
 };
 
-template <bool kLift>
+template <AlnMode kMode>
 __global__ void aln_count_kernel(AlnArgs a) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n_reads) return;
@@ -406,15 +550,17 @@ __global__ void aln_count_kernel(AlnArgs a) {
     const NsReadMeta r = a.reads[i];
     AlnCount c;
     c.L = r.seq_len;
-    aln_read<kLift>(a, r, c);
+    aln_read<kMode>(a, r, c);
     a.n_rec[i] = c.n_aln ? c.n_aln : 1;                         // no alignment: the unmapped record
     a.n_cig[i] = c.words;
     a.primary[i] = c.prim;
 }
 
-// kLift: refID is the haplotype's source record and POS the lifted one; a part inside an <INV> is a record on the other
-// strand, its CIGAR words (written in haplotype order) reversed in place and its stored bases mirrored
-template <bool kLift>
+// ALN_LIFT: refID is the haplotype's source record and POS the lifted one; a part inside an <INV> is a record on the other
+// strand, its CIGAR words (written in haplotype order) reversed in place and its stored bases mirrored.  ALN_SPLICE: refID
+// is the genome record and POS the leftmost genome base; a minus-strand transcript's part is a record on the other strand
+// as an <INV> part is, and the strand goes into the XS field.
+template <AlnMode kMode>
 struct AlnWrite {
     uint32_t i, L, nl, prim, rev;
     BamAln* rec;                    // the read's records
@@ -436,9 +582,11 @@ struct AlnWrite {
         w0 = w;
         if (q > 0) cig[w++] = (q << 4) | (n_aln == prim ? CIG_S : CIG_H);
     }
-    __device__ void place(uint32_t a, bool in) {
-        at = a;
-        inv = in;
+    template <class Walk>
+    __device__ void place(const Walk& w) {
+        at = w.at;
+        inv = w.inv;
+        if constexpr (kMode == ALN_SPLICE) chrom = w.chrom;
     }
     __device__ void op(uint32_t kind, uint32_t len) { cig[w++] = (len << 4) | kind; }
     __device__ void end(uint32_t q1, uint32_t rf1) {
@@ -452,8 +600,8 @@ struct AlnWrite {
         b.span = rf1 - rf0;
         b.n_cig = w - w0;
         uint64_t p;
-        if constexpr (kLift) {
-            b.ref_id = lift.hap_chrom[chrom];
+        if constexpr (kMode != ALN_PLAIN) {
+            b.ref_id = kMode == ALN_LIFT ? lift.hap_chrom[chrom] : chrom;
             p = inv ? at - b.span : at;
             if (inv) {
                 if (!primary) b.q0 = L - q1;
@@ -469,21 +617,22 @@ struct AlnWrite {
         b.pos = (uint32_t)p;
         b.bin = (uint16_t)bam_reg2bin(p, p + b.span);
         b.flag = (uint16_t)(((rev ^ (uint32_t)inv) ? 16u : 0u) | (primary ? 0u : 0x800u));
-        if constexpr (kLift) b.flag |= (uint16_t)(lift.hap_number[chrom] << BAM_HP_SHIFT);
+        if constexpr (kMode == ALN_LIFT) b.flag |= (uint16_t)(lift.hap_number[chrom] << BAM_HP_SHIFT);
+        if constexpr (kMode == ALN_SPLICE) b.flag |= (uint16_t)((uint32_t)inv << BAM_HP_SHIFT);
         b.cig_off = cig_off + w0;
         rec[n_aln] = b;
-        size[n_aln] = bam_mapped_size(nl, b, kLift ? 4 : 0);
+        size[n_aln] = bam_mapped_size(nl, b, kMode != ALN_PLAIN ? 4 : 0);
         ++n_aln;
     }
 };
 
-template <bool kLift>
+template <AlnMode kMode>
 __global__ void aln_write_kernel(AlnArgs a) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n_reads) return;
     const NsReadMeta r = a.reads[i];
     const uint64_t r0 = a.rec_first[i];
-    AlnWrite<kLift> s;
+    AlnWrite<kMode> s;
     s.lift = a.lift;
     s.i = i;
     s.L = r.seq_len;
@@ -494,7 +643,7 @@ __global__ void aln_write_kernel(AlnArgs a) {
     s.cig_off = a.cig_first[i];
     s.cig = a.cigar + s.cig_off;
     s.size = a.rec_size + r0;
-    aln_read<kLift>(a, r, s);
+    aln_read<kMode>(a, r, s);
     if (s.n_aln == 0) {                                         // the unmapped record of ns_compress_bam
         BamAln b{};
         b.read = i;

@@ -128,6 +128,10 @@ struct Tables {
     // ns_set_lift: the lift table of the resident haplotype records (aln_kernel.cuh's AlnLift)
     DevBuf lift_seg, lift_kind, lift_first, lift_chrom, lift_hp;
     bool have_lift = false;
+    // ns_set_splice: the transcripts' exons on the genome records (aln_kernel.cuh's AlnSplice)
+    DevBuf splice_exon, splice_first, splice_minus;
+    uint32_t splice_n_trx = 0, splice_genome_first = NS_SPLICE_NO_GENOME;
+    bool have_splice = false;
 };
 
 // transcript lengths ascending + their record indices (ns_configure, transcriptome mode); a clone that configures another
@@ -811,6 +815,8 @@ int ns_set_reference(NsContext* ctx, const NsReference* ref) {
     tab.h_haploid_off.clear();
     tab.have_lift = false;
     for (DevBuf* b : {&tab.lift_seg, &tab.lift_kind, &tab.lift_first, &tab.lift_chrom, &tab.lift_hp}) b->release();
+    tab.have_splice = false;
+    for (DevBuf* b : {&tab.splice_exon, &tab.splice_first, &tab.splice_minus}) b->release();
     ctx->have_batch = false;
     ctx->opt_ok[0] = ctx->opt_ok[1] = false;
     return NS_OK;
@@ -973,6 +979,72 @@ int ns_set_lift(NsContext* ctx, const NsVariants* v) {
     tab.have_lift = true;
     if (v->peak_bytes)
         *v->peak_bytes = tab.lift_seg.cap + tab.lift_kind.cap + tab.lift_first.cap + tab.lift_chrom.cap + tab.lift_hp.cap;
+    return NS_OK;
+}
+
+int ns_set_splice(NsContext* ctx, const NsSplice* sp) {
+    static const char* fname = "ns_set_splice";
+    if (!ctx || !sp || !sp->exon_off || (sp->n_trx && !sp->minus) || (sp->n_genome && !sp->genome_len) ||
+        (sp->exon_off[sp->n_trx] && (!sp->exon_chrom || !sp->exon_start || !sp->exon_len)))
+        return fail(ctx, NS_EINVAL, "%s: null argument", fname);
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "%s: a cloned context shares its parent's tables", fname);
+    Tables& tab = *ctx->tables;
+    if (!tab.have_ref) return fail(ctx, NS_ESTATE, "%s: set the reference first (ns_set_reference or ns_bcast_nccl)", fname);
+    const std::vector<uint64_t>& off = tab.h_chrom_off;
+    const uint32_t n_res = tab.dref.n_chrom;
+    if (sp->n_trx > n_res) return fail(ctx, NS_EINVAL, "%s: %u transcripts for %u resident records", fname, sp->n_trx, n_res);
+    if (sp->genome_first != NS_SPLICE_NO_GENOME) {
+        if (sp->genome_first < sp->n_trx || (uint64_t)sp->genome_first + sp->n_genome != n_res)
+            return fail(ctx, NS_EINVAL, "%s: genome records %u .. %llu are not the resident records behind the %u transcripts", fname,
+                        sp->genome_first, (unsigned long long)sp->genome_first + sp->n_genome, sp->n_trx);
+        for (uint32_t g = 0; g < sp->n_genome; ++g) {
+            const uint64_t res = off[sp->genome_first + g + 1] - off[sp->genome_first + g];
+            if (sp->genome_len[g] != res)
+                return fail(ctx, NS_EINVAL, "%s: genome record %u has %llu bases, the resident record %u has %llu", fname, g,
+                            (unsigned long long)sp->genome_len[g], sp->genome_first + g, (unsigned long long)res);
+        }
+    }
+    if (sp->exon_off[0] != 0) return fail(ctx, NS_EINVAL, "%s: exon_off must start at 0", fname);
+    const uint64_t n_exon = sp->exon_off[sp->n_trx];
+    if (n_exon > 0xffffffffull) return fail(ctx, NS_EINVAL, "%s: %llu exons are too many", fname, (unsigned long long)n_exon);
+    std::vector<SpliceExon> ex(n_exon);
+    for (uint32_t t = 0; t < sp->n_trx; ++t) {
+        if (sp->exon_off[t + 1] < sp->exon_off[t]) return fail(ctx, NS_EINVAL, "%s: exon_off decreases at transcript %u", fname, t);
+        const bool minus = sp->minus[t] != 0;
+        uint64_t cum = 0;
+        for (uint64_t j = sp->exon_off[t]; j < sp->exon_off[t + 1]; ++j) {
+            const uint32_t c = sp->exon_chrom[j], s = sp->exon_start[j], l = sp->exon_len[j];
+            if (c >= sp->n_genome || l == 0 || (uint64_t)s + l > sp->genome_len[c])
+                return fail(ctx, NS_EINVAL, "%s: exon %llu of transcript %u leaves its genome record", fname,
+                            (unsigned long long)(j - sp->exon_off[t]), t);
+            if (j > sp->exon_off[t]) {
+                const uint32_t pc = sp->exon_chrom[j - 1], ps = sp->exon_start[j - 1], pl = sp->exon_len[j - 1];
+                if (c != pc || (minus ? s > ps : s < ps))
+                    return fail(ctx, NS_EINVAL, "%s: the exons of transcript %u are not monotone in transcript order at exon %llu", fname,
+                                t, (unsigned long long)(j - sp->exon_off[t]));
+                if (minus ? (uint64_t)s + l > ps : s < (uint64_t)ps + pl)
+                    return fail(ctx, NS_EINVAL, "%s: exons %llu and %llu of transcript %u overlap", fname,
+                                (unsigned long long)(j - 1 - sp->exon_off[t]), (unsigned long long)(j - sp->exon_off[t]), t);
+            }
+            ex[j] = SpliceExon{c, s, l, (uint32_t)cum};
+            cum += l;
+        }
+        const uint64_t res = off[t + 1] - off[t];
+        if (sp->exon_off[t + 1] > sp->exon_off[t] && cum != res)
+            return fail(ctx, NS_EINVAL, "%s: the exons of transcript %u add up to %llu bases, the resident record %u has %llu", fname, t,
+                        (unsigned long long)cum, t, (unsigned long long)res);
+    }
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    tab.have_splice = false;
+    CK(upload(tab.splice_exon, ex.data(), std::max<size_t>(ex.size(), 1) * sizeof(SpliceExon), st));
+    CK(upload(tab.splice_first, sp->exon_off, ((size_t)sp->n_trx + 1) * 8, st));
+    CK(upload(tab.splice_minus, sp->minus, std::max<size_t>(sp->n_trx, 1), st));
+    CK(cudaStreamSynchronize(st));
+    tab.splice_n_trx = sp->n_trx;
+    tab.splice_genome_first = sp->genome_first;
+    tab.have_splice = true;
+    if (sp->peak_bytes) *sp->peak_bytes = tab.splice_exon.cap + tab.splice_first.cap + tab.splice_minus.cap;
     return NS_OK;
 }
 
@@ -1835,10 +1907,14 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
     if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
     if (ctx->last_kind != NS_KIND_ALIGNED) return fail(ctx, NS_EINVAL, "%s: the last batch is unaligned reads, which have no alignment", fname);
-    if (ctx->hcfg.mode == 2)
-        return fail(ctx, NS_EINVAL, "%s: transcriptome reads are not written as mapped records", fname);
     const Tables& tab = *ctx->tables;
-    const bool lift = tab.have_lift;
+    const bool splice = ctx->hcfg.mode == 2;
+    if (splice && !tab.have_splice)
+        return fail(ctx, NS_EINVAL, "%s: transcriptome reads are written as mapped records only with a splice map (ns_set_splice)", fname);
+    if (splice && ctx->hcfg.trx_records && (tab.splice_n_trx != ctx->hcfg.trx_records || tab.splice_genome_first != ctx->hcfg.trx_records))
+        return fail(ctx, NS_EINVAL, "%s: the splice map's transcripts and genome records are not the run's (trx_records %u)", fname,
+                    ctx->hcfg.trx_records);
+    const bool lift = !splice && tab.have_lift;
     if (lift && ctx->hcfg.circular) return fail(ctx, NS_EINVAL, "%s: lifted records need linear haplotype records", fname);
     CK(cudaSetDevice(ctx->device));
     const uint32_t n = ctx->last.n_reads;
@@ -1870,8 +1946,11 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     if (lift)
         aa.lift = AlnLift{tab.lift_seg.as<HapLift>(), tab.lift_kind.as<uint8_t>(), tab.lift_first.as<uint64_t>(), tab.lift_chrom.as<uint32_t>(),
                           tab.lift_hp.as<uint8_t>()};
+    if (splice)
+        aa.splice = AlnSplice{tab.splice_exon.as<SpliceExon>(), tab.splice_first.as<uint64_t>(), tab.splice_minus.as<uint8_t>(), tab.splice_n_trx,
+                              tab.splice_genome_first};
     const unsigned grid = (n + 255) / 256;
-    CK(launch(ctx, lift ? aln_count_kernel<true> : aln_count_kernel<false>, grid, 256, 0, aa));
+    CK(launch(ctx, splice ? aln_count_kernel<ALN_SPLICE> : lift ? aln_count_kernel<ALN_LIFT> : aln_count_kernel<ALN_PLAIN>, grid, 256, 0, aa));
     // the record and CIGAR-word totals borrow the text and member-bytes slots, which the later scans overwrite
     uint64_t* rec_first = ctx->m_first.as<uint64_t>();
     if (int rc = scan_total(ctx, aa.n_rec, rec_first, n, NS_T_Z_TEXT)) return rc;
@@ -1895,7 +1974,7 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     aa.aln = ctx->m_aln.as<BamAln>();
     aa.cigar = ctx->m_cig.as<uint32_t>();
     aa.rec_size = ctx->scan_in.as<uint64_t>();
-    CK(launch(ctx, lift ? aln_write_kernel<true> : aln_write_kernel<false>, grid, 256, 0, aa));
+    CK(launch(ctx, splice ? aln_write_kernel<ALN_SPLICE> : lift ? aln_write_kernel<ALN_LIFT> : aln_write_kernel<ALN_PLAIN>, grid, 256, 0, aa));
     if (int rc = scan_total(ctx, aa.rec_size, ctx->z_rec_off.as<uint64_t>(), (uint32_t)n_rec, NS_T_Z_TEXT)) return rc;
     if (int rc = publish_totals_and_wait(ctx)) return rc;
     BgzfMembers zm;
@@ -1913,6 +1992,12 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
         lifted.rec_off = src.rec_off;
         lifted.n_recs = src.n_recs;
         if (int rc = deflate_members(ctx, lifted, zm, n_blocks)) return rc;
+    } else if (splice) {
+        BgzfRecords<BgzfSplicedLayout> spliced;
+        spliced.tab = src.tab;
+        spliced.rec_off = src.rec_off;
+        spliced.n_recs = src.n_recs;
+        if (int rc = deflate_members(ctx, spliced, zm, n_blocks)) return rc;
     } else if (int rc = deflate_members(ctx, src, zm, n_blocks)) {
         return rc;
     }

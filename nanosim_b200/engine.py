@@ -111,6 +111,19 @@ class Engine:
         self._check(self._lib.ns_set_lift(self._ctx, C.byref(_variants(tables, n))))
         return int(n.value)
 
+    def set_splice(self, m):
+        """transcriptome --spliced_bam: keeps the transcripts' exons on the genome records (a splice.SpliceMap; ns_set_splice),
+        so that compress_bam_mapped() writes the reads' spliced alignments to the genome.  Call before clone().  Returns the
+        device bytes the map keeps."""
+        n = C.c_uint64()
+        arrs = [np.ascontiguousarray(x, dtype=d) for x, d in ((m.exon_off, np.uint64), (m.exon_chrom, np.uint32), (m.exon_start, np.uint32),
+                                                               (m.exon_len, np.uint32), (m.minus, np.uint8), (m.genome_len, np.uint64))]
+        first = L.NS_SPLICE_NO_GENOME if m.genome_first is None else int(m.genome_first)
+        s = L.NsSplice(len(arrs[0]) - 1, _ptr(arrs[0]), _ptr(arrs[1]), _ptr(arrs[2]), _ptr(arrs[3]), _ptr(arrs[4]), len(arrs[5]), _ptr(arrs[5]),
+                       first, C.pointer(n))
+        self._check(self._lib.ns_set_splice(self._ctx, C.byref(s)))
+        return int(n.value)
+
     def set_abundance(self, abun, inflated=None):
         """dict_abun / dict_abun_inflated of one sample, per species in genome-list order (metagenome mode)."""
         a = np.ascontiguousarray(abun, dtype=np.float64)
@@ -297,7 +310,8 @@ class Engine:
     def compress_bam_mapped(self, names):
         """The last aligned batch as mapped BAM records, the true alignment of every read (``names`` as for compress_bam),
         as BGZF members built on the device and kept there (ns_compress_bam_mapped); they replace those of the last
-        compress_records() / compress_bam().  After set_lift() the records are lifted onto the haploid reference.  Returns
+        compress_records() / compress_bam().  After set_lift() the records are lifted onto the haploid reference; in
+        transcriptome mode set_splice() must come first, and the records are spliced onto the genome.  Returns
         their size in bytes; neither the BAM header nor the end-of-file block."""
         from .records import _name_blob
         blob, offs = _name_blob(names)

@@ -124,21 +124,23 @@ class _RemoteReference(PackedReference):
 
 def read_profile(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                  polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                 device=0, seed=0, ir_files=None, ref_on_host=True, vcf=None, lift=False):
+                 device=0, seed=0, ir_files=None, ref_on_host=True, vcf=None, lift=False, spliced=False):
     """read_profile (:244-591).  Under torchrun (WORLD_SIZE > 1) only rank 0 reads the reference files; the other ranks get
     names and offsets through torch.distributed and the bases through ONE NCCL broadcast into their HBM (ns_bcast_nccl).
     ref_on_host: those ranks also copy the bases back to the host, which only the plain error profile's formatter reads.
     vcf (genome mode): the reads come from the haplotypes of the VCF's first sample.  Rank 0 parses it and hands the
     tables to the other ranks; every rank builds the haplotypes in its HBM from the haploid reference (ns_apply_variants),
     and with ref_on_host copies them back to the host.  lift (``--lift_mapped_bam``): every rank also keeps the lift of the
-    haplotypes onto the haploid records (ns_set_lift), so that mapped BAM records are against those."""
+    haplotypes onto the haploid records (ns_set_lift), so that mapped BAM records are against those.  spliced
+    (transcriptome ``--spliced_bam``): rank 0 also builds the transcripts' map onto the genome records (prof.splice) and
+    their header list (prof.spliced_refs) and hands both to the other ranks."""
     rank, world = _dist_world()
     if world > 1:
         return _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun,
                                          polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host, vcf,
-                                         lift)
+                                         lift, spliced)
     prof = _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
-                               chimeric, homopolymer, fastq, device, seed, ir_files, vcf)
+                               chimeric, homopolymer, fastq, device, seed, ir_files, vcf, spliced)
     if prof.haplotypes is not None:
         _apply_variants(prof, prof.haplotypes, ref_on_host, lift)
     return prof
@@ -163,18 +165,20 @@ def _apply_variants(prof, tables, ref_on_host, lift=False):
 
 
 def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp,
-                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True, vcf=None, lift=False):
+                              model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True, vcf=None, lift=False,
+                              spliced=False):
     dist = _dist_init()
     box = [None]
     if rank == 0:
         prof = _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
-                                   chimeric, homopolymer, fastq, device, seed, ir_files, vcf)
+                                   chimeric, homopolymer, fastq, device, seed, ir_files, vcf, spliced)
         r = prof.ref
         box[0] = {"names": r.names, "raw": r.raw_names, "offsets": r.offsets, "haplotypes": prof.haplotypes,
                   "meta": (r.species, r.chrom_species, r.chrom_circular, r.chrom_keys) if mode == "metagenome" else None,
                   "nccl_id": prof.engine.nccl_unique_id(),
                   "extra": {k: getattr(prof, k) for k in ("samples", "number_list", "expr_chrom", "expr_weights", "polya_flags", "max_chrom",
-                                                          "n_trx", "coverage_ref_len", "counts", "number_aligned", "number_unaligned")
+                                                          "n_trx", "coverage_ref_len", "counts", "number_aligned", "number_unaligned",
+                                                          "splice", "spliced_refs")
                             if hasattr(prof, k)}}
     dist.broadcast_object_list(box, src=0)
     info = box[0]
@@ -222,7 +226,7 @@ def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per
 
 def _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                         polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                        device=0, seed=0, ir_files=None, vcf=None):
+                        device=0, seed=0, ir_files=None, vcf=None, spliced=False):
     prof = Profile()
     prof.ir = None
     prof.n_trx = 0
@@ -278,6 +282,8 @@ def _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness,
             prof.ref = PackedReference.concat(trx, genome)
             if prof.polya_flags is not None:
                 prof.polya_flags = np.concatenate([prof.polya_flags, np.zeros(len(genome.names), dtype=np.uint8)])
+        if spliced:
+            _splice_profile(prof, ref_g, _gff3_path(model_prefix, ir_files), st if model_ir else None, genome if model_ir else None)
     else:
         prof.ref = PackedReference.from_fasta(ref_g)
     if mode != "transcriptome":
@@ -314,6 +320,37 @@ def _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness,
         pr, al = build_alias(prof.expr_weights)
         prof.engine.set_expression(pr, al, prof.expr_chrom, prof.polya_flags)
     return prof
+
+
+def _gff3_path(model_prefix, ir_files):
+    """The GFF3 with the exon / intron features: --ir_gff3, else <model_prefix>_added_intron_final.gff3."""
+    base = model_prefix[:-4] if model_prefix.endswith(".npz") else model_prefix
+    return (ir_files or {}).get("gff3") or base + "_added_intron_final.gff3"
+
+
+def _splice_profile(prof, ref_g, gff3, st=None, genome=None):
+    """--spliced_bam: the map of the transcript records (the first ones of prof.ref) onto the -rg genome records
+    (prof.splice) and the genome's header list (prof.spliced_refs).  With intron retention the genome and the structures
+    are those it read, and the genome is resident behind the transcripts; without it only the genome's record names and
+    lengths are kept (its bases never reach the device) and the GFF3 is read here."""
+    from .intron_retention import TranscriptStructures
+    from .splice import build_splice_map
+    n_trx = prof.n_trx or len(prof.ref.names)
+    if genome is None:
+        g = PackedReference.from_fasta(ref_g)
+        genome = _RemoteReference(g.names, g.offsets, g.raw_names)
+    try:
+        prof.spliced_refs = bam_refs(genome)
+    except ValueError as e:
+        sys.stderr.write("\n--spliced_bam: %s!\n" % e)
+        sys.exit(1)
+    if st is None:
+        _log("Read in GFF3 annotation file")
+        st = TranscriptStructures.from_gff3(gff3, prof.ref.names[:n_trx], genome.raw_names)
+    prof.splice = build_splice_map(st, prof.ref.lengths[:n_trx], genome.lengths, n_trx if prof.n_trx else None)
+    expressed = np.unique(np.asarray(prof.expr_chrom, dtype=np.int64))
+    _log("%d expressed transcripts have no usable exon structure in %s: their reads are written unmapped"
+         % (int((~prof.splice.has_map()[expressed]).sum()), gff3))
 
 
 def _shard(n, rank, world):
@@ -502,6 +539,10 @@ GZIP_ERR_HELP = ('With --gzip or --bam: write the error profile as BGZF-compress
 BAM_HELP = ('Write the reads as unaligned BAM, <out>_aligned_reads.bam and <out>_unaligned_reads.bam (one unmapped record per '
             'read, as Dorado writes them), encoded and compressed on the GPU. The error profile stays plain text unless '
             '--gzip_error_profile is given (Default = False)')
+SPLICED_BAM_HELP = ('With --bam and -rg: write <out>_aligned_reads.bam as mapped records, the true spliced alignment of every '
+                    'aligned read to the -rg genome records (N for every intron the read skips, XS:A for the transcript\'s strand), '
+                    'built on the GPU with the exons of the GFF3 (--ir_gff3 or its default, also without intron retention). '
+                    'Read names, the error profile and <out>_unaligned_reads.bam are unchanged (Default = False)')
 MAPPED_BAM_HELP = ('With --bam: write <out>_aligned_reads.bam as mapped records, the true alignment of every aligned read to the '
                    'reference records (one record per segment, supplementary ones for chimeric reads, CIGAR from the simulated '
                    'errors), built on the GPU. <out>_unaligned_reads.bam is unchanged (Default = False)')
@@ -646,6 +687,7 @@ def build_parser():
     t.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     t.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     t.add_argument('--mapped_bam', help=argparse.SUPPRESS, action='store_true', default=False)     # a usage error here
+    t.add_argument('--spliced_bam', help=SPLICED_BAM_HELP, action='store_true', default=False)
     return parser, g, mg, t
 
 
@@ -686,6 +728,11 @@ def main_transcriptome(args, parser_t):
         print("\nPlease input basecaller to simulate polyA tails from.\n")
         parser_t.print_help(sys.stderr)
         sys.exit(1)
+    gff3 = _gff3_path(args.model_prefix, {"gff3": args.ir_gff3})
+    if args.spliced_bam and not os.path.exists(gff3):
+        sys.stderr.write("\n--spliced_bam: the GFF3 annotation %s does not exist!\n" % gff3)
+        parser_t.print_help(sys.stderr)
+        sys.exit(1)
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     device = args.device if args.device is not None else int(os.environ.get("LOCAL_RANK", "0"))
@@ -697,7 +744,12 @@ def main_transcriptome(args, parser_t):
     prof = read_profile(args.ref_g, number, args.model_prefix, args.perfect, "transcriptome", args.strandness,
                         ref_t=args.ref_t, dna_type="linear", model_ir=model_ir, polya=args.polya, exp=args.exp,
                         homopolymer=args.homopolymer, fastq=args.fastq, device=device, seed=args.seed or 0,
-                        ir_files={"markov": args.ir_markov_model, "gff3": args.ir_gff3}, ref_on_host=_plain_error_profile(args))
+                        ir_files={"markov": args.ir_markov_model, "gff3": args.ir_gff3}, ref_on_host=_plain_error_profile(args),
+                        spliced=args.spliced_bam)
+    mapped_refs = None
+    if args.spliced_bam:
+        prof.engine.set_splice(prof.splice)
+        mapped_refs = prof.spliced_refs
     if args.coverage is not None:
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
@@ -705,7 +757,7 @@ def main_transcriptome(args, parser_t):
     simulation(prof, "transcriptome", args.output, "transcriptome", args.perfect, args.KmerBias if args.homopolymer else None,
                args.basecaller, max_len, min_len, max(args.num_threads, 1), args.fastq, None, None, model_ir, args.uracil,
                args.polya, batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world,
-               gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam)
+               gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam, mapped_refs=mapped_refs)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
@@ -713,7 +765,7 @@ def main_transcriptome(args, parser_t):
         dist.barrier()
         if rank == 0:
             merge_rank_files(args.output, args.fastq, args.perfect, world, gzip=args.gzip,
-                             gzip_error_profile=args.gzip_error_profile, bam=args.bam)
+                             gzip_error_profile=args.gzip_error_profile, bam=args.bam, mapped_refs=mapped_refs)
         dist.barrier()
     _log("Finished!")
 
@@ -825,6 +877,10 @@ def main(argv=None):
         usage = "--gzip_error_profile needs --gzip or --bam"
     elif args.mapped_bam and args.mode == "transcriptome":
         usage = "--mapped_bam is not available in transcriptome mode: reads that retain an intron lie on the genome"
+    elif getattr(args, "spliced_bam", False) and not args.bam:
+        usage = "--spliced_bam needs --bam"
+    elif getattr(args, "spliced_bam", False) and not args.ref_g:
+        usage = "--spliced_bam needs -rg: its records are against the genome"
     elif args.mapped_bam and not args.bam:
         usage = "--mapped_bam needs --bam"
     elif getattr(args, "lift_mapped_bam", False) and not args.vcf:
