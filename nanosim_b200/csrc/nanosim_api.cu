@@ -141,6 +141,13 @@ struct TrxTable {
     uint32_t n = 0;
 };
 
+// the packed BGZF members of one compressed output of the last batch: `bytes` of `buf`, fetchable while `valid`
+struct MemberSlot {
+    DevBuf buf;
+    uint64_t bytes = 0;
+    bool valid = false;
+};
+
 }  // namespace
 
 struct NsContext {
@@ -172,15 +179,13 @@ struct NsContext {
     Event ev_pack;
     Event ev_block;                 // cudaEventBlockingSync: long waits sleep instead of spinning (wait_stream)
     // ns_compress_records: the uploaded names, record layout, members as the deflate kernel leaves them, and the packed
-    // BGZF members of the last batch (z_bytes of z_out; valid while have_z)
-    DevBuf z_names, z_name_off, z_name_len, z_rec_off, z_stage, z_msize, z_moff, z_trailer, z_out;
-    uint64_t z_bytes = 0;
-    bool have_z = false;
-    // ns_compress_error_profile: the rows of the last aligned batch and their BGZF members (ep_bytes of ep_out; valid while
-    // have_ep).  Names, layout and staging are the z_ buffers above: only the members outlive a call.
-    DevBuf ep_text, ep_out;
-    uint64_t ep_bytes = 0;
-    bool have_ep = false;
+    // BGZF members of the last batch
+    DevBuf z_names, z_name_off, z_name_len, z_rec_off, z_stage, z_msize, z_moff, z_trailer;
+    MemberSlot z_out;
+    // ns_compress_error_profile: the rows of the last aligned batch and their BGZF members.  Names, layout and staging are
+    // the z_ buffers above: only the members outlive a call.
+    DevBuf ep_text;
+    MemberSlot ep_out;
     // ns_compress_bam_mapped: per read its record and CIGAR-word counts (2n) and their offsets (2n), its primary alignment;
     // the records' descriptors and CIGAR words.  Its members go to z_out.
     DevBuf m_cnt, m_first, m_prim, m_aln, m_cig;
@@ -197,6 +202,33 @@ struct NsContext {
     ~NsContext() {
         if (stream) cudaStreamDestroy(stream);
     }
+};
+
+// NsContext::totals: the counters of a batch (ns_simulate zeroes them all) and of a compression (which zeroes its own, from
+// NS_T_Z_TEXT on), published to h_totals by publish_totals_and_wait
+enum TotalsSlot : int {
+    NS_T_PIECES,                // pieces of the batch
+    NS_T_OVERFLOW_OPS,          // script ops of the pieces of reads whose script overflowed its slot
+    NS_T_SEQ_BYTES,             // sequence bytes (read_layout)
+    NS_T_BASES,                 // bases (read_layout)
+    NS_T_SLOT_OPS,              // script ops of the capped slots
+    NS_T_FLAGGED,               // reads whose script overflowed its slot
+    NS_T_HP_OPS,                // script ops the homopolymer pass writes
+    NS_T_POOL_CURSOR,           // the bump pool of re-drawn unaligned reads (uread_kernel.cuh): its cursor,
+    NS_T_POOL,                  // its base
+    NS_T_POOL_SIZE,             // and its size
+    NS_T_PRIMARY,               // script ops of the primary area
+    NS_T_ABORT,                 // abort flags (bit 0: script area too small, bit 1: with the overflow area, bit 2: sequence
+                                // buffers too small)
+    NS_T_Z_TEXT,                // compression: text bytes
+    NS_T_Z_BYTES,               // compression: member bytes
+    NS_T_Z_OVERSIZE,            // compression: members above 64 KiB
+    NS_T_Z_LONG_NAMES,          // compression: read names too long for BAM
+    NS_T_COUNT,
+    // ns_compress_bam_mapped's record and CIGAR-word totals borrow the text and member-bytes slots, which its later scans
+    // overwrite
+    NS_T_M_RECORDS = NS_T_Z_TEXT,
+    NS_T_M_CIGAR_WORDS = NS_T_Z_BYTES,
 };
 
 // Wait for everything queued on the context's stream.  cudaStreamSynchronize spins: a host thread per overlapped context then
@@ -324,29 +356,23 @@ __global__ void pack_bases_kernel(const uint4* __restrict__ seq, uint32_t* __res
 // The batch totals the host needs mid-pipeline are written straight into mapped pinned host memory: a cudaMemcpy
 // would queue behind another context's multi-GB device->host transfer on the copy engine and serialise the pipelines.
 __global__ void publish_totals(const uint64_t* totals, volatile uint64_t* host) {
-    if (threadIdx.x < 16) host[threadIdx.x] = totals[threadIdx.x];
+    if (threadIdx.x < NS_T_COUNT) host[threadIdx.x] = totals[threadIdx.x];
     __threadfence_system();
 }
-// totals[] slots: 0 pieces, 1 overflow ops, 2 sequence bytes, 3 bases, 4 slot ops, 5 flagged reads, 6 hp ops, 7 pool cursor,
-// 8 pool base, 9 pool size, 10 primary ops, 11 abort flags (bit 0: script area too small, bit 1: with the overflow area,
-// bit 2: sequence buffers too small)
-#define NS_T_POOL 8
-#define NS_T_PRIMARY 10
-#define NS_T_ABORT 11
 // sync-free batches: what the host would compute from the scans, computed and checked against the capacities on the device
 __global__ void capacity_stage_a(uint64_t* totals, uint32_t fast_unaligned, uint64_t ops_cap) {
     if (threadIdx.x || blockIdx.x) return;
-    const uint64_t slot_ops = totals[4];
+    const uint64_t slot_ops = totals[NS_T_SLOT_OPS];
     const uint64_t pool_ops = fast_unaligned ? slot_ops / 16 + (1u << 20) : 0;
     totals[NS_T_POOL] = slot_ops;
-    totals[NS_T_POOL + 1] = pool_ops;
+    totals[NS_T_POOL_SIZE] = pool_ops;
     totals[NS_T_PRIMARY] = slot_ops + pool_ops;
     if (slot_ops + pool_ops + 4 > ops_cap) totals[NS_T_ABORT] |= 1u;
 }
 __global__ void capacity_stage_b(uint64_t* totals, uint64_t ops_cap, uint64_t seq_cap) {
     if (threadIdx.x || blockIdx.x) return;
-    if (totals[NS_T_PRIMARY] + totals[1] + 4 > ops_cap) totals[NS_T_ABORT] |= 2u;
-    if (totals[2] + 16 > seq_cap) totals[NS_T_ABORT] |= 4u;
+    if (totals[NS_T_PRIMARY] + totals[NS_T_OVERFLOW_OPS] + 4 > ops_cap) totals[NS_T_ABORT] |= 2u;
+    if (totals[NS_T_SEQ_BYTES] + 16 > seq_cap) totals[NS_T_ABORT] |= 4u;
 }
 __global__ void gather_read_bytes(const NsReadMeta* reads, uint32_t n, uint64_t* out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -552,16 +578,16 @@ int scan_total(NsContext* ctx, const uint64_t* in, uint64_t* out, uint32_t n, in
     return NS_OK;
 }
 
-// a 16-byte aligned sequence slot per read: reads[i].seq_off, totals[2] = sequence bytes, totals[3] = bases
+// a 16-byte aligned sequence slot per read: reads[i].seq_off, and the sequence bytes and bases in totals
 int read_layout(NsContext* ctx, uint32_t n) {
     const unsigned gb = (n + 255) / 256;
     NsReadMeta* reads = ctx->reads.as<NsReadMeta>();
     uint64_t* totals = ctx->totals.as<uint64_t>();
     CK(launch(ctx, gather_read_bytes, gb, 256, 0, reads, n, ctx->scan_in.as<uint64_t>()));
-    if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n, 2)) return rc;
+    if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->scan_out.as<uint64_t>(), n, NS_T_SEQ_BYTES)) return rc;
     CK(launch(ctx, scatter_read_off, gb, 256, 0, reads, n, ctx->scan_out.as<uint64_t>()));
-    CK(cudaMemsetAsync(totals + 3, 0, sizeof(uint64_t), ctx->stream));
-    CK(launch(ctx, sum_bases, std::min(gb, 1024u), 256, 0, reads, n, (unsigned long long*)(totals + 3)));
+    CK(cudaMemsetAsync(totals + NS_T_BASES, 0, sizeof(uint64_t), ctx->stream));
+    CK(launch(ctx, sum_bases, std::min(gb, 1024u), 256, 0, reads, n, (unsigned long long*)(totals + NS_T_BASES)));
     return NS_OK;
 }
 
@@ -671,7 +697,7 @@ int ns_create(int device, uint64_t seed, NsContext** out) {
     cudaError_t e = cudaSetDevice(device);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
     for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = cudaEventCreate(&ctx->ev[i].e);
-    if (e == cudaSuccess) e = ctx->h_totals.ensure(16 * sizeof(uint64_t), cudaHostAllocMapped);
+    if (e == cudaSuccess) e = ctx->h_totals.ensure(NS_T_COUNT * sizeof(uint64_t), cudaHostAllocMapped);
     if (e == cudaSuccess) e = cudaHostGetDevicePointer((void**)&ctx->h_totals_dev, ctx->h_totals.p, 0);
     if (e == cudaSuccess && device >= 0 && device < 64 && !g_base[device]) {
         e = cudaEventCreate(&g_base[device]);
@@ -1397,8 +1423,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     ctx->have_batch = false;
-    ctx->have_z = false;
-    ctx->have_ep = false;
+    ctx->z_out.valid = ctx->ep_out.valid = false;
     memset(&ctx->last, 0, sizeof ctx->last);
     if (n_reads == 0) {
         if (info) *info = ctx->last;
@@ -1420,15 +1445,15 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     const unsigned tb = 256, gb = (n + tb - 1) / tb;
     CK(ctx->reads.ensure((size_t)n * sizeof(NsReadMeta)));
     CK(ctx->counter.ensure(64));
-    CK(ctx->totals.ensure(16 * sizeof(uint64_t)));
+    CK(ctx->totals.ensure(NS_T_COUNT * sizeof(uint64_t)));
     CK(ctx->scan_in.ensure((size_t)n * (2 * NS_MAX_SEGMENTS) * sizeof(uint64_t)));
     CK(ctx->scan_out.ensure((size_t)n * (2 * NS_MAX_SEGMENTS) * sizeof(uint64_t)));
-    CK(cudaMemsetAsync(ctx->totals.p, 0, 16 * sizeof(uint64_t), st));
+    CK(cudaMemsetAsync(ctx->totals.p, 0, NS_T_COUNT * sizeof(uint64_t), st));
     CK(cudaEventRecord(ctx->ev[0], st));
     const uint64_t ops_cap = ctx->ops.cap / sizeof(uint32_t), seq_cap = ctx->seq.cap;
     uint64_t* d_totals = ctx->totals.as<uint64_t>();
     const uint64_t* h_totals = ctx->h_totals.as<uint64_t>();      // as of the last publish_totals_and_wait
-    auto script_ops = [h_totals] { return h_totals[NS_T_PRIMARY] + h_totals[1] + h_totals[6]; };
+    auto script_ops = [h_totals] { return h_totals[NS_T_PRIMARY] + h_totals[NS_T_OVERFLOW_OPS] + h_totals[NS_T_HP_OPS]; };
     uint64_t* scan_in = ctx->scan_in.as<uint64_t>();
     uint64_t* scan_out = ctx->scan_out.as<uint64_t>();
     const uint32_t* d_abort = sync_free ? (const uint32_t*)(d_totals + NS_T_ABORT) : nullptr;
@@ -1444,10 +1469,10 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         CK(launch(ctx, segments_kernel, gb, tb, 0, tab.dmodel, ctx->dcfg, (uint32_t)kind, first_read_id, n, ctx->nseg.as<uint32_t>(),
                   ctx->npieces.as<uint32_t>()));
         CK(launch(ctx, widen_u32, gb, tb, 0, ctx->npieces.as<uint32_t>(), n, scan_in));
-        if (int rc = scan_total(ctx, scan_in, scan_out, n, 0)) return rc;
+        if (int rc = scan_total(ctx, scan_in, scan_out, n, NS_T_PIECES)) return rc;
         CK(launch(ctx, narrow_u64, gb, tb, 0, scan_out, n, ctx->piece_first.as<uint32_t>()));
         if (int rc = publish_totals_and_wait(ctx)) return rc;
-        n_pieces = (uint32_t)h_totals[0];
+        n_pieces = (uint32_t)h_totals[NS_T_PIECES];
         d_nseg = ctx->nseg.as<uint32_t>();
         d_pfirst = ctx->piece_first.as<uint32_t>();
     }
@@ -1468,9 +1493,9 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     CK(launch(ctx, lengths_kernel, gb, tb, 0, tab.dmodel, ctx->dcfg, (uint32_t)kind, first_read_id, n, d_nseg, d_pfirst, pieces,
               1.0f / std::max(1.0f, tab.hmodel.mean_ref_per_event), std::min(8.0f, std::max(1.0f, tab.hmodel.ref_per_event_cv)),
               exact_only ? 1u : 0u, scan_in, keys_in, vals_in));
-    if (int rc = scan_total(ctx, scan_in, scan_out, n_pieces, 4)) return rc;
+    if (int rc = scan_total(ctx, scan_in, scan_out, n_pieces, NS_T_SLOT_OPS)) return rc;
     CK(launch(ctx, scatter_piece_off, gp, tb, 0, pieces, n_pieces, scan_out));
-    CK(launch(ctx, set_sentinel_off, 1, 32, 0, pieces, n_pieces, d_totals + 4));
+    CK(launch(ctx, set_sentinel_off, 1, 32, 0, pieces, n_pieces, d_totals + NS_T_SLOT_OPS));
     if (int rc = sort_pairs_descending(ctx, keys_in, keys_out, vals_in, vals_out, n)) return rc;
     // primary script area = the capped slots (+ a bump pool for re-drawn unaligned reads, uread_kernel.cuh)
     CK(launch(ctx, capacity_stage_a, 1, 32, 0, d_totals, fast_unaligned ? 1u : 0u, sync_free ? ops_cap : ~0ull));
@@ -1529,7 +1554,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     pa.ops = ctx->ops.as<uint32_t>();
     pa.order = vals_out;
     pa.counter = ctx->counter.as<uint32_t>();
-    pa.n_flagged = (uint32_t*)(d_totals + 5);
+    pa.n_flagged = (uint32_t*)(d_totals + NS_T_FLAGGED);
     pa.batch_reversed = batch_reversed;
     pa.abort = d_abort;
     const unsigned plan_tb = 128;
@@ -1553,7 +1578,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     ua.order = vals_out;
     ua.counter = pa.counter;
     ua.n_flagged = pa.n_flagged;
-    ua.pool_cursor = (unsigned long long*)(d_totals + 7);
+    ua.pool_cursor = (unsigned long long*)(d_totals + NS_T_POOL_CURSOR);
     ua.pool = d_totals + NS_T_POOL;             // {base, size} of the bump pool, written by capacity_stage_a
     ua.abort = d_abort;
     ua.cta_min_len = (ctx->hcfg.flags & NS_FLAG_EMIT_WHOLE) ? 0u : (uint32_t)UREAD_CTA_MIN_LEN;
@@ -1583,18 +1608,18 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     // ---- sequence slots per read (scan); exact offsets for scripts that overflowed their slot
     if (int rc = read_layout(ctx, n)) return rc;
     CK(launch(ctx, gather_flagged_ops, gp, tb, 0, pieces, reads, n_pieces, scan_in));
-    if (int rc = scan_total(ctx, scan_in, scan_out, n_pieces, 1)) return rc;
+    if (int rc = scan_total(ctx, scan_in, scan_out, n_pieces, NS_T_OVERFLOW_OPS)) return rc;
     if (sync_free) {
         CK(launch(ctx, capacity_stage_b, 1, 32, 0, d_totals, ops_cap, seq_cap));
     } else {
         if (int rc = publish_totals_and_wait(ctx)) return rc;
-        CK(ctx->seq.ensure((size_t)h_totals[2] + 16));
-        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)h_totals[2] + 16));
+        CK(ctx->seq.ensure((size_t)h_totals[NS_T_SEQ_BYTES] + 16));
+        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)h_totals[NS_T_SEQ_BYTES] + 16));
     }
     CK(cudaEventRecord(ctx->ev[3], st));
     // rare: replay the flagged reads and write their scripts behind the primary area.  A sync-free batch does not know
     // whether there are any, so it always submits the (normally empty) replay.
-    if (sync_free || (uint32_t)h_totals[5] > 0) {
+    if (sync_free || (uint32_t)h_totals[NS_T_FLAGGED] > 0) {
         if (!sync_free)
             CK(ctx->ops.ensure_keep((size_t)(script_ops() + 4) * sizeof(uint32_t), (size_t)h_totals[NS_T_PRIMARY] * sizeof(uint32_t), st));
         pa.ops = ua.ops = ctx->ops.as<uint32_t>();
@@ -1637,7 +1662,7 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         CK(launch(ctx, hp_kernel<false>, hp_blocks, 128, 0, ha));
         CK(launch(ctx, hp_fix_reads, gb, tb, 0, reads, pieces, n));
         CK(ctx->hp_off.ensure((size_t)n_pieces * sizeof(uint64_t)));
-        if (int rc = scan_total(ctx, scan_in, ctx->hp_off.as<uint64_t>(), n_pieces, 6)) return rc;
+        if (int rc = scan_total(ctx, scan_in, ctx->hp_off.as<uint64_t>(), n_pieces, NS_T_HP_OPS)) return rc;
         CK(launch(ctx, add_base_u64, gp, tb, 0, ctx->hp_off.as<uint64_t>(), n_pieces, event_ops));
         if (int rc = read_layout(ctx, n)) return rc;
         if (int rc = publish_totals_and_wait(ctx)) return rc;
@@ -1645,8 +1670,8 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
         // filters them in place: ns_reemit lays retaining reads out on the genome by cutting the unfiltered scripts
         raw_ops = ctx->hcfg.trx_records ? event_ops : 0;
         CK(ctx->ops.ensure_keep((size_t)(script_ops() + raw_ops + 4) * sizeof(uint32_t), (size_t)event_ops * sizeof(uint32_t), st));
-        CK(ctx->seq.ensure((size_t)h_totals[2] + 16));
-        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)h_totals[2] + 16));
+        CK(ctx->seq.ensure((size_t)h_totals[NS_T_SEQ_BYTES] + 16));
+        if (ctx->hcfg.fastq) CK(ctx->qual.ensure((size_t)h_totals[NS_T_SEQ_BYTES] + 16));
         if (raw_ops) {
             raw_ev_off = script_ops();
             CK(cudaMemcpyAsync(ctx->ops.as<uint32_t>() + raw_ev_off, ctx->ops.p, (size_t)raw_ops * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
@@ -1689,10 +1714,10 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     }
 
     NsBatchInfo& bi = ctx->last;
-    bi.seq_bytes = h_totals[2];
+    bi.seq_bytes = h_totals[NS_T_SEQ_BYTES];
     bi.n_ops = script_ops() + raw_ops;
     bi.raw_ev_off = raw_ev_off;
-    bi.total_bases = h_totals[3];
+    bi.total_bases = h_totals[NS_T_BASES];
     bi.n_reads = n;
     bi.n_pieces = n_pieces;
     auto ms = [](cudaEvent_t a, cudaEvent_t b) {
@@ -1751,76 +1776,105 @@ int ns_fetch(NsContext* ctx, uint8_t* seq, uint8_t* qual, NsReadMeta* reads, NsP
     return NS_OK;
 }
 
-// totals[] slots of ns_compress_records (behind the batch's): text bytes, compressed bytes, members above 64 KiB; of
-// ns_compress_bam: read names too long for BAM
-#define NS_T_Z_TEXT 12
-#define NS_T_Z_BYTES 13
-#define NS_T_Z_OVERSIZE 14
-#define NS_T_Z_LONG_NAMES 15
+extern "C++" {    // templates cannot have C linkage
 
-// the n names (ns_format_records' layout) into z_names / z_name_off; room for the names' lengths, the per-read sizes
-// (scan_in) and their offsets (z_rec_off); the totals slots of a compression zeroed
-static int upload_names(NsContext* ctx, const char* names, const uint64_t* name_off, uint32_t n) {
-    cudaStream_t st = ctx->stream;
-    uint64_t blob = 0;                      // the names' extent: every name with its NUL
-    for (uint32_t i = 0; i < n; ++i) blob = std::max<uint64_t>(blob, name_off[i] + strlen(names + name_off[i]) + 1);
-    CK(upload(ctx->z_names, names, blob, st));
-    CK(upload(ctx->z_name_off, name_off, (size_t)n * sizeof(uint64_t), st));
-    CK(ctx->z_name_len.ensure((size_t)n * sizeof(uint32_t)));
-    CK(ctx->z_rec_off.ensure((size_t)n * sizeof(uint64_t)));
-    CK(ctx->scan_in.ensure((size_t)n * sizeof(uint64_t)));
-    CK(cudaMemsetAsync(ctx->totals.as<uint64_t>() + NS_T_Z_TEXT, 0, 4 * sizeof(uint64_t), st));
+// The checks every compression makes first, in this order: its arguments, a simulated batch and, where the entry needs
+// aligned reads (`lacks`: what unaligned reads have none of), an aligned batch
+static int check_compress(NsContext* ctx, const char* fname, const char* names, const uint64_t* name_off, const uint64_t* nbytes,
+                          const char* lacks) {
+    if (!ctx) return NS_EINVAL;
+    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
+    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
+    if (lacks && ctx->last_kind != NS_KIND_ALIGNED)
+        return fail(ctx, NS_EINVAL, "%s: the last batch is unaligned reads, which have no %s", fname, lacks);
     return NS_OK;
 }
 
-// the last of a compression's steps: member offsets, their total (second host round trip), the members packed into `out`
-static int pack_members(NsContext* ctx, const char* fname, uint32_t n_blocks, DevBuf& out, uint64_t* total) {
+// After those checks and the entry's own: `out` invalidated and *n the last batch's reads.  A batch without reads leaves
+// `out` valid and empty.  Otherwise the n names (ns_format_records' layout) go into z_names / z_name_off, with room for the
+// names' lengths, the per-read sizes (scan_in) and their offsets (z_rec_off), and the totals slots of a compression zeroed.
+static int begin_members(NsContext* ctx, const char* names, const uint64_t* name_off, MemberSlot& out, uint64_t* nbytes,
+                         uint32_t* n) {
+    CK(cudaSetDevice(ctx->device));
+    out.valid = false;
+    out.bytes = 0;
+    *n = ctx->last.n_reads;
+    if (*n == 0) {
+        out.valid = true;
+        *nbytes = 0;
+        return NS_OK;
+    }
+    cudaStream_t st = ctx->stream;
+    uint64_t blob = 0;                      // the names' extent: every name with its NUL
+    for (uint32_t i = 0; i < *n; ++i) blob = std::max<uint64_t>(blob, name_off[i] + strlen(names + name_off[i]) + 1);
+    CK(upload(ctx->z_names, names, blob, st));
+    CK(upload(ctx->z_name_off, name_off, (size_t)*n * sizeof(uint64_t), st));
+    CK(ctx->z_name_len.ensure((size_t)*n * sizeof(uint32_t)));
+    CK(ctx->z_rec_off.ensure((size_t)*n * sizeof(uint64_t)));
+    CK(ctx->scan_in.ensure((size_t)*n * sizeof(uint64_t)));
+    CK(cudaMemsetAsync(ctx->totals.as<uint64_t>() + NS_T_Z_TEXT, 0, (NS_T_COUNT - NS_T_Z_TEXT) * sizeof(uint64_t), st));
+    return NS_OK;
+}
+
+// the host round trip after a size pass that counts the read names too long for BAM: NS_EINVAL names the first of them
+static int publish_sizes(NsContext* ctx, const char* fname, const char* names, const uint64_t* name_off, uint32_t n) {
+    if (int rc = publish_totals_and_wait(ctx)) return rc;
+    const uint64_t n_long = ctx->h_totals.as<uint64_t>()[NS_T_Z_LONG_NAMES];
+    if (n_long == 0) return NS_OK;
+    uint32_t i = 0;                                             // the first such name, for the message
+    while (i + 1 < n && strlen(names + name_off[i]) <= BAM_MAX_NAME) ++i;
+    return fail(ctx, NS_EINVAL, "%s: read %u has a name of %zu bytes, more than the %u BAM holds (%llu such reads)", fname, i,
+                strlen(names + name_off[i]), BAM_MAX_NAME, (unsigned long long)n_long);
+}
+
+// The back of every compression: the members of the `text` bytes of text that `src` brings into shared memory, staged
+// where bgzf_deflate_kernel leaves them; their offsets and total (the last host round trip); the members packed into `out`,
+// which becomes valid.  NS_EINVAL when the text is too much for one call.
+template <class Source>
+static int end_members(NsContext* ctx, const char* fname, uint64_t text, const Source& src, MemberSlot& out, uint64_t* nbytes) {
+    const uint64_t n_blocks64 = (text + BGZF_BLOCK - 1) / BGZF_BLOCK;
+    if (n_blocks64 > 0x7fffffffu) return fail(ctx, NS_EINVAL, "%s: %llu bytes of text is too much for one call", fname,
+                                              (unsigned long long)text);
+    const uint32_t n_blocks = (uint32_t)n_blocks64;
+    CK(ctx->z_stage.ensure((size_t)n_blocks * BGZF_SLOT));
+    CK(ctx->z_msize.ensure((size_t)n_blocks * sizeof(uint64_t)));
+    CK(ctx->z_moff.ensure((size_t)n_blocks * sizeof(uint64_t)));
+    CK(ctx->z_trailer.ensure((size_t)n_blocks * sizeof(uint2)));
+    const BgzfMembers zm{text, ctx->z_stage.as<uint8_t>(), ctx->z_msize.as<uint64_t>(), ctx->z_trailer.as<uint2>(),
+                         (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_OVERSIZE)};
+    const int smem = (int)sizeof(typename Source::Smem);
+    CK(cudaFuncSetAttribute(bgzf_deflate_kernel<Source>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CK(launch(ctx, bgzf_deflate_kernel<Source>, n_blocks, BGZF_THREADS, (size_t)smem, src, zm));
     if (int rc = scan_total(ctx, ctx->z_msize.as<uint64_t>(), ctx->z_moff.as<uint64_t>(), n_blocks, NS_T_Z_BYTES)) return rc;
     if (int rc = publish_totals_and_wait(ctx)) return rc;
     const uint64_t* h = ctx->h_totals.as<uint64_t>();
     if (h[NS_T_Z_OVERSIZE])
         return fail(ctx, NS_ESTATE, "%s: %llu BGZF members exceed %u bytes", fname, (unsigned long long)h[NS_T_Z_OVERSIZE],
                     BGZF_MAX_MEMBER);
-    *total = h[NS_T_Z_BYTES];
-    CK(out.ensure((size_t)*total));
+    const uint64_t total = h[NS_T_Z_BYTES];
+    CK(out.buf.ensure((size_t)total));
     CK(launch(ctx, bgzf_pack_kernel, n_blocks, 256, 0, (const uint8_t*)ctx->z_stage.p, (const uint64_t*)ctx->z_msize.p,
-              (const uint64_t*)ctx->z_moff.p, (const uint2*)ctx->z_trailer.p, out.as<uint8_t>()));
+              (const uint64_t*)ctx->z_moff.p, (const uint2*)ctx->z_trailer.p, out.buf.as<uint8_t>()));
     CK(wait_stream(ctx, false));
+    out.bytes = total;
+    out.valid = true;
+    *nbytes = total;
     return NS_OK;
 }
 
-// staging of the members of `text` bytes of text, where bgzf_deflate_kernel leaves them; NS_EINVAL when that is too
-// much for one call
-static int stage_members(NsContext* ctx, const char* fname, uint64_t text, BgzfMembers* zm, uint32_t* n_blocks) {
-    const uint64_t n_blocks64 = (text + BGZF_BLOCK - 1) / BGZF_BLOCK;
-    if (n_blocks64 > 0x7fffffffu) return fail(ctx, NS_EINVAL, "%s: %llu bytes of text is too much for one call", fname,
-                                              (unsigned long long)text);
-    *n_blocks = (uint32_t)n_blocks64;
-    CK(ctx->z_stage.ensure((size_t)*n_blocks * BGZF_SLOT));
-    CK(ctx->z_msize.ensure((size_t)*n_blocks * sizeof(uint64_t)));
-    CK(ctx->z_moff.ensure((size_t)*n_blocks * sizeof(uint64_t)));
-    CK(ctx->z_trailer.ensure((size_t)*n_blocks * sizeof(uint2)));
-    zm->text_bytes = text;
-    zm->stage = ctx->z_stage.as<uint8_t>();
-    zm->member_size = ctx->z_msize.as<uint64_t>();
-    zm->trailer = ctx->z_trailer.as<uint2>();
-    zm->oversize = (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_OVERSIZE);
-    return NS_OK;
-}
-
-static int fetch_members(NsContext* ctx, const char* fname, bool have, const DevBuf& src, uint64_t bytes, uint8_t* out, uint64_t cap) {
-    if (!have) return fail(ctx, NS_ESTATE, "%s: the last batch has not been compressed", fname);
-    if (cap < bytes) return fail(ctx, NS_ENOMEM, "%s: %llu bytes do not fit in %llu", fname, (unsigned long long)bytes,
-                                 (unsigned long long)cap);
-    if (bytes == 0) return NS_OK;
+static int fetch_members(NsContext* ctx, const char* fname, const MemberSlot& m, uint8_t* out, uint64_t cap) {
+    if (!m.valid) return fail(ctx, NS_ESTATE, "%s: the last batch has not been compressed", fname);
+    if (cap < m.bytes) return fail(ctx, NS_ENOMEM, "%s: %llu bytes do not fit in %llu", fname, (unsigned long long)m.bytes,
+                                   (unsigned long long)cap);
+    if (m.bytes == 0) return NS_OK;
     if (!out) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
     CK(cudaSetDevice(ctx->device));
-    CK(cudaMemcpyAsync(out, src.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(wait_stream(ctx, bytes >= (64u << 20)));
+    CK(cudaMemcpyAsync(out, m.buf.p, m.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(wait_stream(ctx, m.bytes >= (64u << 20)));
     return NS_OK;
 }
 
-// the last batch's reads with the names upload_names left on the device
+// the last batch's reads with the names begin_members left on the device
 static BgzfReadTable read_table(NsContext* ctx) {
     BgzfReadTable t;
     t.fastq = ctx->hcfg.fastq ? 1u : 0u;
@@ -1833,62 +1887,25 @@ static BgzfReadTable read_table(NsContext* ctx) {
     return t;
 }
 
-extern "C++" {    // templates cannot have C linkage
-
-// the n_blocks members of the text `src` brings into shared memory
-template <class Source>
-static int deflate_members(NsContext* ctx, const Source& src, const BgzfMembers& zm, uint32_t n_blocks) {
-    const int smem = (int)sizeof(typename Source::Smem);
-    CK(cudaFuncSetAttribute(bgzf_deflate_kernel<Source>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CK(launch(ctx, bgzf_deflate_kernel<Source>, n_blocks, BGZF_THREADS, (size_t)smem, src, zm));
-    return NS_OK;
-}
-
 // ns_compress_records (FASTA/FASTQ text) and ns_compress_bam (BAM records): the last batch's records in that layout as
 // BGZF members in z_out
 template <class Layout>
 static int compress_records(NsContext* ctx, const char* fname, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
-    if (!ctx) return NS_EINVAL;
-    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
-    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
-    CK(cudaSetDevice(ctx->device));
-    const NsBatchInfo& bi = ctx->last;
-    const uint32_t n = bi.n_reads;
-    ctx->have_z = false;
-    ctx->z_bytes = 0;
-    if (n == 0) {
-        ctx->have_z = true;
-        *nbytes = 0;
-        return NS_OK;
-    }
-    if (int rc = upload_names(ctx, names, name_off, n)) return rc;
+    uint32_t n = 0;
+    if (int rc = check_compress(ctx, fname, names, name_off, nbytes, nullptr)) return rc;
+    if (int rc = begin_members(ctx, names, name_off, ctx->z_out, nbytes, &n)) return rc;
+    if (n == 0) return NS_OK;
     const uint32_t fastq = ctx->hcfg.fastq ? 1u : 0u;
     CK(launch(ctx, record_size_kernel<Layout>, (n + 255) / 256, 256, 0, ctx->reads.as<NsReadMeta>(), n, ctx->z_names.as<char>(),
               ctx->z_name_off.as<uint64_t>(), fastq, ctx->z_name_len.as<uint32_t>(), ctx->scan_in.as<uint64_t>(),
               (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_LONG_NAMES)));
     if (int rc = scan_total(ctx, ctx->scan_in.as<uint64_t>(), ctx->z_rec_off.as<uint64_t>(), n, NS_T_Z_TEXT)) return rc;
-    if (int rc = publish_totals_and_wait(ctx)) return rc;
-    if (const uint64_t n_long = ctx->h_totals.as<uint64_t>()[NS_T_Z_LONG_NAMES]) {
-        uint32_t i = 0;                                         // the first such name, for the message
-        while (i + 1 < n && strlen(names + name_off[i]) <= BAM_MAX_NAME) ++i;
-        return fail(ctx, NS_EINVAL, "%s: read %u has a name of %zu bytes, more than the %u BAM holds (%llu such reads)", fname, i,
-                    strlen(names + name_off[i]), BAM_MAX_NAME, (unsigned long long)n_long);
-    }
-    const uint64_t text = ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT];
-    BgzfMembers zm;
-    uint32_t n_blocks = 0;
-    if (int rc = stage_members(ctx, fname, text, &zm, &n_blocks)) return rc;
+    if (int rc = publish_sizes(ctx, fname, names, name_off, n)) return rc;
     BgzfRecords<Layout> src;
     src.tab = read_table(ctx);
     src.rec_off = ctx->z_rec_off.as<uint64_t>();
     src.n_recs = n;
-    if (int rc = deflate_members(ctx, src, zm, n_blocks)) return rc;
-    uint64_t total = 0;
-    if (int rc = pack_members(ctx, fname, n_blocks, ctx->z_out, &total)) return rc;
-    ctx->z_bytes = total;
-    ctx->have_z = true;
-    *nbytes = total;
-    return NS_OK;
+    return end_members(ctx, fname, ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT], src, ctx->z_out, nbytes);
 }
 
 }  // extern "C++"
@@ -1903,38 +1920,27 @@ int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off,
 
 int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
     static const char* fname = "ns_compress_bam_mapped";
-    if (!ctx) return NS_EINVAL;
-    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
-    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
-    if (ctx->last_kind != NS_KIND_ALIGNED) return fail(ctx, NS_EINVAL, "%s: the last batch is unaligned reads, which have no alignment", fname);
+    if (int rc = check_compress(ctx, fname, names, name_off, nbytes, "alignment")) return rc;
     const Tables& tab = *ctx->tables;
-    const bool splice = ctx->hcfg.mode == 2;
-    if (splice && !tab.have_splice)
+    // the walk: spliced onto the genome in transcriptome mode, lifted onto the haploid records after ns_set_lift, else plain
+    const AlnMode mode = ctx->hcfg.mode == 2 ? ALN_SPLICE : tab.have_lift ? ALN_LIFT : ALN_PLAIN;
+    if (mode == ALN_SPLICE && !tab.have_splice)
         return fail(ctx, NS_EINVAL, "%s: transcriptome reads are written as mapped records only with a splice map (ns_set_splice)", fname);
-    if (splice && ctx->hcfg.trx_records && (tab.splice_n_trx != ctx->hcfg.trx_records || tab.splice_genome_first != ctx->hcfg.trx_records))
+    if (mode == ALN_SPLICE && ctx->hcfg.trx_records && (tab.splice_n_trx != ctx->hcfg.trx_records || tab.splice_genome_first != ctx->hcfg.trx_records))
         return fail(ctx, NS_EINVAL, "%s: the splice map's transcripts and genome records are not the run's (trx_records %u)", fname,
                     ctx->hcfg.trx_records);
-    const bool lift = !splice && tab.have_lift;
-    if (lift && ctx->hcfg.circular) return fail(ctx, NS_EINVAL, "%s: lifted records need linear haplotype records", fname);
-    CK(cudaSetDevice(ctx->device));
-    const uint32_t n = ctx->last.n_reads;
-    ctx->have_z = false;
-    ctx->z_bytes = 0;
-    if (n == 0) {
-        ctx->have_z = true;
-        *nbytes = 0;
-        return NS_OK;
-    }
-    if (int rc = upload_names(ctx, names, name_off, n)) return rc;
+    if (mode == ALN_LIFT && ctx->hcfg.circular) return fail(ctx, NS_EINVAL, "%s: lifted records need linear haplotype records", fname);
+    uint32_t n = 0;
+    if (int rc = begin_members(ctx, names, name_off, ctx->z_out, nbytes, &n)) return rc;
+    if (n == 0) return NS_OK;
     CK(ctx->m_cnt.ensure((size_t)2 * n * sizeof(uint64_t)));
     CK(ctx->m_first.ensure((size_t)2 * n * sizeof(uint64_t)));
     CK(ctx->m_prim.ensure((size_t)n * sizeof(uint32_t)));
-    uint64_t* totals = ctx->totals.as<uint64_t>();
     AlnArgs aa{};
     aa.reads = ctx->reads.as<NsReadMeta>();
     aa.pieces = ctx->pieces.as<NsPieceMeta>();
     aa.ops = ctx->ops.as<uint32_t>();
-    aa.chrom_off = ctx->tables->dref.chrom_off;
+    aa.chrom_off = tab.dref.chrom_off;
     aa.names = ctx->z_names.as<char>();
     aa.name_off = ctx->z_name_off.as<uint64_t>();
     aa.n_reads = n;
@@ -1942,95 +1948,61 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     aa.n_rec = ctx->m_cnt.as<uint64_t>();
     aa.n_cig = aa.n_rec + n;
     aa.primary = ctx->m_prim.as<uint32_t>();
-    aa.long_names = (unsigned long long*)(totals + NS_T_Z_LONG_NAMES);
-    if (lift)
-        aa.lift = AlnLift{tab.lift_seg.as<HapLift>(), tab.lift_kind.as<uint8_t>(), tab.lift_first.as<uint64_t>(), tab.lift_chrom.as<uint32_t>(),
-                          tab.lift_hp.as<uint8_t>()};
-    if (splice)
-        aa.splice = AlnSplice{tab.splice_exon.as<SpliceExon>(), tab.splice_first.as<uint64_t>(), tab.splice_minus.as<uint8_t>(), tab.splice_n_trx,
-                              tab.splice_genome_first};
-    const unsigned grid = (n + 255) / 256;
-    CK(launch(ctx, splice ? aln_count_kernel<ALN_SPLICE> : lift ? aln_count_kernel<ALN_LIFT> : aln_count_kernel<ALN_PLAIN>, grid, 256, 0, aa));
-    // the record and CIGAR-word totals borrow the text and member-bytes slots, which the later scans overwrite
+    aa.long_names = (unsigned long long*)(ctx->totals.as<uint64_t>() + NS_T_Z_LONG_NAMES);
     uint64_t* rec_first = ctx->m_first.as<uint64_t>();
-    if (int rc = scan_total(ctx, aa.n_rec, rec_first, n, NS_T_Z_TEXT)) return rc;
-    if (int rc = scan_total(ctx, aa.n_cig, rec_first + n, n, NS_T_Z_BYTES)) return rc;
-    if (int rc = publish_totals_and_wait(ctx)) return rc;
-    const uint64_t* h = ctx->h_totals.as<uint64_t>();
-    if (const uint64_t n_long = h[NS_T_Z_LONG_NAMES]) {
-        uint32_t i = 0;                                         // the first such name, for the message
-        while (i + 1 < n && strlen(names + name_off[i]) <= BAM_MAX_NAME) ++i;
-        return fail(ctx, NS_EINVAL, "%s: read %u has a name of %zu bytes, more than the %u BAM holds (%llu such reads)", fname, i,
-                    strlen(names + name_off[i]), BAM_MAX_NAME, (unsigned long long)n_long);
-    }
-    const uint64_t n_rec = h[NS_T_Z_TEXT], n_words = h[NS_T_Z_BYTES];
-    if (n_rec > 0xffffffffu) return fail(ctx, NS_EINVAL, "%s: %llu records are too many for one call", fname, (unsigned long long)n_rec);
-    CK(ctx->m_aln.ensure((size_t)n_rec * sizeof(BamAln)));
-    CK(ctx->m_cig.ensure((size_t)std::max<uint64_t>(n_words, 1) * sizeof(uint32_t)));
-    CK(ctx->scan_in.ensure((size_t)n_rec * sizeof(uint64_t)));
-    CK(ctx->z_rec_off.ensure((size_t)n_rec * sizeof(uint64_t)));
-    aa.rec_first = rec_first;
-    aa.cig_first = rec_first + n;
-    aa.aln = ctx->m_aln.as<BamAln>();
-    aa.cigar = ctx->m_cig.as<uint32_t>();
-    aa.rec_size = ctx->scan_in.as<uint64_t>();
-    CK(launch(ctx, splice ? aln_write_kernel<ALN_SPLICE> : lift ? aln_write_kernel<ALN_LIFT> : aln_write_kernel<ALN_PLAIN>, grid, 256, 0, aa));
-    if (int rc = scan_total(ctx, aa.rec_size, ctx->z_rec_off.as<uint64_t>(), (uint32_t)n_rec, NS_T_Z_TEXT)) return rc;
-    if (int rc = publish_totals_and_wait(ctx)) return rc;
-    BgzfMembers zm;
-    uint32_t n_blocks = 0;
-    if (int rc = stage_members(ctx, fname, h[NS_T_Z_TEXT], &zm, &n_blocks)) return rc;
-    BgzfRecords<BgzfMappedLayout> src;
-    src.tab.reads = read_table(ctx);
-    src.tab.aln = aa.aln;
-    src.tab.cigar = aa.cigar;
-    src.rec_off = ctx->z_rec_off.as<uint64_t>();
-    src.n_recs = (uint32_t)n_rec;
-    if (lift) {
-        BgzfRecords<BgzfLiftedLayout> lifted;
-        lifted.tab = src.tab;
-        lifted.rec_off = src.rec_off;
-        lifted.n_recs = src.n_recs;
-        if (int rc = deflate_members(ctx, lifted, zm, n_blocks)) return rc;
-    } else if (splice) {
-        BgzfRecords<BgzfSplicedLayout> spliced;
-        spliced.tab = src.tab;
-        spliced.rec_off = src.rec_off;
-        spliced.n_recs = src.n_recs;
-        if (int rc = deflate_members(ctx, spliced, zm, n_blocks)) return rc;
-    } else if (int rc = deflate_members(ctx, src, zm, n_blocks)) {
-        return rc;
-    }
-    uint64_t total = 0;
-    if (int rc = pack_members(ctx, fname, n_blocks, ctx->z_out, &total)) return rc;
-    ctx->z_bytes = total;
-    ctx->have_z = true;
-    *nbytes = total;
-    return NS_OK;
+    const unsigned grid = (n + 255) / 256;
+    // the rest, with the walk's kernels and record layout instantiated for that mode
+    auto run = [&](auto walk) -> int {
+        constexpr AlnMode kMode = decltype(walk)::value;
+        using Layout = std::conditional_t<kMode == ALN_LIFT, BgzfLiftedLayout,
+                                          std::conditional_t<kMode == ALN_SPLICE, BgzfSplicedLayout, BgzfMappedLayout>>;
+        if constexpr (kMode == ALN_LIFT)
+            aa.lift = AlnLift{tab.lift_seg.as<HapLift>(), tab.lift_kind.as<uint8_t>(), tab.lift_first.as<uint64_t>(),
+                              tab.lift_chrom.as<uint32_t>(), tab.lift_hp.as<uint8_t>()};
+        if constexpr (kMode == ALN_SPLICE)
+            aa.splice = AlnSplice{tab.splice_exon.as<SpliceExon>(), tab.splice_first.as<uint64_t>(), tab.splice_minus.as<uint8_t>(),
+                                  tab.splice_n_trx, tab.splice_genome_first};
+        CK(launch(ctx, aln_count_kernel<kMode>, grid, 256, 0, aa));
+        if (int rc = scan_total(ctx, aa.n_rec, rec_first, n, NS_T_M_RECORDS)) return rc;
+        if (int rc = scan_total(ctx, aa.n_cig, rec_first + n, n, NS_T_M_CIGAR_WORDS)) return rc;
+        if (int rc = publish_sizes(ctx, fname, names, name_off, n)) return rc;
+        const uint64_t* h = ctx->h_totals.as<uint64_t>();
+        const uint64_t n_rec = h[NS_T_M_RECORDS], n_words = h[NS_T_M_CIGAR_WORDS];
+        if (n_rec > 0xffffffffu) return fail(ctx, NS_EINVAL, "%s: %llu records are too many for one call", fname, (unsigned long long)n_rec);
+        CK(ctx->m_aln.ensure((size_t)n_rec * sizeof(BamAln)));
+        CK(ctx->m_cig.ensure((size_t)std::max<uint64_t>(n_words, 1) * sizeof(uint32_t)));
+        CK(ctx->scan_in.ensure((size_t)n_rec * sizeof(uint64_t)));
+        CK(ctx->z_rec_off.ensure((size_t)n_rec * sizeof(uint64_t)));
+        aa.rec_first = rec_first;
+        aa.cig_first = rec_first + n;
+        aa.aln = ctx->m_aln.as<BamAln>();
+        aa.cigar = ctx->m_cig.as<uint32_t>();
+        aa.rec_size = ctx->scan_in.as<uint64_t>();
+        CK(launch(ctx, aln_write_kernel<kMode>, grid, 256, 0, aa));
+        if (int rc = scan_total(ctx, aa.rec_size, ctx->z_rec_off.as<uint64_t>(), (uint32_t)n_rec, NS_T_Z_TEXT)) return rc;
+        if (int rc = publish_totals_and_wait(ctx)) return rc;
+        BgzfRecords<Layout> src;
+        src.tab = BgzfMappedTable{read_table(ctx), aa.aln, aa.cigar};
+        src.rec_off = ctx->z_rec_off.as<uint64_t>();
+        src.n_recs = (uint32_t)n_rec;
+        return end_members(ctx, fname, h[NS_T_Z_TEXT], src, ctx->z_out, nbytes);
+    };
+    if (mode == ALN_SPLICE) return run(std::integral_constant<AlnMode, ALN_SPLICE>{});
+    if (mode == ALN_LIFT) return run(std::integral_constant<AlnMode, ALN_LIFT>{});
+    return run(std::integral_constant<AlnMode, ALN_PLAIN>{});
 }
 
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap) {
     if (!ctx) return NS_EINVAL;
-    return fetch_members(ctx, "ns_fetch_compressed", ctx->have_z, ctx->z_out, ctx->z_bytes, out, cap);
+    return fetch_members(ctx, "ns_fetch_compressed", ctx->z_out, out, cap);
 }
 
 int ns_compress_error_profile(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
     static const char* fname = "ns_compress_error_profile";
-    if (!ctx) return NS_EINVAL;
-    if (!names || !name_off || !nbytes) return fail(ctx, NS_EINVAL, "%s: null argument", fname);
-    if (!ctx->have_batch) return fail(ctx, NS_ESTATE, "%s: no simulated batch", fname);
-    if (ctx->last_kind != NS_KIND_ALIGNED) return fail(ctx, NS_EINVAL, "%s: the last batch is unaligned reads, which have no error profile", fname);
-    CK(cudaSetDevice(ctx->device));
-    const NsBatchInfo& bi = ctx->last;
-    const uint32_t n = bi.n_reads;
-    ctx->have_ep = false;
-    ctx->ep_bytes = 0;
-    if (n == 0) {
-        ctx->have_ep = true;
-        *nbytes = 0;
-        return NS_OK;
-    }
-    if (int rc = upload_names(ctx, names, name_off, n)) return rc;
+    uint32_t n = 0;
+    if (int rc = check_compress(ctx, fname, names, name_off, nbytes, "error profile")) return rc;
+    if (int rc = begin_members(ctx, names, name_off, ctx->ep_out, nbytes, &n)) return rc;
+    if (n == 0) return NS_OK;
     const Tables& tab = *ctx->tables;
     EpArgs ea;
     ea.reads = ctx->reads.as<NsReadMeta>();
@@ -2053,30 +2025,21 @@ int ns_compress_error_profile(NsContext* ctx, const char* names, const uint64_t*
     if (int rc = publish_totals_and_wait(ctx)) return rc;
     const uint64_t text = ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT];
     if (text == 0) {                                            // no error events
-        ctx->have_ep = true;
+        ctx->ep_out.valid = true;
         *nbytes = 0;
         return NS_OK;
     }
-    BgzfMembers zm;
-    uint32_t n_blocks = 0;
-    if (int rc = stage_members(ctx, fname, text, &zm, &n_blocks)) return rc;
     CK(ctx->ep_text.ensure((size_t)text));
     ea.text = ctx->ep_text.as<uint8_t>();
     CK(launch(ctx, errprof_write_kernel, warps_grid, 256, 0, ea));
     BgzfRows src;
-    src.text = ctx->ep_text.as<uint8_t>();
-    if (int rc = deflate_members(ctx, src, zm, n_blocks)) return rc;
-    uint64_t total = 0;
-    if (int rc = pack_members(ctx, fname, n_blocks, ctx->ep_out, &total)) return rc;
-    ctx->ep_bytes = total;
-    ctx->have_ep = true;
-    *nbytes = total;
-    return NS_OK;
+    src.text = ea.text;
+    return end_members(ctx, fname, text, src, ctx->ep_out, nbytes);
 }
 
 int ns_fetch_compressed_error_profile(NsContext* ctx, uint8_t* out, uint64_t cap) {
     if (!ctx) return NS_EINVAL;
-    return fetch_members(ctx, "ns_fetch_compressed_error_profile", ctx->have_ep, ctx->ep_out, ctx->ep_bytes, out, cap);
+    return fetch_members(ctx, "ns_fetch_compressed_error_profile", ctx->ep_out, out, cap);
 }
 
 int ns_transfer_info(NsContext* ctx, uint32_t* packed_bases, uint32_t* n_threads) {
@@ -2186,8 +2149,7 @@ int ns_reemit(NsContext* ctx, const uint32_t* read_slots, const NsReadMeta* new_
     if (!read_slots || !new_reads || !new_pieces || (n_new_ops && !new_ops)) return fail(ctx, NS_EINVAL, "ns_reemit: null argument");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
-    ctx->have_z = false;
-    ctx->have_ep = false;
+    ctx->z_out.valid = ctx->ep_out.valid = false;
     NsBatchInfo& bi = ctx->last;
     const uint32_t old_np = bi.n_pieces;
     const uint64_t old_ops = bi.n_ops;

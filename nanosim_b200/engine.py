@@ -280,31 +280,29 @@ class Engine:
             return C.c_void_p(int(x)) if x else None
         self._check(self._lib.ns_fetch(self._ctx, vp(seq_ptr), vp(qual_ptr), vp(reads_ptr), vp(pieces_ptr), vp(ops_ptr)))
 
-    def compress_records(self, names):
-        """The last batch's FASTA/FASTQ records (read ``names``: a records.NameTable or a list of str) as BGZF members,
-        built on the device and kept there (ns_compress_records).  Returns their size in bytes; no end-of-file block."""
+    def _compress(self, name, names):
+        """ns_<name> over the last batch with its read ``names`` (a records.NameTable or a list of str) -> the size of the
+        members it keeps on the device."""
         from .records import _name_blob
         blob, offs = _name_blob(names)
         offs = np.ascontiguousarray(offs, dtype=np.uint64)
         if len(offs) != int(self.info.n_reads):
-            raise ValueError("compress_records: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
+            raise ValueError("%s: %d names for %d reads" % (name, len(offs), int(self.info.n_reads)))
         n = C.c_uint64()
-        self._check(self._lib.ns_compress_records(self._ctx, blob, _ptr(offs), C.byref(n)))
-        self._z_bytes = int(n.value)
+        self._check(getattr(self._lib, "ns_" + name)(self._ctx, blob, _ptr(offs), C.byref(n)))
+        return int(n.value)
+
+    def compress_records(self, names):
+        """The last batch's FASTA/FASTQ records (read ``names``: a records.NameTable or a list of str) as BGZF members,
+        built on the device and kept there (ns_compress_records).  Returns their size in bytes; no end-of-file block."""
+        self._z_bytes = self._compress("compress_records", names)
         return self._z_bytes
 
     def compress_bam(self, names):
         """The last batch's reads as unaligned BAM records (``names`` as for compress_records; at most 254 bytes each)
         as BGZF members, built on the device and kept there (ns_compress_bam); they replace those of the last
         compress_records().  Returns their size in bytes; neither the BAM header nor the end-of-file block."""
-        from .records import _name_blob
-        blob, offs = _name_blob(names)
-        offs = np.ascontiguousarray(offs, dtype=np.uint64)
-        if len(offs) != int(self.info.n_reads):
-            raise ValueError("compress_bam: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
-        n = C.c_uint64()
-        self._check(self._lib.ns_compress_bam(self._ctx, blob, _ptr(offs), C.byref(n)))
-        self._z_bytes = int(n.value)
+        self._z_bytes = self._compress("compress_bam", names)
         return self._z_bytes
 
     def compress_bam_mapped(self, names):
@@ -313,14 +311,7 @@ class Engine:
         compress_records() / compress_bam().  After set_lift() the records are lifted onto the haploid reference; in
         transcriptome mode set_splice() must come first, and the records are spliced onto the genome.  Returns
         their size in bytes; neither the BAM header nor the end-of-file block."""
-        from .records import _name_blob
-        blob, offs = _name_blob(names)
-        offs = np.ascontiguousarray(offs, dtype=np.uint64)
-        if len(offs) != int(self.info.n_reads):
-            raise ValueError("compress_bam_mapped: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
-        n = C.c_uint64()
-        self._check(self._lib.ns_compress_bam_mapped(self._ctx, blob, _ptr(offs), C.byref(n)))
-        self._z_bytes = int(n.value)
+        self._z_bytes = self._compress("compress_bam_mapped", names)
         return self._z_bytes
 
     def fetch_compressed(self, out=None):
@@ -335,14 +326,7 @@ class Engine:
         """The last aligned batch's error-profile rows (records.format_error_profile's bytes, no header line) as BGZF
         members, formatted and compressed on the device and kept there (ns_compress_error_profile).  ``names`` as for
         compress_records.  Returns their size in bytes (0: no error events); no end-of-file block."""
-        from .records import _name_blob
-        blob, offs = _name_blob(names)
-        offs = np.ascontiguousarray(offs, dtype=np.uint64)
-        if len(offs) != int(self.info.n_reads):
-            raise ValueError("compress_error_profile: %d names for %d reads" % (len(offs), int(self.info.n_reads)))
-        n = C.c_uint64()
-        self._check(self._lib.ns_compress_error_profile(self._ctx, blob, _ptr(offs), C.byref(n)))
-        self._ep_bytes = int(n.value)
+        self._ep_bytes = self._compress("compress_error_profile", names)
         return self._ep_bytes
 
     def fetch_compressed_error_profile(self, out=None):

@@ -65,7 +65,7 @@ class BatchPipeline:
         self.fetch, self.want_ops, self.want_pieces, self.compress = fetch, want_ops, want_pieces, compress
         self.compress_profile, self.bam, self.mapped_bam = compress_profile, bam, mapped_bam
         self.bufs = [_HostBuffers(engine.fastq) for _ in self.engines]
-        self.hint = {"seq": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0, "gz_err": 0}     # largest batch seen by any slot (pinned allocs are slow)
+        self.hint = {"seq": 0, "qual": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0, "gz_err": 0}     # largest batch seen by any slot (pinned allocs are slow)
 
     def close(self):
         for e in self.engines[1:]:
@@ -75,25 +75,26 @@ class BatchPipeline:
         kind, first, n = job
         return self.engines[slot].simulate(kind, first, n)
 
-    def _fetch(self, slot, job, info):
-        if self.compress is not None:
-            return self._fetch_compressed(slot, job, info)
-        kind, first, n = job
-        eng, hb = self.engines[slot], self.bufs[slot]
-        fastq = eng.fastq
-        nb = {"seq": int(info.seq_bytes), "reads": int(info.n_reads) * L.READ_DTYPE.itemsize,
+    def _pinned(self, slot, info):
+        """take(key) -> the slot's pinned buffer ``key`` cut to the batch's bytes, grown for the largest batch any slot has seen."""
+        nb = {"seq": int(info.seq_bytes), "qual": int(info.seq_bytes), "reads": int(info.n_reads) * L.READ_DTYPE.itemsize,
               "pieces": int(info.n_pieces) * L.PIECE_DTYPE.itemsize, "ops": int(info.n_ops) * 4}
         for k, v in nb.items():
             if v > self.hint[k]:
                 self.hint[k] = v
-        seq = hb.ensure("seq", nb["seq"], self.hint["seq"])[:nb["seq"]]
-        qual = hb.ensure("qual", nb["seq"], self.hint["seq"])[:nb["seq"]] if fastq else None
-        reads = hb.ensure("reads", nb["reads"], self.hint["reads"])[:nb["reads"]]
-        pieces = ops = None
-        if self.want_pieces:
-            pieces = hb.ensure("pieces", nb["pieces"], self.hint["pieces"])[:nb["pieces"]]
-        if self.want_ops and info.n_ops:
-            ops = hb.ensure("ops", nb["ops"], self.hint["ops"])[:nb["ops"]]
+        return lambda key: self.bufs[slot].ensure(key, nb[key], self.hint[key])[:nb[key]]
+
+    def _fetch(self, slot, job, info):
+        if self.compress is not None:
+            return self._fetch_compressed(slot, job, info)
+        kind, first, n = job
+        eng, hb, take = self.engines[slot], self.bufs[slot], self._pinned(slot, info)
+        fastq = eng.fastq
+        seq = take("seq")
+        qual = take("qual") if fastq else None
+        reads = take("reads")
+        pieces = take("pieces") if self.want_pieces else None
+        ops = take("ops") if self.want_ops and info.n_ops else None
         eng.fetch_into(hb.ptr("seq"), hb.ptr("qual") if fastq else None, hb.ptr("reads"),
                        hb.ptr("pieces") if pieces is not None else None, hb.ptr("ops") if ops is not None else None)
         return Batch(info, seq, qual, reads.view(L.READ_DTYPE), pieces.view(L.PIECE_DTYPE) if pieces is not None else None,
@@ -101,19 +102,14 @@ class BatchPipeline:
 
     def _fetch_compressed(self, slot, job, info):
         kind, first, n = job
-        eng, hb = self.engines[slot], self.bufs[slot]
-        nb = {"seq": int(info.seq_bytes), "reads": int(info.n_reads) * L.READ_DTYPE.itemsize,
-              "pieces": int(info.n_pieces) * L.PIECE_DTYPE.itemsize, "ops": int(info.n_ops) * 4}
-        for k, v in nb.items():
-            if v > self.hint[k]:
-                self.hint[k] = v
-        reads = hb.ensure("reads", nb["reads"], self.hint["reads"])[:nb["reads"]]
-        pieces = hb.ensure("pieces", nb["pieces"], self.hint["pieces"])[:nb["pieces"]]
+        eng, hb, take = self.engines[slot], self.bufs[slot], self._pinned(slot, info)
+        reads = take("reads")
+        pieces = take("pieces")
         seq = ops = None
         if self.want_ops:                  # the error-profile formatter reads bases back from the sequence
-            seq = hb.ensure("seq", nb["seq"], self.hint["seq"])[:nb["seq"]]
+            seq = take("seq")
             if info.n_ops:
-                ops = hb.ensure("ops", nb["ops"], self.hint["ops"])[:nb["ops"]]
+                ops = take("ops")
         eng.fetch_into(hb.ptr("seq") if seq is not None else None, None, hb.ptr("reads"), hb.ptr("pieces"),
                        hb.ptr("ops") if ops is not None else None)
         b = Batch(info, seq, None, reads.view(L.READ_DTYPE), pieces.view(L.PIECE_DTYPE),

@@ -16,6 +16,7 @@ import os
 import struct
 import sys
 import zlib
+from collections import namedtuple
 from textwrap import dedent
 from time import strftime
 
@@ -79,6 +80,29 @@ def bam_refs(ref, circular=False):
                              % (j, ref.names[j], i, ref.names[i], n))
         seen[n] = i
     return list(zip(names, lengths, circ))
+
+
+# One output file of a run: <out><name>, or <out><rank_name % r> for rank r's part under torchrun, which has neither header
+# nor trailer; members: its content arrives as BGZF members
+OutputFile = namedtuple("OutputFile", "name rank_name header trailer members")
+
+
+def output_files(fastq, gzip=False, gzip_error_profile=False, bam=False, mapped_refs=None):
+    """What the format flags make of each output file: {"aligned", "error_profile", "unaligned"} -> OutputFile.  gzip and
+    bam: the reads files are BGZF members that end with the end-of-file block, and bam's start with the BAM header (with
+    mapped_refs' @SQ lines for the aligned reads).  gzip_error_profile: the error profile is BGZF members too, the first one
+    its header line."""
+    ext = ".bam" if bam else (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
+    packed = gzip or bam
+    trailer = BGZF_EOF if packed else b""
+    header = bam_header() if bam else b""
+    aligned_header = bam_header(mapped_refs) if bam and mapped_refs is not None else header
+    err = ".gz" if gzip_error_profile else ""
+    err_header = bgzf_member(ERR_HEADER) if gzip_error_profile else ERR_HEADER
+    return {"aligned": OutputFile("_aligned_reads" + ext, "_aligned_reads%d" + ext, aligned_header, trailer, packed),
+            "error_profile": OutputFile("_aligned_error_profile" + err, "_error_profile%d" + err, err_header,
+                                        BGZF_EOF if gzip_error_profile else b"", gzip_error_profile),
+            "unaligned": OutputFile("_unaligned_reads" + ext, "_unaligned_reads%d" + ext, header, trailer, packed)}
 
 
 def _log(msg):
@@ -382,26 +406,21 @@ def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min
                   # the reference's 2-D KDE sample has one row per read of a WORKER (:1072): -t sets its size as it does there
                   kde2d_sample=max(1, (hi_a - lo_a) // max(1, num_threads)),
                   trx_records=prof.n_trx if (trx and prof.ir is not None) else 0)
-    ext = ".bam" if bam else (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
-    suffix = "" if world == 1 else str(rank)
     want_err = error_profile and not per
     gz_err = (gzip or bam) and gzip_error_profile and want_err
+    files = output_files(fastq, gzip, gz_err, bam, mapped_refs)
     pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err and not gz_err, compress_profile=gz_err, bam=bam,
                          mapped_bam=mapped_refs is not None)
     totals = {"reads": 0, "bases": 0, "bytes": 0}
     try:
-        _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                         gzip, gz_err, bam, mapped_refs)
+        _simulation_body(prof, pipe, out, per, fastq, meta, trx, files, want_err, world, rank, batch_reads, fmt_threads, totals)
     finally:
         pipe.close()         # the cloned contexts own device batch buffers and pinned staging
     return totals            # what this rank simulated and wrote (the reference returns nothing)
 
 
-def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, want_err, world, rank, batch_reads, fmt_threads, totals,
-                     gzip=False, gz_err=False, bam=False, mapped_refs=None):
-    packed = gzip or bam            # the records are compressed on the device: the batches arrive as BGZF members
-    reads_header = bam_header() if bam and world == 1 else b""
-    aligned_header = bam_header(mapped_refs) if mapped_refs is not None and world == 1 else reads_header
+def _simulation_body(prof, pipe, out, per, fastq, meta, trx, files, want_err, world, rank, batch_reads, fmt_threads, totals):
+    packed = files["aligned"].members       # the records are compressed on the device: the batches arrive as BGZF members
 
     def jobs(kind, lo, hi):
         return [(kind, start, min(batch_reads, hi - start)) for start in range(lo, hi, batch_reads)]
@@ -419,31 +438,24 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             return
         put_members(f, b.gz)
 
-    def end_bgzf(f):
-        if world == 1:
-            f.pos += os.pwrite(f.fd, BGZF_EOF, f.pos)
-
-    def end_reads(f):
-        if packed:
-            end_bgzf(f)
-
     class _Out:
         """An output file written at explicit offsets: the library's formatter threads pwrite() into it."""
 
-        def __init__(self, path, header=b""):
-            self.fd = os.open(path, os.O_WRONLY | os.O_CREAT | os.O_TRUNC, 0o644)
-            self.pos = 0
-            if header:
-                self.pos = os.pwrite(self.fd, header, 0)
+        def __init__(self, f):
+            self.fd = os.open(out + (f.name if world == 1 else f.rank_name % rank), os.O_WRONLY | os.O_CREAT | os.O_TRUNC, 0o644)
+            self.pos = os.pwrite(self.fd, f.header, 0) if world == 1 else 0
+            self.trailer = f.trailer if world == 1 else b""        # under torchrun merge_rank_files writes both
+
+        def end(self):
+            self.pos += os.pwrite(self.fd, self.trailer, self.pos)
 
         def close(self):
             os.close(self.fd)
 
     _log("Start simulation of aligned reads")
     lo, hi = _shard(prof.number_aligned, rank, world)
-    f_reads = _Out(out + "_aligned_reads" + suffix + ext, aligned_header)
-    f_err = _Out(out + ("_aligned_error_profile" if world == 1 else "_error_profile" + suffix) + (".gz" if gz_err else ""),
-                 b"" if world > 1 else bgzf_member(ERR_HEADER) if gz_err else ERR_HEADER)
+    f_reads = _Out(files["aligned"])
+    f_err = _Out(files["error_profile"])
     try:
         def aligned_names(b, job):
             return name_table(b, prof.ref.names, job[1], perfect=per, metagenome=meta, transcriptome=trx)
@@ -453,7 +465,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
             put_reads(f_reads, b, names)
             totals["reads"] += int(info.n_reads)
             totals["bases"] += int(info.total_bases)
-            if gz_err:
+            if files["error_profile"].members:
                 put_members(f_err, b.gz_err)
             elif want_err:
                 f_err.pos += write_error_profile(f_err.fd, f_err.pos, b, names, prof.ref, seed=prof.seed, n_threads=fmt_threads)
@@ -469,9 +481,8 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
         pipe.compress = aligned_names if packed else None
         pipe.run(jobs(L.NS_KIND_ALIGNED, lo, hi), sink_aligned, static_assign=meta,
                  after_simulate=retain_introns if (trx and prof.ir is not None and not per) else None)
-        end_reads(f_reads)
-        if gz_err:
-            end_bgzf(f_err)
+        f_reads.end()
+        f_err.end()
     finally:
         totals["bytes"] += f_reads.pos + f_err.pos
         f_reads.close()
@@ -480,7 +491,7 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
         _log("Start simulation of random reads")
         lo, hi = _shard(prof.number_unaligned, rank, world)
         pipe.want_ops = pipe.compress_profile = False      # unaligned reads are not logged (:1482-1549)
-        f_un = _Out(out + "_unaligned_reads" + suffix + ext, reads_header)
+        f_un = _Out(files["unaligned"])
         try:
             def unaligned_names(b, job):
                 # the reference's read index keeps counting after the aligned reads (shared total_simulated, :1574)
@@ -493,34 +504,22 @@ def _simulation_body(prof, pipe, mode, out, per, fastq, meta, trx, ext, suffix, 
 
             pipe.compress = unaligned_names if packed else None
             pipe.run(jobs(L.NS_KIND_UNALIGNED, lo, hi), sink_unaligned, static_assign=meta)
-            end_reads(f_un)
+            f_un.end()
         finally:
             totals["bytes"] += f_un.pos
             f_un.close()
 
 
 def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=False, bam=False, mapped_refs=None):
-    """Rank 0: concatenate per-rank sub-files in rank order and delete them (:1626-1639, :1667-1672).  gzip: the reads
-    files are BGZF members without an end-of-file block; the merged file gets it once, at its end.  bam: so are the
-    ``.bam`` reads files, and the merged ones start with the BAM header's members (with mapped_refs' @SQ lines for the
-    aligned reads).  gzip_error_profile: so are the error-profile files (``_error_profile{r}.gz``); the merged one starts
-    with the header line's member."""
-    ext = ".bam" if bam else (".fastq" if fastq else ".fasta") + (".gz" if gzip else "")
-    header = bam_header() if bam else b""
-    trailer = BGZF_EOF if gzip or bam else b""
-    aligned_header = bam_header(mapped_refs) if bam and mapped_refs is not None else header
-    jobs = [("_aligned_reads%d" + ext, "_aligned_reads" + ext, aligned_header, trailer)]
-    if gzip_error_profile:
-        jobs.append(("_error_profile%d.gz", "_aligned_error_profile.gz", bgzf_member(ERR_HEADER), BGZF_EOF))
-    else:
-        jobs.append(("_error_profile%d", "_aligned_error_profile", ERR_HEADER, b""))
-    if not per:
-        jobs.append(("_unaligned_reads%d" + ext, "_unaligned_reads" + ext, header, trailer))
-    for pat, dst, header, end in jobs:
-        with open(out + dst, "wb") as o:
-            o.write(header)
+    """Rank 0: concatenate per-rank sub-files in rank order and delete them (:1626-1639, :1667-1672), between each file's
+    header and trailer (output_files)."""
+    for key, f in output_files(fastq, gzip, gzip_error_profile, bam, mapped_refs).items():
+        if key == "unaligned" and per:
+            continue
+        with open(out + f.name, "wb") as o:
+            o.write(f.header)
             for r in range(world):
-                p = out + (pat % r)
+                p = out + (f.rank_name % r)
                 with open(p, "rb") as i:
                     while True:
                         blk = i.read(1 << 24)
@@ -528,7 +527,7 @@ def merge_rank_files(out, fastq, per, world, gzip=False, gzip_error_profile=Fals
                             break
                         o.write(blk)
                 os.remove(p)
-            o.write(end)
+            o.write(f.trailer)
 
 
 GZIP_HELP = ('Write the reads as BGZF-compressed <out>_aligned_reads.fast{a,q}.gz and <out>_unaligned_reads.fast{a,q}.gz, '
