@@ -143,6 +143,13 @@ __device__ __forceinline__ double u01_double(uint64_t r) {    // [0, 1)
     return (double)(r >> 11) * (1.0 / 9007199254740992.0);
 }
 
+// Box-Muller N(0, 1) from two words, cosine branch only: radius sqrt(-2 ln u1) with u1 = ((r1 >> 8) + 1) / 2^24 in (0, 1]
+// (|z| <= sqrt(48 ln 2) = 5.77), angle 2 pi u2 with u2 = (r2 >> 8) / 2^24.  The two factors are separate functions so that
+// tests/test_device_draws.py can hold each of them, over all 2^24 inputs, against float64.
+__device__ __forceinline__ float nf32_radius(uint32_t r1) { return sqrtf(-2.0f * logf(u01_open_low(r1))); }
+__device__ __forceinline__ float nf32_cos(uint32_t r2) { return cospif(2.0f * ((float)(r2 >> 8) * (1.0f / 16777216.0f))); }
+__device__ __forceinline__ float normal_f32(uint32_t r1, uint32_t r2) { return nf32_radius(r1) * nf32_cos(r2); }
+
 // Walker alias draw from table t with one 32-bit word.
 __device__ __forceinline__ uint32_t alias_draw(const DevModel& m, uint32_t t, uint32_t r) {
     uint32_t n = m.tab_n[t];
@@ -168,17 +175,13 @@ __device__ __forceinline__ double kde_draw(const DevKde& k, Rng& rng) {
     uint64_t r0 = rng.next64();
     uint32_t r1 = rng.next(), r2 = rng.next();
     uint32_t i = (uint32_t)__umul64hi(r0, (uint64_t)k.n);
-    float u1 = u01_open_low(r1);
-    float u2 = (float)(r2 >> 8) * (1.0f / 16777216.0f);
-    float z = sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
-    return (double)__ldg(&k.data[i]) + (double)k.bw * (double)z;
+    return (double)__ldg(&k.data[i]) + (double)k.bw * (double)normal_f32(r1, r2);
 }
 
 // numpy.random.lognormal(mean, sigma) = exp(mean + sigma * N(0,1))
 __device__ __forceinline__ double lognormal_draw(double mean, double sigma, Rng& rng) {
     uint32_t r1 = rng.next(), r2 = rng.next();
-    float z = sqrtf(-2.0f * logf(u01_open_low(r1))) * cospif(2.0f * ((float)(r2 >> 8) * (1.0f / 16777216.0f)));
-    return exp(mean + sigma * (double)z);
+    return exp(mean + sigma * (double)normal_f32(r1, r2));
 }
 
 // base <-> index helpers: A C G T -> 0 1 3 2 via (c >> 1) & 3 ; complement = idx ^ 2
@@ -190,20 +193,24 @@ __device__ __forceinline__ uint32_t emit_char(uint32_t i, uint32_t uracil) {
 }
 __device__ __forceinline__ bool is_acgt(uint32_t c) { return c == 'A' || c == 'C' || c == 'G' || c == 'T'; }
 // bit i of 0x80045 is set for i = 'A'-'A', 'C'-'A', 'G'-'A', 'T'-'A'
-__device__ __forceinline__ bool acgt_fast(uint32_t c) {
+__host__ __device__ __forceinline__ bool acgt_fast(uint32_t c) {
     uint32_t d = c - 'A';
     return d < 26u && ((0x80045u >> d) & 1u);
 }
 // Base qualities: per quality state a Walker alias table with 2^QLUT_BITS slots over the state's 24-bit pmf (built on the
-// host, nanosim_api.cu:build_qlut; sampled in emit_kernel.cuh:qual_pick).
+// host, qual_table.h:build_qlut; sampled in emit_kernel.cuh:qual_pick).
 #define QLUT_BITS 11
 #define QLUT_SIZE (1 << QLUT_BITS)
 
 __device__ __forceinline__ uint32_t op_len(uint32_t op) { return (op >> 28) == NS_OP_LIT ? (op & 0x00ffffffu) : (op & 0x0fffffffu); }
 
+// A uniform pick among three from 16 uniform bits: 21846 : 21845 : 21845 of the 2^16 values give 0 : 1 : 2 (relative
+// bias 2^-15).
+__host__ __device__ __forceinline__ uint32_t three_way16(uint32_t h) { return ((h & 0xffffu) * 3u) >> 16; }
+
 // IUPAC resolution of case_convert (:744-746): members in the reference's list order, picked uniformly.
 // r8 is a uniform byte; t3 a uniform value in {0,1,2}.
-__device__ __forceinline__ uint32_t resolve_iupac(uint32_t c, uint32_t r8, uint32_t t3) {
+__host__ __device__ __forceinline__ uint32_t resolve_iupac(uint32_t c, uint32_t r8, uint32_t t3) {
     uint32_t n, set;   // set: up to 4 members packed one byte each
     switch (c) {
     case 'Y': n = 2; set = 'C' | ('T' << 8); break;
@@ -223,36 +230,42 @@ __device__ __forceinline__ uint32_t resolve_iupac(uint32_t c, uint32_t r8, uint3
     uint32_t k = (n == 3) ? t3 : ((r8 >> 4) & (n - 1));
     return (set >> (8 * k)) & 0xffu;
 }
+// An upper-case reference byte resolved with the 16 bits h of its base: two- and four-member codes take bits [5:4] of h
+// (exactly uniform), three-member codes three_way16(h).
+__host__ __device__ __forceinline__ uint32_t resolve_iupac16(uint32_t c, uint32_t h) {
+    return resolve_iupac(c, h & 0xffu, three_way16(h));
+}
 
 // case_convert of ONE reference base of one read, as a pure function of (read, piece, forward offset in the segment):
 // every kernel that looks at the same base of the same read (emit, homopolymer pass) sees the same resolution.
-__device__ __forceinline__ uint32_t converted_ref_base(uint32_t c, uint64_t seed, uint64_t rid, uint32_t piece_in_read,
-                                                       uint32_t fwd_off) {
+__host__ __device__ __forceinline__ uint32_t converted_ref_base(uint32_t c, uint64_t seed, uint64_t rid, uint32_t piece_in_read,
+                                                                uint32_t fwd_off) {
     if (c - 'a' < 26u) c -= 32;
     if (acgt_fast(c)) return c;
     const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
     uint4 w = philox4x32_7(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_IUPAC, 0, piece_in_read), fwd_off >> 3), key);
     uint32_t wd = (fwd_off & 4u) ? ((fwd_off & 2u) ? w.w : w.z) : ((fwd_off & 2u) ? w.y : w.x);
     uint32_t h = (fwd_off & 1u) ? (wd >> 16) : (wd & 0xffffu);
-    uint32_t r8 = h & 0xffu, r3 = h >> 8;
-    return resolve_iupac(c, r8, r3 == 255u ? 0u : r3 % 3u);
+    return resolve_iupac16(c, h);
 }
 
 // Bases of a MIS / INS event that the homopolymer pass rewrites (hp_kernel.cuh, ST_BASE); the error-profile formatter
-// (host_io.cu) gives those events the same bases.  Base t of the event comes from byte t % 16 of Philox-7 block
-// (event index in the piece's event script << 8) + (t >> 4) on stream ST_EMIT_B of the piece (key: the seed).
+// (host_io.cu) gives those events the same bases.  Base t of the event comes from the 16-bit half t % 8 of Philox-7 block
+// (event index in the piece's event script << 9) + (t >> 3) on stream ST_EMIT_B of the piece (key: the seed): an event has
+// 4096 bases before its blocks reach the next event's.  Callers draw a new block whenever t % EVENT_BASES_PER_BLOCK == 0.
+#define EVENT_BASES_PER_BLOCK 8u
 __host__ __device__ __forceinline__ uint4 event_base_block(uint2 key, uint64_t rid, uint32_t piece_in_read, uint32_t event,
                                                            uint32_t t) {
-    return philox4x32_7(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_EMIT_B, 0, piece_in_read), (event << 8) + (t >> 4)), key);
+    return philox4x32_7(make_uint4((uint32_t)rid, (uint32_t)(rid >> 32), stream_word(ST_EMIT_B, 0, piece_in_read),
+                                   (event << 9) + t / EVENT_BASES_PER_BLOCK), key);
 }
-__host__ __device__ __forceinline__ uint32_t event_byte(const uint4& blk, uint32_t t) {
-    const uint32_t wd = (t & 8u) ? ((t & 4u) ? blk.w : blk.z) : ((t & 4u) ? blk.y : blk.x);
-    return (wd >> (8u * (t & 3u))) & 0xffu;
+__host__ __device__ __forceinline__ uint32_t event_draw(const uint4& blk, uint32_t t) {
+    const uint32_t wd = (t & 4u) ? ((t & 2u) ? blk.w : blk.z) : ((t & 2u) ? blk.y : blk.x);
+    return (t & 1u) ? (wd >> 16) : (wd & 0xffffu);
 }
-// base index (A 0, C 1, T 2, G 3) from that byte: an inserted base is r8 & 3, a substituted one differs from the original
-// base index `orig`
-__host__ __device__ __forceinline__ uint32_t event_base(uint32_t r8, bool mis, uint32_t orig) {
-    if (!mis) return r8 & 3u;
-    const uint32_t rr = r8 == 255u ? 0u : r8;
-    return ((orig & 3u) + 1u + rr % 3u) & 3u;
+// base index (A 0, C 1, T 2, G 3) from that draw h: an inserted base is h & 3 (exactly uniform), a substituted one is one
+// of the three base indices other than `orig`, picked by three_way16(h)
+__host__ __device__ __forceinline__ uint32_t event_base(uint32_t h, bool mis, uint32_t orig) {
+    if (!mis) return h & 3u;
+    return ((orig & 3u) + 1u + three_way16(h)) & 3u;
 }

@@ -149,7 +149,7 @@ __device__ __forceinline__ void draw_chunk_qual(ChunkQual<FASTQ>& r, uint32_t id
 // a base index to replace it by one of the three other bases (random.choice of the remaining bases,
 // simulator.py:1968-1973).  Field i is the first non-zero one among the seven 2-bit draws X1[i] .. X7[i] -- uniform over
 // {1,2,3} -- and 1 if all seven are zero (probability 4^-7: relative bias 1.2e-4).
-__device__ __forceinline__ uint32_t sub_offsets(const uint32_t (&XA)[3], const uint32_t (&XB)[4]) {
+__host__ __device__ __forceinline__ uint32_t sub_offsets(const uint32_t (&XA)[3], const uint32_t (&XB)[4]) {
     uint32_t sub = XA[0];
 #pragma unroll
     for (int j = 1; j < 7; ++j) {
@@ -159,13 +159,13 @@ __device__ __forceinline__ uint32_t sub_offsets(const uint32_t (&XA)[3], const u
     return sub | (~(sub | (sub >> 1)) & 0x55555555u);
 }
 // per-field (a + b) mod 4 of two words of 16 2-bit fields
-__device__ __forceinline__ uint32_t add_fields_mod4(uint32_t a, uint32_t b) {
+__host__ __device__ __forceinline__ uint32_t add_fields_mod4(uint32_t a, uint32_t b) {
     return a ^ b ^ ((a & b & 0x55555555u) << 1);
 }
 
 // Base quality from an alias-table entry: [31:19] 13-bit acceptance threshold, [15:8] alias character, [7:0] primary
-// character (nanosim_api.cu:build_qlut).  The draw w carries the slot in bits [18:8] and the threshold draw in [31:19].
-__device__ __forceinline__ uint32_t qual_pick(uint32_t e, uint32_t w) {
+// character (qual_table.h:build_qlut).  The draw w carries the slot in bits [18:8] and the threshold draw in [31:19].
+__host__ __device__ __forceinline__ uint32_t qual_pick(uint32_t e, uint32_t w) {
     return ((w | 0x7ffffu) < e) ? e : (e >> 8);          // the character is the low byte of the result
 }
 

@@ -181,10 +181,10 @@ __device__ void ep_write_row(const EpArgs& a, const NsReadMeta& r, uint32_t i, c
         uint4 blk;
         const uint64_t rid = a.first_id + i;
         for (uint32_t t = 0; t < e.len; ++t) {
-            if ((t & 15u) == 0) blk = event_base_block(a.key, rid, e.k, e.j, t);
+            if (t % EVENT_BASES_PER_BLOCK == 0) blk = event_base_block(a.key, rid, e.k, e.j, t);
             const uint8_t rc = e.ty == NS_OP_MIS ? ref_char(t) : (uint8_t)'-';
             const uint32_t orig = rc == 'C' ? 1u : (rc == 'T' ? 2u : (rc == 'G' ? 3u : 0u));
-            p[t] = (uint8_t)"ACTG"[event_base(event_byte(blk, t), e.ty == NS_OP_MIS, orig)];
+            p[t] = (uint8_t)"ACTG"[event_base(event_draw(blk, t), e.ty == NS_OP_MIS, orig)];
         }
     } else {
         const uint8_t* rs = a.seq + r.seq_off;

@@ -18,7 +18,7 @@
 #include <vector>
 
 #include "nanosim_b200.h"
-#include "device_common.cuh"      // event_base_block / event_byte / event_base: bases of events the homopolymer pass rewrote
+#include "device_common.cuh"      // event_base_block / event_draw / event_base: bases of events the homopolymer pass rewrote
 #include "host_io.h"
 
 namespace {
@@ -352,10 +352,10 @@ int64_t format_error_profile_impl(const uint8_t* seq, const NsReadMeta* reads, c
                 } else if (w.rewritten) {
                     uint4 blk;
                     for (uint32_t t = 0; t < w.len; ++t) {
-                        if ((t & 15u) == 0) blk = event_base_block(key, rid, w.piece, w.index, t);
+                        if (t % EVENT_BASES_PER_BLOCK == 0) blk = event_base_block(key, rid, w.piece, w.index, t);
                         const char rc = refp[t];
                         const uint32_t orig = rc == 'C' ? 1u : (rc == 'T' ? 2u : (rc == 'G' ? 3u : 0u));
-                        p[t] = "ACTG"[event_base(event_byte(blk, t), w.type == NS_OP_MIS, orig)];
+                        p[t] = "ACTG"[event_base(event_draw(blk, t), w.type == NS_OP_MIS, orig)];
                     }
                 } else {
                     for (uint32_t t = 0; t < w.len; ++t) {

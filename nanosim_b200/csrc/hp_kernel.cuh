@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
             const double L = (double)run_len;
             const double mu = p[0] + p[1] * L + p[2] * fmax(L - p[3], 0.0);
             const double sigma = p[4] + p[5] * L;
-            const float z = sqrtf(-2.0f * logf(u01_open_low(r.x))) * cospif(2.0f * ((float)(r.y >> 8) * (1.0f / 16777216.0f)));
+            const float z = normal_f32(r.x, r.y);
             double x = mu + sigma * (double)z;
             if (x < 0.0) x = 0.0;
             const uint32_t nn = (uint32_t)rint(x);
@@ -377,13 +377,13 @@ __global__ void __launch_bounds__(128, HP_MIN_BLOCKS) hp_kernel(const __grid_con
             } else if (bsrc == SRC_EXACT) {
                 b = w.base_at(rpos + t);
             } else {
-                if ((t & 15u) == 0) rblk = event_base_block(key, rid, w.piece_in_read, kk, t);
-                const uint32_t r8 = event_byte(rblk, t);
+                if (t % EVENT_BASES_PER_BLOCK == 0) rblk = event_base_block(key, rid, w.piece_in_read, kk, t);
+                const uint32_t h = event_draw(rblk, t);
                 if (bsrc == SRC_MIS) {
-                    b = event_base(r8, true, w.packed ? (w.bases16(rpos + t) & 3u) : w.base_at(rpos + t));
+                    b = event_base(h, true, w.packed ? (w.bases16(rpos + t) & 3u) : w.base_at(rpos + t));
                     bkind = 1;
                 } else {
-                    b = event_base(r8, false, 0u);
+                    b = event_base(h, false, 0u);
                     bkind = 2;
                 }
             }

@@ -293,8 +293,7 @@ __device__ __forceinline__ uint32_t nearest_aligned_length(const DevModel& m, ui
     uint32_t r = (uint32_t)__umul64hi(rng.next64(), (uint64_t)(cnt > 0 ? cnt : 1));
     const uint32_t row = cnt == 0 ? (a0 < M ? a0 : M - 1) : (r < a1 - a0 ? a0 + r : b0 + (r - (a1 - a0)));
     const uint32_t r1 = rng.next(), r2 = rng.next();
-    const float z = sqrtf(-2.0f * logf(u01_open_low(r1))) * cospif(2.0f * ((float)(r2 >> 8) * (1.0f / 16777216.0f)));
-    const double y = (double)__ldg(&m.kde2d_y[row]) + (double)m.kde2d_bw * (double)z;
+    const double y = (double)__ldg(&m.kde2d_y[row]) + (double)m.kde2d_bw * (double)normal_f32(r1, r2);
     return y > 0.0 ? (uint32_t)y : 0u;
 }
 

@@ -232,19 +232,19 @@ def _philox4x32(ctr, key, rounds):
 
 
 def event_bases_hp(seed, rid, piece_in_read, k, n, is_mis, orig_idx=None):
-    """Bases the homopolymer pass assigned to error event k of a segment (csrc/hp_kernel.cuh): one byte of Philox-7
-    block (k<<8)+(t>>4) per base.  Returns ACGT index array in the device's order A C T G = 0 1 2 3."""
+    """Bases the homopolymer pass assigned to error event k of a segment (csrc/hp_kernel.cuh): 16 bits h of Philox-7
+    block (k<<9)+(t>>3) per base (csrc/device_common.cuh:event_base).  Returns ACGT index array in the device's order
+    A C T G = 0 1 2 3."""
     t = np.arange(n, dtype=np.uint64)
     stream = (6 << 28) | (piece_in_read & 0x07ffffff)            # ST_EMIT_B, kind 0
     ctr = np.stack([np.full(n, rid & 0xFFFFFFFF, dtype=np.uint64), np.full(n, (rid >> 32) & 0xFFFFFFFF, dtype=np.uint64),
-                    np.full(n, stream, dtype=np.uint64), (np.uint64(k) << np.uint64(8)) + (t >> np.uint64(4))], axis=1)
+                    np.full(n, stream, dtype=np.uint64), (np.uint64(k) << np.uint64(9)) + (t >> np.uint64(3))], axis=1)
     blk = _philox4x32(ctr, (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF), 7)
-    word = blk[np.arange(n), ((t >> np.uint64(2)) & np.uint64(3)).astype(np.int64)]
-    r8 = ((word >> (np.uint64(8) * (t & np.uint64(3)))) & np.uint64(0xFF)).astype(np.int64)
+    word = blk[np.arange(n), ((t >> np.uint64(1)) & np.uint64(3)).astype(np.int64)]
+    h = ((word >> (np.uint64(16) * (t & np.uint64(1)))) & np.uint64(0xFFFF)).astype(np.int64)
     if not is_mis:
-        return r8 & 3
-    rr = np.where(r8 == 255, 0, r8)
-    return (orig_idx + 1 + rr % 3) & 3
+        return h & 3
+    return (orig_idx + 1 + ((h * 3) >> 16)) & 3
 
 
 _IDX_BASE = np.frombuffer(b"ACTG", dtype=np.uint8)
