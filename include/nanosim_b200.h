@@ -298,6 +298,27 @@ typedef struct {
 } NsSplice;
 int ns_set_splice(NsContext* ctx, const NsSplice* splice);
 
+/* --aln_tags: NM and SA on every mapped record of ns_compress_bam_mapped (DESIGN.md §3 "NM and SA tags").  ref_names /
+ * ref_name_off: the mapped header's @SQ SN names in refID order, name k being bytes [ref_name_off[k], ref_name_off[k+1])
+ * (no NUL): the resident records, the haploid records with a lift, the genome records with a splice map.  With a lift
+ * (ns_set_lift first): n_var its variant count and ref_paired the haploid bytes [var_pos, var_pos + min(alt_len,
+ * var_ref_len)) of every kind-0 variant back to back in NsVariants order (the REF bases an ALT's first bases are aligned
+ * to); without one n_var and ref_paired_bytes are 0.  Host pointers; the tables are kept with the tables the context and
+ * its clones share.  NS_EINVAL for an empty name, and (naming the table) when n_var or ref_paired_bytes is not the lift's;
+ * ns_compress_bam_mapped fails with NS_EINVAL when the names are not one per refID of its records.  peak_bytes, when
+ * given, receives the device bytes the tables keep.  Call after ns_set_lift / ns_set_splice and before ns_clone; NS_ESTATE
+ * on a clone.  A later ns_set_reference, ns_apply_variants, ns_set_lift or ns_set_splice drops them. */
+typedef struct {
+    uint32_t n_ref;
+    const char* ref_names;
+    const uint64_t* ref_name_off;    /* n_ref + 1 */
+    uint64_t n_var;
+    const uint8_t* ref_paired;
+    uint64_t ref_paired_bytes;
+    uint64_t* peak_bytes;            /* out, may be NULL */
+} NsAlnTags;
+int ns_set_aln_tags(NsContext* ctx, const NsAlnTags* tags);
+
 int ns_configure(NsContext* ctx, const NsRunConfig* cfg);
 /* metagenome: dict_abun / dict_abun_inflated of the current sample (main() :2497-2514), one value per species in
  * genome-list order; resets the running per-species base counts that assign_species (:758-811) keeps per worker. */
@@ -446,8 +467,10 @@ int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off,
  * In transcriptome mode the records are spliced onto the genome records of the context's splice map (ns_set_splice):
  * refID is the genome record, an intron the read skips is an N, a minus-strand transcript's read is a record on the other
  * strand, and every mapped record has XS:A:<+ or -> (the transcript's strand) as its first aux field (DESIGN.md §3
- * "Spliced mapped BAM").  NS_EINVAL when the last batch is unaligned reads, the context is in transcriptome mode without
- * a splice map (or with one whose records are not the run's), or a lift meets a circular configuration. */
+ * "Spliced mapped BAM").  When the context has ns_set_aln_tags' tables, every mapped record also has NM:I and, when its
+ * read has more than one record, SA:Z, after HP/XS and before CG (DESIGN.md §3 "NM and SA tags"); nothing else changes.
+ * NS_EINVAL when the last batch is unaligned reads, the context is in transcriptome mode without a splice map (or with one
+ * whose records are not the run's), a lift meets a circular configuration, or the tags' names are not one per refID. */
 int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
 /* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' (or ns_compress_bam's)
  * *nbytes. */

@@ -25,7 +25,7 @@ NS_STATS_WORDS = NS_STATS_COMP_OFF + 4
 EXPORTS = ["ns_create", "ns_destroy", "ns_last_error", "ns_clone", "ns_set_abundance", "ns_set_expression", "ns_set_reference", "ns_set_model", "ns_configure",
            "ns_simulate", "ns_fetch", "ns_reemit", "ns_batch_info", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases",
            "ns_compress_records", "ns_fetch_compressed", "ns_compress_error_profile", "ns_fetch_compressed_error_profile", "ns_compress_bam", "ns_apply_variants",
-           "ns_compress_bam_mapped", "ns_set_lift", "ns_set_splice"]
+           "ns_compress_bam_mapped", "ns_set_lift", "ns_set_splice", "ns_set_aln_tags"]
 
 
 class NsReference(C.Structure):
@@ -46,6 +46,11 @@ class NsSplice(C.Structure):
     _fields_ = [("n_trx", C.c_uint32), ("exon_off", C.c_void_p), ("exon_chrom", C.c_void_p), ("exon_start", C.c_void_p),
                 ("exon_len", C.c_void_p), ("minus", C.c_void_p), ("n_genome", C.c_uint32), ("genome_len", C.c_void_p),
                 ("genome_first", C.c_uint32), ("peak_bytes", C.POINTER(C.c_uint64))]
+
+
+class NsAlnTags(C.Structure):
+    _fields_ = [("n_ref", C.c_uint32), ("ref_names", C.c_void_p), ("ref_name_off", C.c_void_p), ("n_var", C.c_uint64),
+                ("ref_paired", C.c_void_p), ("ref_paired_bytes", C.c_uint64), ("peak_bytes", C.POINTER(C.c_uint64))]
 
 
 class NsKde(C.Structure):
@@ -150,6 +155,8 @@ def lib():
     L.ns_set_lift.restype = C.c_int
     L.ns_set_splice.argtypes = [P, C.POINTER(NsSplice)]
     L.ns_set_splice.restype = C.c_int
+    L.ns_set_aln_tags.argtypes = [P, C.POINTER(NsAlnTags)]
+    L.ns_set_aln_tags.restype = C.c_int
     L.ns_set_model.argtypes = [P, C.POINTER(NsModel)]
     L.ns_set_model.restype = C.c_int
     L.ns_set_abundance.argtypes = [P, P, P, C.c_uint32]

@@ -11,6 +11,9 @@
 // ALN_SPLICE (ns_set_splice, DESIGN §3 "Spliced mapped BAM"): transcriptome reads, the walk composed with the transcript's
 // exons (or, for a read that retains an intron, with its chain of genome pieces), so the records are against the genome
 // with an N for every intron the read skips.
+// NM and SA (ns_set_aln_tags, DESIGN §3 "NM and SA tags"): aln_write_tags_kernel is the same write walk counting every
+// record's NM on the way (AlnWrite<kMode, true>::bases); aln_aux_size_kernel and aln_aux_write_kernel then lay out and
+// fill each record's aux fields (HP/XS, NM, SA) for bgzf_deflate_kernel<BgzfRecords<BgzfTaggedLayout>>.
 #pragma once
 
 #include <type_traits>
@@ -25,6 +28,9 @@ enum : uint32_t { CIG_M = 0, CIG_I = 1, CIG_D = 2, CIG_N = 3, CIG_S = 4, CIG_H =
 constexpr uint32_t ALN_CUT = 15;                    // the origin of a circular record: one alignment ends, the next starts
 constexpr uint32_t BAM_MAX_CIGAR = 65535;           // n_cigar_op is 16 bits; more ops go into a CG:B,I field
 constexpr uint32_t BAM_MAPQ = 60;
+// where an M of aln_script comes from (the third argument of its fn): a COPY op, a MIS op, or the M part of a LIT group
+// followed by a DEL; every other kind passes ALN_SRC_COPY
+enum : uint32_t { ALN_SRC_COPY = 0, ALN_SRC_MIS = 1, ALN_SRC_LIT = 2 };
 
 // one mapped record (or, flag 4, the unmapped record ns_compress_bam writes)
 struct BamAln {
@@ -152,6 +158,45 @@ struct BgzfMappedLayout : BgzfMappedLayoutOf<ALN_PLAIN> {};
 struct BgzfLiftedLayout : BgzfMappedLayoutOf<ALN_LIFT> {};
 struct BgzfSplicedLayout : BgzfMappedLayoutOf<ALN_SPLICE> {};
 
+// With NM and SA (every walk): a mapped record's aux fields up to CG (HP/XS, NM, SA) are aux_len bytes that
+// aln_aux_write_kernel left at aux; CG:B,I follows as in BgzfMappedLayoutOf
+struct BgzfTaggedRec {
+    BgzfMappedRec m;
+    const uint8_t* aux;
+    uint32_t aux_len;
+};
+struct BgzfTaggedTable {
+    BgzfMappedTable m;
+    const uint8_t* aux;
+    const uint64_t* aux_off;        // exclusive prefix sum of the records' aux bytes
+    uint64_t aux_total;
+    uint32_t n_recs;
+    __device__ __forceinline__ BgzfTaggedRec operator[](uint32_t r) const {
+        const uint64_t o = aux_off[r], e = r + 1 < n_recs ? aux_off[r + 1] : aux_total;
+        return BgzfTaggedRec{m[r], aux + o, (uint32_t)(e - o)};
+    }
+};
+struct BgzfTaggedLayout {
+    using Table = BgzfTaggedTable;
+    static __device__ __forceinline__ uint8_t byte(uint64_t q, const BgzfTaggedRec& rc) {
+        const BamAln& a = rc.m.a;
+        if (a.flag & 4) return BgzfBamLayout::byte(q, rc.m.rd);
+        const uint32_t nl = rc.m.rd.nl;
+        if (q < 4) return (uint8_t)(((uint32_t)bam_mapped_size(nl, a, rc.aux_len) - 4) >> (8 * (uint32_t)q));     // block_size
+        const bool cg = a.n_cig > BAM_MAX_CIGAR;
+        const uint64_t core = bam_mapped_size(nl, a, 0) - (cg ? 8 + 4ull * a.n_cig : 0);        // up to the qualities
+        // the fixed fields (flag without the HP/strand bits), name, CIGAR, bases and qualities
+        if (q < core) return BgzfMappedLayoutOf<ALN_LIFT>::byte(q, rc.m);
+        q -= core;
+        if (q < rc.aux_len) return rc.aux[q];
+        q -= rc.aux_len;
+        if (q < 4) return (uint8_t)"CGBI"[q];
+        const uint32_t k = (uint32_t)(q - 4) >> 2;
+        const uint32_t w = k == 0 ? a.n_cig : rc.m.cig[k - 1];
+        return (uint8_t)(w >> (8 * ((uint32_t)q & 3)));
+    }
+};
+
 // ns_set_lift's table in HBM: haplotype record h's segments are seg[first[h] .. first[h + 1]) in haplotype order, their
 // kinds kind[...]; hap_chrom[h] its source record and hap_number[h] its HP value
 struct AlnLift {
@@ -186,22 +231,22 @@ __device__ __forceinline__ void lift_advance(LiftWalk& w, Fn& fn) {
             w.d_done = true;
             w.at = g.ref0 + g.hap_len;
             w.inv = false;
-            fn(CIG_D, g.ref_len - g.hap_len);
+            fn(CIG_D, g.ref_len - g.hap_len, ALN_SRC_COPY);
         }
         if (w.s == w.s_last) return;
         ++w.s;
         w.t = 0;
         w.d_done = false;
-        if (k == HAP_LIFT_INV || w.kind[w.s] != HAP_LIFT_SEQ) fn(ALN_CUT, 0u);
+        if (k == HAP_LIFT_INV || w.kind[w.s] != HAP_LIFT_SEQ) fn(ALN_CUT, 0u, ALN_SRC_COPY);
     }
 }
 
 // A read op (M, I or D over the haplotype) composed with the lift: I stays I; M and D over 1:1 bases stay M and D; over
 // the inserted bases of a sequence ALT an M becomes I and a D vanishes
 template <class Fn>
-__device__ __forceinline__ void lift_put(LiftWalk& w, uint32_t kind, uint32_t len, Fn& fn) {
+__device__ __forceinline__ void lift_put(LiftWalk& w, uint32_t kind, uint32_t len, uint32_t src, Fn& fn) {
     if (kind == CIG_I) {
-        fn(CIG_I, len);
+        fn(CIG_I, len, src);
         return;
     }
     while (len) {
@@ -225,7 +270,7 @@ __device__ __forceinline__ void lift_put(LiftWalk& w, uint32_t kind, uint32_t le
                 out = kind == CIG_M ? CIG_I : ~0u;
             }
         }
-        if (out != ~0u) fn(out, n);
+        if (out != ~0u) fn(out, n, src);
         w.t += n;
         len -= n;
         lift_advance(w, fn);
@@ -277,9 +322,9 @@ __device__ __forceinline__ void splice_interval(const SpliceWalk& w, uint32_t k,
 // (nothing when it is 0: an exon and the retained intron beside it), or an ALN_CUT when that interval is on another record
 // or does not lie further on
 template <class Fn>
-__device__ __forceinline__ void splice_put(SpliceWalk& w, uint32_t kind, uint32_t len, Fn& fn) {
+__device__ __forceinline__ void splice_put(SpliceWalk& w, uint32_t kind, uint32_t len, uint32_t src, Fn& fn) {
     if (kind == CIG_I) {
-        fn(CIG_I, len);
+        fn(CIG_I, len, src);
         return;
     }
     while (len) {
@@ -287,8 +332,8 @@ __device__ __forceinline__ void splice_put(SpliceWalk& w, uint32_t kind, uint32_
             uint32_t c, s, l;
             splice_interval(w, w.k + 1, c, s, l);
             const int64_t gap = w.inv ? (int64_t)w.start - ((int64_t)s + l) : (int64_t)s - ((int64_t)w.start + w.len);
-            if (c != w.chrom || gap < 0) fn(ALN_CUT, 0u);
-            else if (gap) fn(CIG_N, (uint32_t)gap);
+            if (c != w.chrom || gap < 0) fn(ALN_CUT, 0u, ALN_SRC_COPY);
+            else if (gap) fn(CIG_N, (uint32_t)gap, ALN_SRC_COPY);
             ++w.k;
             w.t = 0;
             w.chrom = c;
@@ -297,7 +342,7 @@ __device__ __forceinline__ void splice_put(SpliceWalk& w, uint32_t kind, uint32_
         }
         const uint32_t n = w.t < w.len ? min(len, w.len - w.t) : len;     // past the last interval (no valid map gets here)
         w.at = w.inv ? w.start + w.len - w.t : w.start + w.t;
-        fn(kind, n);
+        fn(kind, n, src);
         w.t += n;
         len -= n;
     }
@@ -339,27 +384,27 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
                                            Fn fn) {
     uint64_t rf = 0;
     uint32_t lit = 0;
-    auto put = [&](uint32_t kind, uint32_t len) {
+    auto put = [&](uint32_t kind, uint32_t len, uint32_t src = ALN_SRC_COPY) {
         if (len == 0) return;
         if constexpr (kMode == ALN_LIFT) {
-            lift_put(w, kind, len, fn);
+            lift_put(w, kind, len, src, fn);
             return;
         } else if constexpr (kMode == ALN_SPLICE) {
-            splice_put(w, kind, len, fn);
+            splice_put(w, kind, len, src, fn);
             return;
         }
         if (kind != CIG_I) {
             while (rf <= cut && rf + len > cut) {
                 const uint32_t a = (uint32_t)(cut - rf);
-                if (a) fn(kind, a);
-                fn(ALN_CUT, 0u);
+                if (a) fn(kind, a, src);
+                fn(ALN_CUT, 0u, ALN_SRC_COPY);
                 rf += a;
                 len -= a;
                 cut += period;
             }
             rf += len;
         }
-        fn(kind, len);
+        fn(kind, len, src);
     };
     uint32_t n_src = 1;
     if constexpr (kMode == ALN_SPLICE) n_src = w.n_src;
@@ -376,13 +421,13 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
             }
             if (lit && ty == NS_OP_DEL) {
                 put(lit > ln ? CIG_I : CIG_D, lit > ln ? lit - ln : ln - lit);
-                put(CIG_M, min(lit, ln));
+                put(CIG_M, min(lit, ln), ALN_SRC_LIT);
                 lit = 0;
                 continue;
             }
             put(CIG_I, lit);
             lit = 0;
-            put(ty == NS_OP_DEL ? CIG_D : (ty == NS_OP_COPY || ty == NS_OP_MIS) ? CIG_M : CIG_I, ln);
+            put(ty == NS_OP_DEL ? CIG_D : (ty == NS_OP_COPY || ty == NS_OP_MIS) ? CIG_M : CIG_I, ln, ty == NS_OP_MIS ? ALN_SRC_MIS : ALN_SRC_COPY);
         }
     }
     put(CIG_I, lit);
@@ -401,7 +446,7 @@ __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, 
     for (uint32_t want = 0; want < n_parts; ++want) {
         uint32_t first = ~0u, last = 0, idx = 0, part = 0;
         AlnWalk<kMode> w = start;
-        aln_script<kMode>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t) {
+        aln_script<kMode>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t, uint32_t) {
             if (kind == ALN_CUT) {
                 ++part;
             } else if (kind == CIG_M && part == want) {
@@ -415,7 +460,7 @@ __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, 
         idx = 0;
         uint32_t q = q_start, rf = 0, ck = 0, cl = 0;
         w = start;
-        aln_script<kMode>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t len) {
+        aln_script<kMode>(sc, n_ops, cut, period, w, [&](uint32_t kind, uint32_t len, uint32_t src) {
             if (idx >= first && idx <= last) {
                 if (idx == first) {
                     sink.begin(q, rf);
@@ -423,6 +468,7 @@ __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, 
                     ck = kind;
                     cl = 0;
                 }
+                sink.bases(kind, len, src, q, rf, w);
                 if (kind == ck) {
                     cl += len;
                 } else {
@@ -527,6 +573,8 @@ struct AlnCount {
     }
     template <class Walk>
     __device__ void place(const Walk&) {}
+    template <class Walk>
+    __device__ void bases(uint32_t, uint32_t, uint32_t, uint32_t, uint32_t, const Walk&) {}
     __device__ void op(uint32_t, uint32_t) { ++body; }
     __device__ void end(uint32_t q1, uint32_t rf1) {
         words += body + (q0 > 0) + (q1 < L);
@@ -556,11 +604,33 @@ __global__ void aln_count_kernel(AlnArgs a) {
     a.primary[i] = c.prim;
 }
 
+// With NM (aln_write_tags_kernel): where the walk finds the bases an M is compared with
+struct AlnTagArgs {
+    const uint8_t* seq;             // the batch's bases (NsReadMeta::seq_off)
+    const uint8_t* bases;           // the resident reference (DevRef: bases, chrom_off, pk_off, exc_pre)
+    const uint64_t* chrom_off;
+    const uint64_t* pk_off;
+    const uint32_t* exc_pre;
+    const uint8_t* pair;            // ALN_LIFT: the REF bytes the ALT of variant v pairs with its first bases, at pair_off[v]
+    const uint64_t* pair_off;
+    uint32_t* nm;                   // every record's NM
+};
+
+// bases [off, off + n) of resident record rec lie in 4096-base blocks without an exception (DevRef::exc_pre): every byte is
+// one of a/c/g/t in either case
+__device__ __forceinline__ bool aln_ref_plain(const AlnTagArgs& g, uint32_t rec, uint32_t off, uint32_t n) {
+    const uint64_t pk0 = g.pk_off[rec], w_lo = pk0 + (off >> 4), w_hi = pk0 + ((off + n - 1) >> 4);
+    return __ldg(&g.exc_pre[(w_hi >> REF_EXC_BLOCK_SHIFT) + 1]) == __ldg(&g.exc_pre[w_lo >> REF_EXC_BLOCK_SHIFT]);
+}
+
 // ALN_LIFT: refID is the haplotype's source record and POS the lifted one; a part inside an <INV> is a record on the other
 // strand, its CIGAR words (written in haplotype order) reversed in place and its stored bases mirrored.  ALN_SPLICE: refID
 // is the genome record and POS the leftmost genome base; a minus-strand transcript's part is a record on the other strand
 // as an <INV> part is, and the strand goes into the XS field.
-template <AlnMode kMode>
+// kTags: every record's NM into tg.nm: its I and D lengths and the M bases whose 4-bit code differs from the reference
+// byte's, or either is N (DESIGN §3 "NM and SA tags").  An M of a COPY (MIS) op over blocks without an exception matches
+// (differs) base for base; any other M compares the read's bases with the reference bytes.
+template <AlnMode kMode, bool kTags = false>
 struct AlnWrite {
     uint32_t i, L, nl, prim, rev;
     BamAln* rec;                    // the read's records
@@ -571,15 +641,21 @@ struct AlnWrite {
     uint32_t n_aln = 0, w = 0, w0 = 0, q0 = 0, rf0 = 0, chrom = 0, pos = 0, at = 0;
     bool inv = false;
     uint64_t clen = 0;
+    AlnTagArgs tg;                  // kTags only
+    const uint8_t* sq = nullptr;    // the read's bases
+    uint32_t* nm_out = nullptr;     // its records' NM
+    uint32_t nm = 0, piece_rec = 0; // NM of the alignment so far; the segment's resident record
     __device__ void segment(const NsPieceMeta& pc, uint64_t len) {
         chrom = pc.chrom;
         pos = pc.pos;
         clen = len;
+        piece_rec = pc.chrom;
     }
     __device__ void begin(uint32_t q, uint32_t rf) {
         q0 = q;
         rf0 = rf;
         w0 = w;
+        nm = 0;
         if (q > 0) cig[w++] = (q << 4) | (n_aln == prim ? CIG_S : CIG_H);
     }
     template <class Walk>
@@ -587,6 +663,50 @@ struct AlnWrite {
         at = w.at;
         inv = w.inv;
         if constexpr (kMode == ALN_SPLICE) chrom = w.chrom;
+    }
+    // an op of the alignment, its first base at read offset q and segment reference offset rf, the walk as it stands
+    template <class Walk>
+    __device__ void bases(uint32_t kind, uint32_t len, uint32_t src, uint32_t q, uint32_t rf, const Walk& wk) {
+        if constexpr (kTags) {
+            if (kind == CIG_I || kind == CIG_D) nm += len;
+            if (kind != CIG_M) return;
+            uint32_t rc = piece_rec, off;                       // resident record and lowest offset of the M's bases
+            bool comp = false;                                  // the bases run backwards there, complemented
+            const uint8_t* paired = nullptr;                    // the REF bytes of an ALT
+            bool inv_u = false;                                 // inside an <INV>: a U/u byte stands for the haploid's U
+            if constexpr (kMode == ALN_PLAIN) {
+                const uint64_t x = (uint64_t)pos + rf;
+                off = (uint32_t)(x < clen ? x : x % clen);      // behind a circular record's origin only
+            } else if constexpr (kMode == ALN_LIFT) {
+                // haplotype h's segments alternate stretch, variant, ..., stretch from lift.first[h] = 2 var_off[h] + h, so
+                // segment s is a variant when s - h is odd, and then it is variant (s - h - 1) / 2 in NsVariants order (the
+                // global index pair_off takes)
+                off = wk.seg[wk.s].hap0 + wk.t;
+                const uint64_t s2 = wk.s - piece_rec;            // 2 var_off[h] + the segment's place in its record
+                if (wk.kind[wk.s] == HAP_LIFT_SEQ && (s2 & 1)) paired = tg.pair + tg.pair_off[(s2 - 1) >> 1] + wk.t;
+                inv_u = wk.inv;
+            } else if (wk.exon) {                               // a transcript piece: the transcript's own bases
+                off = wk.exon[wk.k].cum + wk.t;
+            } else {                                            // a chain piece: the genome record's
+                rc = wk.genome_first + wk.chrom;
+                comp = wk.inv;
+                off = wk.inv ? wk.start + wk.len - wk.t - len : wk.start + wk.t;
+            }
+            if (!paired && src != ALN_SRC_LIT && aln_ref_plain(tg, rc, off, len)) {
+                if (src == ALN_SRC_MIS) nm += len;
+                return;
+            }
+            const uint8_t* g = paired ? paired : tg.bases + tg.chrom_off[rc] + off;
+            for (uint32_t j = 0; j < len; ++j) {
+                const uint32_t f = q + j;
+                const uint32_t b = rev ? bam_code_comp(bam_base_code(sq[L - 1 - f])) : bam_base_code(sq[f]);
+                uint32_t r = comp ? bam_code_comp(bam_base_code(g[len - 1 - j])) : bam_base_code(g[j]);
+                // an <INV> segment holds the haploid bytes complemented by hap_complement, which keeps U/u: the haploid
+                // base there is a U (read as T), whose complement is A
+                if (inv_u && (g[j] | 0x20) == 'u') r = 1;
+                nm += b != r || b == 15 || r == 15;
+            }
+        }
     }
     __device__ void op(uint32_t kind, uint32_t len) { cig[w++] = (len << 4) | kind; }
     __device__ void end(uint32_t q1, uint32_t rf1) {
@@ -622,17 +742,18 @@ struct AlnWrite {
         b.cig_off = cig_off + w0;
         rec[n_aln] = b;
         size[n_aln] = bam_mapped_size(nl, b, kMode != ALN_PLAIN ? 4 : 0);
+        if constexpr (kTags) nm_out[n_aln] = nm;
         ++n_aln;
     }
 };
 
-template <AlnMode kMode>
-__global__ void aln_write_kernel(AlnArgs a) {
+template <AlnMode kMode, bool kTags>
+__device__ __forceinline__ void aln_write(const AlnArgs& a, const AlnTagArgs& tg) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n_reads) return;
     const NsReadMeta r = a.reads[i];
     const uint64_t r0 = a.rec_first[i];
-    AlnWrite<kMode> s;
+    AlnWrite<kMode, kTags> s;
     s.lift = a.lift;
     s.i = i;
     s.L = r.seq_len;
@@ -643,6 +764,11 @@ __global__ void aln_write_kernel(AlnArgs a) {
     s.cig_off = a.cig_first[i];
     s.cig = a.cigar + s.cig_off;
     s.size = a.rec_size + r0;
+    if constexpr (kTags) {
+        s.tg = tg;
+        s.sq = tg.seq + r.seq_off;
+        s.nm_out = tg.nm + r0;
+    }
     aln_read<kMode>(a, r, s);
     if (s.n_aln == 0) {                                         // the unmapped record of ns_compress_bam
         BamAln b{};
@@ -651,5 +777,126 @@ __global__ void aln_write_kernel(AlnArgs a) {
         b.flag = 4;
         a.aln[r0] = b;
         a.rec_size[r0] = BgzfBamLayout::size(s.nl, r.seq_len, 0);
+    }
+}
+
+template <AlnMode kMode>
+__global__ void aln_write_kernel(AlnArgs a) {
+    aln_write<kMode, false>(a, AlnTagArgs{});
+}
+
+template <AlnMode kMode>
+__global__ void aln_write_tags_kernel(AlnArgs a, AlnTagArgs tg) {
+    aln_write<kMode, true>(a, tg);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// aux fields with NM and SA, one thread per read over its records (DESIGN §3 "NM and SA tags"): a mapped record's are
+// HP:C (lift) or XS:A (splice), NM:I, and SA:Z when the read has more than one record, with one entry
+// "rname,pos,strand,CIGAR,60,NM;" for each of its other records in record order.  CG:B,I follows in BgzfTaggedLayout.
+// ---------------------------------------------------------------------------------------------------------------------
+struct AlnAuxArgs {
+    const BamAln* aln;
+    const uint32_t* cigar;
+    const uint32_t* nm;
+    const uint64_t* n_rec;          // per read: its records and its first record
+    const uint64_t* rec_first;
+    const char* sn;                 // the header's @SQ SN names back to back, name k at sn_off[k] .. sn_off[k + 1]
+    const uint64_t* sn_off;
+    uint32_t n_reads, mode;         // mode: the AlnMode of the records
+    uint64_t* rec_size;             // size pass: every mapped record's size grows by its NM and SA fields
+    uint64_t* aux_len;              // size pass: every record's aux bytes before CG
+    const uint64_t* aux_off;        // write pass: their exclusive prefix sum, and where they go
+    uint8_t* aux;
+};
+
+__device__ __forceinline__ uint32_t aln_dec_len(uint32_t v) {
+    uint32_t n = 1;
+    for (; v >= 10; v /= 10) ++n;
+    return n;
+}
+__device__ __forceinline__ uint8_t* aln_put_dec(uint8_t* p, uint32_t v) {
+    const uint32_t n = aln_dec_len(v);
+    for (uint32_t k = n; k-- > 0; v /= 10) p[k] = (uint8_t)('0' + v % 10);
+    return p + n;
+}
+
+// bytes of record b's SA entry
+__device__ __forceinline__ uint64_t aln_sa_len(const AlnAuxArgs& x, const BamAln& b, uint32_t nm) {
+    uint64_t n = x.sn_off[b.ref_id + 1] - x.sn_off[b.ref_id] + aln_dec_len(b.pos + 1) + aln_dec_len(nm) + 9;      // ,,+/-,,60,;
+    const uint32_t* c = x.cigar + b.cig_off;
+    for (uint32_t k = 0; k < b.n_cig; ++k) n += aln_dec_len(c[k] >> 4) + 1;
+    return n;
+}
+__device__ __forceinline__ uint8_t* aln_sa_put(const AlnAuxArgs& x, uint8_t* p, const BamAln& b, uint32_t nm) {
+    for (uint64_t k = x.sn_off[b.ref_id]; k < x.sn_off[b.ref_id + 1]; ++k) *p++ = (uint8_t)x.sn[k];
+    *p++ = ',';
+    p = aln_put_dec(p, b.pos + 1);
+    *p++ = ',';
+    *p++ = (b.flag & 16) ? '-' : '+';
+    *p++ = ',';
+    const uint32_t* c = x.cigar + b.cig_off;
+    for (uint32_t k = 0; k < b.n_cig; ++k) {
+        p = aln_put_dec(p, c[k] >> 4);
+        *p++ = (uint8_t)"MIDNSHP=X"[c[k] & 15];
+    }
+    *p++ = ',';
+    *p++ = '6';
+    *p++ = '0';
+    *p++ = ',';
+    p = aln_put_dec(p, nm);
+    *p++ = ';';
+    return p;
+}
+
+__global__ void aln_aux_size_kernel(AlnAuxArgs x) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= x.n_reads) return;
+    const uint64_t r0 = x.rec_first[i], k = x.n_rec[i];
+    if (x.aln[r0].flag & 4) {                                   // the unmapped record: no aux field
+        x.aux_len[r0] = 0;
+        return;
+    }
+    const uint32_t hp = x.mode != ALN_PLAIN ? 4 : 0;
+    uint64_t all = 0;                                           // every record's SA entry
+    if (k > 1)
+        for (uint64_t j = 0; j < k; ++j) all += x.aux_len[r0 + j] = aln_sa_len(x, x.aln[r0 + j], x.nm[r0 + j]);
+    for (uint64_t j = 0; j < k; ++j) {
+        const uint64_t sa = k > 1 ? 3 + all - x.aux_len[r0 + j] + 1 : 0;
+        x.rec_size[r0 + j] += 7 + sa;
+        x.aux_len[r0 + j] = hp + 7 + sa;
+    }
+}
+
+__global__ void aln_aux_write_kernel(AlnAuxArgs x) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= x.n_reads) return;
+    const uint64_t r0 = x.rec_first[i], k = x.n_rec[i];
+    if (x.aln[r0].flag & 4) return;
+    for (uint64_t j = 0; j < k; ++j) {
+        const BamAln b = x.aln[r0 + j];
+        uint8_t* p = x.aux + x.aux_off[r0 + j];
+        if (x.mode != ALN_PLAIN) {
+            const uint32_t v = b.flag >> BAM_HP_SHIFT;
+            p[0] = x.mode == ALN_LIFT ? 'H' : 'X';
+            p[1] = x.mode == ALN_LIFT ? 'P' : 'S';
+            p[2] = x.mode == ALN_LIFT ? 'C' : 'A';
+            p[3] = (uint8_t)(x.mode == ALN_LIFT ? v : v ? '-' : '+');
+            p += 4;
+        }
+        const uint32_t nm = x.nm[r0 + j];
+        p[0] = 'N';
+        p[1] = 'M';
+        p[2] = 'I';
+        for (int s = 0; s < 4; ++s) p[3 + s] = (uint8_t)(nm >> (8 * s));
+        p += 7;
+        if (k == 1) continue;
+        p[0] = 'S';
+        p[1] = 'A';
+        p[2] = 'Z';
+        p += 3;
+        for (uint64_t o = 0; o < k; ++o)
+            if (o != j) p = aln_sa_put(x, p, x.aln[r0 + o], x.nm[r0 + o]);
+        *p = 0;
     }
 }

@@ -131,8 +131,15 @@ struct Tables {
     bool have_lift = false;
     // ns_set_splice: the transcripts' exons on the genome records (aln_kernel.cuh's AlnSplice)
     DevBuf splice_exon, splice_first, splice_minus;
-    uint32_t splice_n_trx = 0, splice_genome_first = NS_SPLICE_NO_GENOME;
+    uint32_t splice_n_trx = 0, splice_genome_first = NS_SPLICE_NO_GENOME, splice_n_genome = 0;
     bool have_splice = false;
+    // ns_set_lift, for ns_set_aln_tags: the lift's variant count and the REF bytes its ALTs pair with (prefix sum per variant)
+    std::vector<uint64_t> h_lift_pair_off;
+    // ns_set_aln_tags: the mapped header's SN names (aln_kernel.cuh's AlnAuxArgs) and, with a lift, the REF bytes
+    // (AlnTagArgs::pair, pair_off)
+    DevBuf tag_sn, tag_sn_off, tag_pair, tag_pair_off;
+    uint32_t tag_n_sn = 0;
+    bool have_aln_tags = false;
 };
 
 // transcript lengths ascending + their record indices (ns_configure, transcriptome mode); a clone that configures another
@@ -190,6 +197,8 @@ struct NsContext {
     // ns_compress_bam_mapped: per read its record and CIGAR-word counts (2n) and their offsets (2n), its primary alignment;
     // the records' descriptors and CIGAR words.  Its members go to z_out.
     DevBuf m_cnt, m_first, m_prim, m_aln, m_cig;
+    // with NM and SA (ns_set_aln_tags): every record's NM, aux bytes, their offsets, and the aux bytes themselves
+    DevBuf m_nm, m_aux_len, m_aux_off, m_aux;
     // Batches of one job have near-identical sizes: once a batch of a kind has run with host-sized buffers, the next ones
     // are submitted in one go (no host round trip between the first and the last kernel) against those capacities; a
     // kernel checks them on the device and a batch that does not fit is simply run again the sized way.
@@ -230,6 +239,7 @@ enum TotalsSlot : int {
     // overwrite
     NS_T_M_RECORDS = NS_T_Z_TEXT,
     NS_T_M_CIGAR_WORDS = NS_T_Z_BYTES,
+    NS_T_M_AUX_BYTES = NS_T_Z_BYTES,    // with NM and SA, at the second wait: the records' aux bytes
 };
 
 // Wait for everything queued on the context's stream.  cudaStreamSynchronize spins: a host thread per overlapped context then
@@ -701,6 +711,13 @@ int ns_clone(NsContext* parent, NsContext** out) {
     return NS_OK;
 }
 
+// ns_set_aln_tags' tables go with every table they were built against
+static void drop_aln_tags(Tables& tab) {
+    tab.have_aln_tags = false;
+    tab.tag_n_sn = 0;
+    for (DevBuf* b : {&tab.tag_sn, &tab.tag_sn_off, &tab.tag_pair, &tab.tag_pair_off}) b->release();
+}
+
 int ns_set_reference(NsContext* ctx, const NsReference* ref) {
     if (!ctx || !ref || !ref->bases || !ref->chrom_off || ref->n_chrom == 0)
         return fail(ctx, NS_EINVAL, "ns_set_reference: null argument or empty reference");
@@ -798,6 +815,7 @@ int ns_set_reference(NsContext* ctx, const NsReference* ref) {
     for (DevBuf* b : {&tab.lift_seg, &tab.lift_kind, &tab.lift_first, &tab.lift_chrom, &tab.lift_hp}) b->release();
     tab.have_splice = false;
     for (DevBuf* b : {&tab.splice_exon, &tab.splice_first, &tab.splice_minus}) b->release();
+    drop_aln_tags(tab);
     ctx->have_batch = false;
     ctx->opt_ok[0] = ctx->opt_ok[1] = false;
     return NS_OK;
@@ -945,6 +963,10 @@ int ns_set_lift(NsContext* ctx, const NsVariants* v) {
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     tab.have_lift = false;
+    drop_aln_tags(tab);
+    tab.h_lift_pair_off.assign(v->n_var + 1, 0);
+    for (uint64_t j = 0; j < v->n_var; ++j)
+        tab.h_lift_pair_off[j + 1] = tab.h_lift_pair_off[j] + ((v->alt_kind ? v->alt_kind[j] : 0) == HAP_LIFT_SEQ ? std::min(v->alt_len[j], v->var_ref_len[j]) : 0);
     DevBuf haploid;
     VariantLayout lay;
     CK(upload(haploid, off.data(), off.size() * 8, st));
@@ -1018,14 +1040,49 @@ int ns_set_splice(NsContext* ctx, const NsSplice* sp) {
     CK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     tab.have_splice = false;
+    drop_aln_tags(tab);
     CK(upload(tab.splice_exon, ex.data(), std::max<size_t>(ex.size(), 1) * sizeof(SpliceExon), st));
     CK(upload(tab.splice_first, sp->exon_off, ((size_t)sp->n_trx + 1) * 8, st));
     CK(upload(tab.splice_minus, sp->minus, std::max<size_t>(sp->n_trx, 1), st));
     CK(cudaStreamSynchronize(st));
     tab.splice_n_trx = sp->n_trx;
     tab.splice_genome_first = sp->genome_first;
+    tab.splice_n_genome = sp->n_genome;
     tab.have_splice = true;
     if (sp->peak_bytes) *sp->peak_bytes = tab.splice_exon.cap + tab.splice_first.cap + tab.splice_minus.cap;
+    return NS_OK;
+}
+
+int ns_set_aln_tags(NsContext* ctx, const NsAlnTags* t) {
+    static const char* fname = "ns_set_aln_tags";
+    if (!ctx || !t || !t->ref_name_off || (t->ref_name_off[t->n_ref] && !t->ref_names) || (t->ref_paired_bytes && !t->ref_paired))
+        return fail(ctx, NS_EINVAL, "%s: null argument", fname);
+    if (ctx->clone) return fail(ctx, NS_ESTATE, "%s: a cloned context shares its parent's tables", fname);
+    Tables& tab = *ctx->tables;
+    if (!tab.have_ref) return fail(ctx, NS_ESTATE, "%s: set the reference first (ns_set_reference or ns_bcast_nccl)", fname);
+    if (t->ref_name_off[0] != 0) return fail(ctx, NS_EINVAL, "%s: ref_name_off must start at 0", fname);
+    for (uint32_t k = 0; k < t->n_ref; ++k)
+        if (t->ref_name_off[k + 1] <= t->ref_name_off[k])
+            return fail(ctx, NS_EINVAL, "%s: reference name %u is empty or ref_name_off decreases there", fname, k);
+    const uint64_t n_var = tab.have_lift ? tab.h_lift_pair_off.size() - 1 : 0;
+    const uint64_t paired = tab.have_lift ? tab.h_lift_pair_off.back() : 0;
+    if (t->n_var != n_var)
+        return fail(ctx, NS_EINVAL, "%s: the REF bytes table is for %llu variants, the lift has %llu", fname, (unsigned long long)t->n_var,
+                    (unsigned long long)n_var);
+    if (t->ref_paired_bytes != paired)
+        return fail(ctx, NS_EINVAL, "%s: the REF bytes table has %llu bytes, the lift's ALTs pair %llu", fname,
+                    (unsigned long long)t->ref_paired_bytes, (unsigned long long)paired);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    drop_aln_tags(tab);
+    CK(upload(tab.tag_sn, t->ref_names, t->ref_name_off[t->n_ref], st));
+    CK(upload(tab.tag_sn_off, t->ref_name_off, ((size_t)t->n_ref + 1) * 8, st));
+    CK(upload(tab.tag_pair, t->ref_paired, paired, st));
+    if (tab.have_lift) CK(upload(tab.tag_pair_off, tab.h_lift_pair_off.data(), tab.h_lift_pair_off.size() * 8, st));
+    CK(cudaStreamSynchronize(st));
+    tab.tag_n_sn = t->n_ref;
+    tab.have_aln_tags = true;
+    if (t->peak_bytes) *t->peak_bytes = tab.tag_sn.cap + tab.tag_sn_off.cap + tab.tag_pair.cap + tab.tag_pair_off.cap;
     return NS_OK;
 }
 
@@ -1885,6 +1942,12 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
         return fail(ctx, NS_EINVAL, "%s: the splice map's transcripts and genome records are not the run's (trx_records %u)", fname,
                     ctx->hcfg.trx_records);
     if (mode == ALN_LIFT && ctx->hcfg.circular) return fail(ctx, NS_EINVAL, "%s: lifted records need linear haplotype records", fname);
+    // NM and SA (ns_set_aln_tags): the header's names must be the records' refIDs
+    const bool tags = tab.have_aln_tags;
+    const uint64_t n_ids = mode == ALN_SPLICE ? tab.splice_n_genome : mode == ALN_LIFT ? tab.h_haploid_off.size() - 1 : tab.dref.n_chrom;
+    if (tags && tab.tag_n_sn != n_ids)
+        return fail(ctx, NS_EINVAL, "%s: ns_set_aln_tags gave %u reference names for %llu reference records", fname, tab.tag_n_sn,
+                    (unsigned long long)n_ids);
     uint32_t n = 0;
     if (int rc = begin_members(ctx, names, name_off, ctx->z_out, nbytes, &n)) return rc;
     if (n == 0) return NS_OK;
@@ -1933,11 +1996,48 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
         aa.aln = ctx->m_aln.as<BamAln>();
         aa.cigar = ctx->m_cig.as<uint32_t>();
         aa.rec_size = ctx->scan_in.as<uint64_t>();
-        CK(launch(ctx, aln_write_kernel<kMode>, grid, 256, 0, aa));
+        // with NM and SA: the tagged walk, the records' aux sizes (added to rec_size) and offsets before the same wait
+        AlnAuxArgs ax{};
+        if (tags) {
+            CK(ctx->m_nm.ensure((size_t)n_rec * sizeof(uint32_t)));
+            CK(ctx->m_aux_len.ensure((size_t)n_rec * sizeof(uint64_t)));
+            CK(ctx->m_aux_off.ensure((size_t)n_rec * sizeof(uint64_t)));
+            const AlnTagArgs tg{ctx->seq.as<uint8_t>(), tab.dref.bases, tab.dref.chrom_off, tab.dref.pk_off, tab.dref.exc_pre,
+                                tab.tag_pair.as<uint8_t>(), tab.tag_pair_off.as<uint64_t>(), ctx->m_nm.as<uint32_t>()};
+            CK(launch(ctx, aln_write_tags_kernel<kMode>, grid, 256, 0, aa, tg));
+            ax.aln = aa.aln;
+            ax.cigar = aa.cigar;
+            ax.nm = tg.nm;
+            ax.n_rec = aa.n_rec;
+            ax.rec_first = rec_first;
+            ax.sn = tab.tag_sn.as<char>();
+            ax.sn_off = tab.tag_sn_off.as<uint64_t>();
+            ax.n_reads = n;
+            ax.mode = (uint32_t)kMode;
+            ax.rec_size = aa.rec_size;
+            ax.aux_len = ctx->m_aux_len.as<uint64_t>();
+            ax.aux_off = ctx->m_aux_off.as<uint64_t>();
+            CK(launch(ctx, aln_aux_size_kernel, grid, 256, 0, ax));
+            if (int rc = scan_total(ctx, ax.aux_len, ctx->m_aux_off.as<uint64_t>(), (uint32_t)n_rec, NS_T_M_AUX_BYTES)) return rc;
+        } else {
+            CK(launch(ctx, aln_write_kernel<kMode>, grid, 256, 0, aa));
+        }
         if (int rc = scan_total(ctx, aa.rec_size, ctx->z_rec_off.as<uint64_t>(), (uint32_t)n_rec, NS_T_Z_TEXT)) return rc;
         if (int rc = publish_totals_and_wait(ctx)) return rc;
+        const BgzfMappedTable mt{read_table(ctx), aa.aln, aa.cigar};
+        if (tags) {
+            const uint64_t aux_total = h[NS_T_M_AUX_BYTES];
+            CK(ctx->m_aux.ensure((size_t)std::max<uint64_t>(aux_total, 1)));
+            ax.aux = ctx->m_aux.as<uint8_t>();
+            CK(launch(ctx, aln_aux_write_kernel, grid, 256, 0, ax));
+            BgzfRecords<BgzfTaggedLayout> src;
+            src.tab = BgzfTaggedTable{mt, ax.aux, ax.aux_off, aux_total, (uint32_t)n_rec};
+            src.rec_off = ctx->z_rec_off.as<uint64_t>();
+            src.n_recs = (uint32_t)n_rec;
+            return end_members(ctx, fname, h[NS_T_Z_TEXT], src, ctx->z_out, nbytes);
+        }
         BgzfRecords<Layout> src;
-        src.tab = BgzfMappedTable{read_table(ctx), aa.aln, aa.cigar};
+        src.tab = mt;
         src.rec_off = ctx->z_rec_off.as<uint64_t>();
         src.n_recs = (uint32_t)n_rec;
         return end_members(ctx, fname, h[NS_T_Z_TEXT], src, ctx->z_out, nbytes);

@@ -124,6 +124,20 @@ class Engine:
         self._check(self._lib.ns_set_splice(self._ctx, C.byref(s)))
         return int(n.value)
 
+    def set_aln_tags(self, ref_names, ref_paired=None, n_var=0):
+        """--aln_tags: compress_bam_mapped() adds NM and SA to every mapped record (ns_set_aln_tags).  ref_names: the mapped
+        header's @SQ names in refID order; with set_lift(tables), ref_paired = tables.ref_paired (the REF bytes the ALTs'
+        first bases pair with) and n_var = its variant count.  Call after set_lift() / set_splice() and before clone().
+        Returns the device bytes the tables keep."""
+        enc = [n.encode() for n in ref_names]
+        blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+        off = np.concatenate([[0], np.cumsum([len(e) for e in enc])]).astype(np.uint64)
+        paired = np.ascontiguousarray(ref_paired if ref_paired is not None else np.zeros(0), dtype=np.uint8)
+        n = C.c_uint64()
+        t = L.NsAlnTags(len(enc), _ptr(blob), _ptr(off), int(n_var), _ptr(paired) if len(paired) else None, len(paired), C.pointer(n))
+        self._check(self._lib.ns_set_aln_tags(self._ctx, C.byref(t)))
+        return int(n.value)
+
     def set_abundance(self, abun, inflated=None):
         """dict_abun / dict_abun_inflated of one sample, per species in genome-list order (metagenome mode)."""
         a = np.ascontiguousarray(abun, dtype=np.float64)

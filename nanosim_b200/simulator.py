@@ -174,6 +174,7 @@ def _apply_variants(prof, tables, ref_on_host, lift=False):
     """Makes the haplotype records of ``tables`` the resident reference of prof.engine (built on the device); the haploid
     records' names and offsets stay in prof.haploid.  lift: ns_set_lift with the same tables."""
     prof.haploid = _RemoteReference(prof.ref.names, prof.ref.offsets, prof.ref.raw_names)
+    prof.haplotypes = tables
     prof.engine.apply_variants(tables)
     if lift:
         prof.engine.set_lift(tables)
@@ -552,6 +553,23 @@ LIFT_HELP = ('With --vcf and --mapped_bam: write the true alignments in <out>_al
              'an aligner or a VCF names them) instead of the haplotype records: variants become CIGAR operations, <INV> and '
              '<DUP> split alignments, and every record has HP:C:1 or HP:C:2 for its haplotype. Read names and the error '
              'profile stay in haplotype coordinates (Default = False)')
+ALN_TAGS_HELP = ('With --mapped_bam (genome, metagenome; lifted or not) or --spliced_bam (transcriptome): give every mapped '
+                 'record of <out>_aligned_reads.bam NM:I (edit distance to the reference bases, as samtools calmd counts it) '
+                 'and, for a read with more than one record, SA:Z listing its other records, computed on the GPU. '
+                 'Nothing else in the output changes (Default = False)')
+
+
+def _set_aln_tags(args, prof, mapped_refs):
+    """--aln_tags: NM and SA against the records of the mapped header (mapped_refs), with the REF bytes of the VCF's
+    ALTs under --lift_mapped_bam; before simulation() clones the engine."""
+    if not getattr(args, "aln_tags", False):
+        return
+    names = [n for n, _, _ in mapped_refs]
+    if getattr(args, "lift_mapped_bam", False):
+        t = prof.haplotypes
+        prof.engine.set_aln_tags(names, t.ref_paired, len(t.var_pos))
+    else:
+        prof.engine.set_aln_tags(names)
 
 
 def _plain_error_profile(args):
@@ -608,6 +626,7 @@ def build_parser():
     g.add_argument('--mapped_bam', help=MAPPED_BAM_HELP, action='store_true', default=False)
     g.add_argument('--vcf', help=VCF_HELP, default=None)
     g.add_argument('--lift_mapped_bam', help=LIFT_HELP, action='store_true', default=False)
+    g.add_argument('--aln_tags', help=ALN_TAGS_HELP, action='store_true', default=False)
     mg = sub.add_parser('metagenome', help="Run the simulator on metagenome mode")
     mg.add_argument('-gl', '--genome_list', help="Reference metagenome list, tsv file, the first column is species/strain "
                     "name, the second column is the reference genome fasta/fastq file directory", required=True)
@@ -644,6 +663,7 @@ def build_parser():
     mg.add_argument('--gzip_error_profile', help=GZIP_ERR_HELP, action='store_true', default=False)
     mg.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     mg.add_argument('--mapped_bam', help=MAPPED_BAM_HELP, action='store_true', default=False)
+    mg.add_argument('--aln_tags', help=ALN_TAGS_HELP, action='store_true', default=False)
     t = sub.add_parser('transcriptome', help="Run the simulator on transcriptome mode")
     t.add_argument('-rt', '--ref_t', help='Input reference transcriptome', required=True)
     t.add_argument('-rg', '--ref_g', help='Input reference genome, required if intron retention simulation is on', default='')
@@ -687,6 +707,7 @@ def build_parser():
     t.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     t.add_argument('--mapped_bam', help=argparse.SUPPRESS, action='store_true', default=False)     # a usage error here
     t.add_argument('--spliced_bam', help=SPLICED_BAM_HELP, action='store_true', default=False)
+    t.add_argument('--aln_tags', help=ALN_TAGS_HELP, action='store_true', default=False)
     return parser, g, mg, t
 
 
@@ -749,6 +770,7 @@ def main_transcriptome(args, parser_t):
     if args.spliced_bam:
         prof.engine.set_splice(prof.splice)
         mapped_refs = prof.spliced_refs
+        _set_aln_tags(args, prof, mapped_refs)
     if args.coverage is not None:
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
@@ -809,6 +831,7 @@ def main_metagenome(args, parser_mg):
                         dna_type=args.dna_type_list, abun=args.abun, chimeric=args.chimeric, homopolymer=args.homopolymer,
                         fastq=args.fastq, device=device, seed=args.seed or 0, ref_on_host=_plain_error_profile(args))
     mapped_refs = _mapped_refs(args, prof, False)
+    _set_aln_tags(args, prof, mapped_refs)
     rnd = random.Random(args.seed)
     L_ = prof.ref.lengths
     total_len = [int(L_[prof.ref.chrom_species == i].sum()) for i in range(len(prof.ref.species))]
@@ -886,6 +909,10 @@ def main(argv=None):
         usage = "--lift_mapped_bam needs --vcf"
     elif getattr(args, "lift_mapped_bam", False) and not args.mapped_bam:
         usage = "--lift_mapped_bam needs --mapped_bam"
+    elif args.aln_tags and args.mode == "transcriptome" and not args.spliced_bam:
+        usage = "--aln_tags needs --spliced_bam in transcriptome mode"
+    elif args.aln_tags and args.mode != "transcriptome" and not args.mapped_bam:
+        usage = "--aln_tags needs --mapped_bam"
     if usage:
         sys.stderr.write("\n" + usage + "!\n")
         {"genome": parser_g, "metagenome": parser_mg, "transcriptome": parser_t}[args.mode].print_help(sys.stderr)
@@ -944,6 +971,7 @@ def main(argv=None):
         prof.number_aligned, prof.number_unaligned = prof.tables.split_counts(number[0], args.perfect)
     max_len = min(max_len, prof.max_chrom)
     mapped_refs = _mapped_refs(args, prof, args.dna_type == "circular")
+    _set_aln_tags(args, prof, mapped_refs)
     simulation(prof, args.mode, args.output, args.dna_type, args.perfect, args.KmerBias if args.homopolymer else None,
                None, max_len, min_len, max(args.num_threads, 1), args.fastq, args.median_len, args.sd_len,
                chimeric=args.chimeric, batch_reads=args.batch_reads, error_profile=not args.no_error_profile,

@@ -72,6 +72,7 @@ class HaplotypeTables:
         self.skipped = np.ascontiguousarray(skipped, dtype=np.int64)    # records of its chromosome skipped by FILTER
         self.skipped_elsewhere = int(skipped_elsewhere)     # records skipped by FILTER on contigs the reference lacks
         self.alt_kind = np.ascontiguousarray(np.zeros(len(self.var_pos)) if alt_kind is None else alt_kind, dtype=np.uint8)
+        self.ref_paired = None      # read_vcf: paired_ref_bytes over the reference the tables were read against
 
     @property
     def applied(self):
@@ -88,6 +89,16 @@ class HaplotypeTables:
     @property
     def offsets(self):
         return np.concatenate([[0], np.cumsum(self.lengths)]).astype(np.uint64)
+
+
+def paired_ref_bytes(tables, ref):
+    """The reference bytes [var_pos, var_pos + min(alt_len, var_ref_len)) of every kind-0 variant of ``tables``, back to
+    back in table order: the REF bases a lifted alignment pairs an ALT's first bases with, which NM compares them to
+    (``ns_set_aln_tags``).  ``ref``: the PackedReference the tables were read against."""
+    n = np.where(tables.alt_kind == 0, np.minimum(tables.alt_len, tables.var_ref_len), 0).astype(np.int64)
+    chrom = np.repeat(tables.hap_chrom.astype(np.int64), np.diff(tables.var_off.astype(np.int64)))
+    pos, _ = _flat(np.asarray(ref.offsets, dtype=np.int64)[chrom] + tables.var_pos.astype(np.int64), n)
+    return np.ascontiguousarray(np.asarray(ref.bases)[pos], dtype=np.uint8)
 
 
 def _read_bytes(path):
@@ -170,6 +181,7 @@ def read_vcf(path, ref):
             continue
         if first_error is not None:
             raise first_error
+        tables.ref_paired = paired_ref_bytes(tables, ref)
         return tables
 
 

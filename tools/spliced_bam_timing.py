@@ -75,6 +75,8 @@ def main():
     ap.add_argument("--chroms", type=int, default=4)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", default=None, help="also write the JSON line here")
+    ap.add_argument("--tags", action="store_true", help="also time spliced records with NM and SA (ns_set_aln_tags), in a "
+                    "second context that simulates the same batch")
     args = ap.parse_args()
     with tempfile.TemporaryDirectory() as d:
         gff3 = os.path.join(d, "annotation.gff3")
@@ -91,6 +93,12 @@ def main():
     res["bases"], res["n_ops"] = int(info.total_bases), int(info.n_ops)
     names = name_table(eng.fetch(), trx.names, 0, transcriptome=True)
     arms = {"bam": eng.compress_bam, "spliced": eng.compress_bam_mapped}
+    if args.tags:
+        tagged, _, _ = pc.make_trx_engine(trx, np.arange(len(trx.names), dtype=np.uint32), w / w.sum(), fastq=True, seed=13)
+        tagged.set_splice(smap)
+        res["tags_bytes"] = tagged.set_aln_tags(list(genome.raw_names))
+        tagged.simulate(L.NS_KIND_ALIGNED, 0, args.reads)
+        arms["spliced_tagged"] = tagged.compress_bam_mapped
     res["bytes"] = {k: f(names) for k, f in arms.items()}                  # grows the context's buffers
     calls = {k: [] for k in arms}
     for _ in range(args.reps):
@@ -114,6 +122,8 @@ def main():
                 kern[name] = kern.get(name, 0.0) + ev.device_time_total / 1e3
         res["kernels_ms"][k] = {n: round(v, 3) for n, v in sorted(kern.items(), key=lambda kv: -kv[1])}
     eng.close()
+    if args.tags:
+        tagged.close()
     res["gpu"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
                                 text=True).stdout.strip()
     line = json.dumps(res)
