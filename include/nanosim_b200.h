@@ -139,9 +139,8 @@ typedef struct {
  * sends every piece down the exact route (tests compare the two). */
 #define NS_FLAG_EMIT_EXACT 4u
 /* Pieces longer than 16 kb are emitted as several work items (each resuming the script walk from a checkpoint), so that the
- * longest read of a batch does not keep one warp busy long after the rest has finished; long unaligned reads are walked by a
- * whole thread block instead of one warp for the same reason.  This flag emits every piece as one item and walks every
- * unaligned read with one warp (tests compare the two: same bytes). */
+ * longest read of a batch does not keep one warp busy long after the rest has finished.  This flag emits every piece as one
+ * item (tests compare the two: same bytes). */
 #define NS_FLAG_EMIT_WHOLE 8u
 
 #define NS_KIND_ALIGNED 0

@@ -1593,7 +1593,6 @@ int ns_simulate(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_rea
     ua.pool_cursor = (unsigned long long*)(d_totals + NS_T_POOL_CURSOR);
     ua.pool = d_totals + NS_T_POOL;             // {base, size} of the bump pool, written by capacity_stage_a
     ua.abort = d_abort;
-    ua.cta_min_len = (ctx->hcfg.flags & NS_FLAG_EMIT_WHOLE) ? 0u : (uint32_t)UREAD_CTA_MIN_LEN;
     const unsigned ublocks = std::min<unsigned>((n + UREAD_WARPS - 1) / UREAD_WARPS, (unsigned)ctx->sm_count * 8u);
     if (chim && !ctx->hcfg.perfect) {
         // chimeric gaps of every read's first attempt, a warp per read (uread_kernel.cuh:gap_kernel)
