@@ -38,6 +38,10 @@
 
 #define EMIT_WARPS 8
 #define EMIT_RING 256
+// Unaligned batches: their scripts hold about 0.87 ops per base, so 256 entries cover only ~290 of a step's 512 bases and
+// 14 of 32 lanes idle.  Every piece of such a batch is unmapped and draws its qualities from one state's alias table, so
+// the 32 KB of the other four tables hold a ring twice as long instead (same shared memory, 3 blocks per SM).
+#define EMIT_RING_UNAL 512
 #ifndef EMIT_MIN_BLOCKS
 #define EMIT_MIN_BLOCKS 3     // resident blocks per SM the register allocation aims for
 #endif
@@ -187,14 +191,15 @@ __device__ __forceinline__ uint32_t entry_ref(const uint4& e, uint32_t rdir, uin
 
 // Exact path for ONE base whose reference byte is not plain ACGT (IUPAC codes): locates the ring entry of padded piece
 // coordinate x again and redoes the base with the same random bits.  Returns the character.
+template <uint32_t RING>
 __device__ __noinline__ uint32_t emit_fix_base(const EmitArgs& a, const EmitPiece& pc, const uint4* ring, uint32_t w_ret,
                                                uint32_t w_loaded, uint32_t x, uint32_t rb2, uint32_t misoff) {
     uint32_t l = w_ret, h = w_loaded;
     while (h - l > 1) {
         uint32_t mid = (l + h) >> 1;
-        if (ring[mid & (EMIT_RING - 1)].x <= 2u * x) l = mid; else h = mid;
+        if (ring[mid & (RING - 1)].x <= 2u * x) l = mid; else h = mid;
     }
-    const uint4 e = ring[l & (EMIT_RING - 1)];
+    const uint4 e = ring[l & (RING - 1)];
     const uint32_t info = e.w;
     uint32_t oi;
     if (info & EMIT_F_REF) {
@@ -217,7 +222,8 @@ __device__ __noinline__ uint32_t emit_fix_base(const EmitArgs& a, const EmitPiec
 // ---- EXACT route: the branch-free 16-base walk of one chunk over the reference bytes.  WRAPS: the piece crosses the
 // origin of a circular chromosome (:1756-1760).  COMP: complementing classification (minus-strand genome pieces).
 // sub = the chunk's substitution offsets (sub_offsets).
-template <bool FASTQ, bool WRAPS, bool COMP>
+// ONE_LUT: every piece is unmapped and `lut` holds only the unmapped state's alias table (the unaligned batches' kernel).
+template <bool FASTQ, bool WRAPS, bool COMP, uint32_t RING, bool ONE_LUT>
 __device__ __forceinline__ void emit_chunk16(const uint4* ring, const uint32_t* lut, const uint8_t* cvt_tables,
                                              const uint8_t* __restrict__ cbase, uint32_t RB, uint32_t sub, const ChunkQual<FASTQ>& Q,
                                              uint32_t& k, uint32_t& rem, uint32_t& rabs, uint32_t& info, uint32_t rdir, uint32_t clen,
@@ -229,7 +235,7 @@ __device__ __forceinline__ void emit_chunk16(const uint4* ring, const uint32_t* 
     for (int i = 0; i < 16; ++i) {
         if (rem == 0) {                                    // next entry (never empty, never a deletion)
             ++k;
-            const uint4 e = ring[k & (EMIT_RING - 1)];
+            const uint4 e = ring[k & (RING - 1)];
             rem = (e.z - e.x) >> 1;
             rabs = entry_ref(e, rdir, e.x >> 1);
             info = e.w;
@@ -248,7 +254,7 @@ __device__ __forceinline__ void emit_chunk16(const uint4* ring, const uint32_t* 
         sel += v << (4 * (i & 3));
         if (FASTQ) {
             const uint32_t w = Q.W[i];
-            const uint32_t e = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(lut) + (info >> 16) +
+            const uint32_t e = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(lut) + (ONE_LUT ? 0u : info >> 16) +
                                                                   ((w >> 6) & 0x1ffcu));
             sq[i >> 2] |= (qual_pick(e, w) & 0xffu) << (8 * (i & 3));
         }
@@ -296,7 +302,7 @@ __device__ __forceinline__ void load_packed_pair(const uint32_t* __restrict__ pk
     w1 = __ldg(pk + widx + 1);
 }
 
-template <bool RDIR>
+template <bool RDIR, uint32_t RING>
 __device__ __forceinline__ uint32_t emit_walk_entries(uint32_t ring_s, const uint32_t* __restrict__ pk, uint32_t pk0w, uint32_t win_s,
                                                       uint32_t win_w0, uint32_t RB, uint32_t& k, uint32_t cs, uint32_t& S, uint32_t& mism) {
     uint32_t acc = 0;
@@ -305,7 +311,7 @@ __device__ __forceinline__ uint32_t emit_walk_entries(uint32_t ring_s, const uin
     const uint32_t cs2 = 2u * cs;
     for (;;) {
         uint4 e;
-        asm("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(e.x), "=r"(e.y), "=r"(e.z), "=r"(e.w) : "r"(ring_s + ((k & (EMIT_RING - 1)) << 4)));
+        asm("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(e.x), "=r"(e.y), "=r"(e.z), "=r"(e.w) : "r"(ring_s + ((k & (RING - 1)) << 4)));
         const uint32_t info = e.w;
         const int32_t d0 = (int32_t)(e.x - cs2);
         const uint32_t lo2 = (uint32_t)(d0 > 0 ? d0 : 0);                   // 2 * first chunk position of the entry
@@ -342,7 +348,7 @@ __device__ __forceinline__ uint32_t emit_walk_entries(uint32_t ring_s, const uin
     return acc;
 }
 
-template <bool FASTQ>
+template <bool FASTQ, uint32_t RING>
 __device__ __forceinline__ void emit_chunk16_fast(uint32_t ring_s, const char* lut_s, const uint32_t* __restrict__ pk, uint32_t pk0w,
                                                   uint32_t win_s, uint32_t win_w0, uint32_t& k,
                                                   uint32_t cs, bool rdir, bool unmapped, uint32_t tbl, uint32_t id_lo, uint32_t id_hi,
@@ -350,8 +356,8 @@ __device__ __forceinline__ void emit_chunk16_fast(uint32_t ring_s, const char* l
     ChunkAux R;
     draw_chunk_aux<FASTQ>(R, id_lo, id_hi, kind, chunk, key);
     uint32_t S, mism;
-    uint32_t acc = rdir ? emit_walk_entries<true>(ring_s, pk, pk0w, win_s, win_w0, R.RB, k, cs, S, mism)
-                        : emit_walk_entries<false>(ring_s, pk, pk0w, win_s, win_w0, R.RB, k, cs, S, mism);
+    uint32_t acc = rdir ? emit_walk_entries<true, RING>(ring_s, pk, pk0w, win_s, win_w0, R.RB, k, cs, S, mism)
+                        : emit_walk_entries<false, RING>(ring_s, pk, pk0w, win_s, win_w0, R.RB, k, cs, S, mism);
     ChunkQual<FASTQ> Q;                                                     // after the walk: 16 fewer live registers in it
     draw_chunk_qual<FASTQ>(Q, id_lo, id_hi, kind, chunk, key);
     // substituted bases: index + 1 + uniform{0,1,2} (mod 4), quality state "mis" (0)
@@ -381,18 +387,27 @@ __device__ __forceinline__ void emit_chunk16_fast(uint32_t ring_s, const char* l
     }
 }
 
-template <bool FASTQ>
+// Shared memory of one block: the alias tables, the classification tables, the rings, the reference windows.
+template <bool FASTQ, uint32_t RING>
+constexpr size_t emit_smem_bytes() {
+    return (FASTQ ? (size_t)(RING == EMIT_RING ? NS_N_QUAL_STATES : 1) * QLUT_SIZE * 4 : 0) + 512 +
+           (size_t)EMIT_WARPS * RING * sizeof(uint4) + EMIT_WINDOW_SMEM;
+}
+
+// RING = EMIT_RING_UNAL: a batch of unaligned reads (every piece unmapped; NS_PIECE_UNALIGNED).
+template <bool FASTQ, uint32_t RING>
 __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(const __grid_constant__ EmitArgs a) {
     if (a.abort && *a.abort) return;
+    constexpr bool UNAL = RING != EMIT_RING;
     extern __shared__ uint4 smem4[];
     uint32_t* lut = reinterpret_cast<uint32_t*>(smem4);                          // FASTQ only
-    uint8_t* cvt_tables = reinterpret_cast<uint8_t*>(lut + (FASTQ ? NS_N_QUAL_STATES * QLUT_SIZE : 0));
+    uint8_t* cvt_tables = reinterpret_cast<uint8_t*>(lut + (FASTQ ? (UNAL ? 1 : NS_N_QUAL_STATES) * QLUT_SIZE : 0));
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint4* ring = reinterpret_cast<uint4*>(cvt_tables + 512) + warp * EMIT_RING;
+    uint4* ring = reinterpret_cast<uint4*>(cvt_tables + 512) + warp * RING;
     const uint32_t ring_s = (uint32_t)__cvta_generic_to_shared(ring);
 #if EMIT_TMA_WINDOW
     // per warp: a 64-word window of the packed reference + the mbarrier its TMA copy completes on
-    const uint32_t win_s = (uint32_t)__cvta_generic_to_shared(reinterpret_cast<uint4*>(cvt_tables + 512) + EMIT_WARPS * EMIT_RING) +
+    const uint32_t win_s = (uint32_t)__cvta_generic_to_shared(reinterpret_cast<uint4*>(cvt_tables + 512) + EMIT_WARPS * RING) +
                            warp * (EMIT_WIN_WORDS * 4);
     const uint32_t mbar_s = win_s + (EMIT_WARPS - warp) * (EMIT_WIN_WORDS * 4) + warp * 8;
     uint32_t win_phase = 0;
@@ -404,7 +419,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
     const uint32_t win_s = 0;
 #endif
     if (FASTQ)
-        for (int i = threadIdx.x; i < NS_N_QUAL_STATES * QLUT_SIZE; i += blockDim.x) lut[i] = a.qlut[i];
+        for (int i = threadIdx.x; i < (UNAL ? 1 : NS_N_QUAL_STATES) * QLUT_SIZE; i += blockDim.x) lut[i] = a.qlut[(UNAL ? 4 * QLUT_SIZE : 0) + i];   // UNAL: state 4 (unmapped) only
     {   // case_convert classification: base index 0..3 (A C T G), 4 = needs the IUPAC path
         uint32_t c = threadIdx.x;
         uint32_t u = (c - 'a' < 26u) ? c - 32u : c;
@@ -480,7 +495,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
         const uint32_t* __restrict__ ops = a.ops + pm.op_off;
         uint8_t* seq_out = a.seq + rm.seq_off + P0;
         uint8_t* qual_out = FASTQ ? a.qual + rm.seq_off + P0 : nullptr;
-        const bool unmapped = NS_PIECE_KIND(pm.kind) != NS_PIECE_SEGMENT;
+        const bool unmapped = UNAL || NS_PIECE_KIND(pm.kind) != NS_PIECE_SEGMENT;
         const uint32_t id_lo = (uint32_t)pc.rid, id_hi = (uint32_t)(pc.rid >> 32);
         const uint32_t info_pad = emit_op_info(NS_OP_HT << 28, unmapped, ref_comp);
         // route: the fast one needs a forward-complement piece that stays inside its chromosome and whose packed words hold
@@ -491,7 +506,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
             const uint64_t w_lo = pk0 + (pm.pos >> 4), w_hi = pk0 + ((pm.pos + ref_len - 1u) >> 4);
             fast = __ldg(&a.ref.exc_pre[(w_hi >> REF_EXC_BLOCK_SHIFT) + 1]) == __ldg(&a.ref.exc_pre[w_lo >> REF_EXC_BLOCK_SHIFT]);
         }
-        const char* lut_s = reinterpret_cast<const char*>(lut) + (unmapped ? 4u * QLUT_SIZE * 4u : 0u);
+        const char* lut_s = reinterpret_cast<const char*>(lut) + (unmapped && !UNAL ? 4u * QLUT_SIZE * 4u : 0u);
 
         uint32_t t_loaded = t_first, w_loaded = 0, w_ret = 0, out_loaded = out_first, ref_loaded = ref_first, prog = x_first;
         bool closed = false;
@@ -503,16 +518,25 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
         auto put_entry = [&](uint32_t slot, uint32_t xo, uint32_t rstart, uint32_t len, uint32_t op) {
             uint32_t ab = pm.pos + (rdir ? ref_len - 1u - rstart : rstart);           // first base in walking order
             if (wraps && ab >= clen) ab -= clen;
-            ring[slot & (EMIT_RING - 1)] = make_uint4(2u * xo, rdir ? ab + xo : ab - xo, 2u * (xo + len), emit_op_info(op, unmapped, ref_comp));
+            ring[slot & (RING - 1)] = make_uint4(2u * xo, rdir ? ab + xo : ab - xo, 2u * (xo + len), emit_op_info(op, unmapped, ref_comp));
         };
+        // the lane's two ops of the next round of the ring build, loaded one round ahead: the load of a step's first round
+        // is in flight while the previous step produces its chunks
+        uint32_t pf0 = 0, pf1 = 0;
+        {
+            const uint32_t t = t_loaded + 2u * lane;
+            if (t < n_ops) pf0 = __ldg(&ops[rev ? n_ops - 1u - t : t]);
+            if (t + 1u < n_ops) pf1 = __ldg(&ops[rev ? n_ops - 2u - t : t + 1u]);
+        }
         while (prog < x_end) {
             // ---- 1. stream ops into the ring, two per lane, until the next 32 chunks are covered or the ring is full
             uint32_t target = prog + 512u < x_end ? prog + 512u : x_end;
-            while (out_loaded < target && t_loaded < n_ops && (w_loaded - w_ret) + 65u <= EMIT_RING) {
+            while (out_loaded < target && t_loaded < n_ops && (w_loaded - w_ret) + 65u <= RING) {
                 const uint32_t t = t_loaded + 2u * lane;
-                uint32_t op0 = 0, op1 = 0;
-                if (t < n_ops) op0 = __ldg(&ops[rev ? n_ops - 1u - t : t]);
-                if (t + 1u < n_ops) op1 = __ldg(&ops[rev ? n_ops - 2u - t : t + 1u]);
+                const uint32_t op0 = pf0, op1 = pf1;
+                pf0 = pf1 = 0;
+                if (t + 64u < n_ops) pf0 = __ldg(&ops[rev ? n_ops - 65u - t : t + 64u]);
+                if (t + 65u < n_ops) pf1 = __ldg(&ops[rev ? n_ops - 66u - t : t + 65u]);
                 const uint32_t ty0 = op0 >> 28, len0 = op_len(op0), ty1 = op1 >> 28, len1 = op_len(op1);
                 const uint32_t o0 = (ty0 == NS_OP_DEL) ? 0u : len0, o1 = (ty1 == NS_OP_DEL) ? 0u : len1;
                 const uint32_t r0 = (ty0 < 2u || ty0 == NS_OP_DEL) ? len0 : 0u, r1 = (ty1 < 2u || ty1 == NS_OP_DEL) ? len1 : 0u;
@@ -529,7 +553,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
             }
             if (!closed && (t_loaded == n_ops || out_loaded >= x_end)) {
                 // sentinel: walking past the end of the piece stays inside the ring (ops left over are deletions)
-                if (lane == 0) ring[w_loaded & (EMIT_RING - 1)] = make_uint4(2u * out_loaded, 0u, 2u * out_loaded + 0x7ffffffeu, info_pad);
+                if (lane == 0) ring[w_loaded & (RING - 1)] = make_uint4(2u * out_loaded, 0u, 2u * out_loaded + 0x7ffffffeu, info_pad);
                 ++w_loaded;
                 closed = true;
             }
@@ -539,10 +563,10 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
             if (fast) {
                 // the first entry at or after the step's first base that reads the reference tells where the step starts on it
                 uint32_t kk = w_ret;
-                uint4 e = ring[kk & (EMIT_RING - 1)];
+                uint4 e = ring[kk & (RING - 1)];
                 while (!(e.w & EMIT_F_REF) && kk + 1u < w_loaded) {
                     ++kk;
-                    e = ring[kk & (EMIT_RING - 1)];
+                    e = ring[kk & (RING - 1)];
                 }
                 if (e.w & EMIT_F_REF) {
                     const uint32_t x0 = e.x >> 1;
@@ -561,7 +585,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
             // ---- 2. what can be produced now: whole chunks up to the loaded frontier (or the piece end)
             uint32_t lim = out_loaded < target ? out_loaded : target;
             if (lim < x_end) lim &= ~15u;
-            // (the ring holds >= 190 entries of >= 1 base beyond w_ret, so lim > prog whenever ops remain)
+            // (the ring holds >= RING - 66 entries of >= 1 base beyond w_ret, so lim > prog whenever ops remain)
             // ---- 3. one 16-byte chunk per lane
             const uint32_t cs = prog + 16u * lane;
             uint32_t k = w_ret;
@@ -569,7 +593,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
                 uint32_t l = w_ret, h = w_loaded;     // last entry whose output start <= cs
                 while (h - l > 1) {
                     uint32_t mid = (l + h) >> 1;
-                    if (ring[mid & (EMIT_RING - 1)].x <= 2u * cs) l = mid; else h = mid;
+                    if (ring[mid & (RING - 1)].x <= 2u * cs) l = mid; else h = mid;
                 }
                 k = l;
                 // ---- all randomness of the chunk is position-indexed: (read id, chunk index in read coordinates)
@@ -582,7 +606,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
                                      ::"r"(mbar_s), "r"(win_phase) : "memory");
                     }
 #endif
-                    emit_chunk16_fast<FASTQ>(ring_s, lut_s, a.ref.packed, (uint32_t)pk0, win_s, win_w0, k, cs, rdir, unmapped, tbl, id_lo, id_hi, a.kind, chunk, key, sb, sq);
+                    emit_chunk16_fast<FASTQ, RING>(ring_s, lut_s, a.ref.packed, (uint32_t)pk0, win_s, win_w0, k, cs, rdir, unmapped, tbl, id_lo, id_hi, a.kind, chunk, key, sb, sq);
                 } else {
                     ChunkAux R;
                     ChunkQual<FASTQ> Q;
@@ -591,7 +615,7 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
                     const uint32_t sub = sub_offsets(R.X, Q.X);
                     uint32_t rem, rabs, info;
                     {
-                        const uint4 e = ring[k & (EMIT_RING - 1)];
+                        const uint4 e = ring[k & (RING - 1)];
                         rem = (e.z >> 1) - cs;
                         info = e.w;
                         rabs = entry_ref(e, rdir, cs);
@@ -599,14 +623,14 @@ __global__ void __launch_bounds__(EMIT_WARPS * 32, EMIT_MIN_BLOCKS) emit_kernel(
                     }
                     uint32_t bad = 0;
                     // three instantiations: plain, circular wrap, complementing (minus-strand genome pieces; keeps the wrap check)
-                    if (ref_comp) emit_chunk16<FASTQ, true, true>(ring, lut, cvt_tables, cbase, R.RB, sub, Q, k, rem, rabs, info, rdir, clen, wrap_fix, tbl, sb, sq, bad);
-                    else if (wraps) emit_chunk16<FASTQ, true, false>(ring, lut, cvt_tables, cbase, R.RB, sub, Q, k, rem, rabs, info, rdir, clen, wrap_fix, tbl, sb, sq, bad);
-                    else emit_chunk16<FASTQ, false, false>(ring, lut, cvt_tables, cbase, R.RB, sub, Q, k, rem, rabs, info, rdir, clen, wrap_fix, tbl, sb, sq, bad);
+                    if (ref_comp) emit_chunk16<FASTQ, true, true, RING, UNAL>(ring, lut, cvt_tables, cbase, R.RB, sub, Q, k, rem, rabs, info, rdir, clen, wrap_fix, tbl, sb, sq, bad);
+                    else if (wraps) emit_chunk16<FASTQ, true, false, RING, UNAL>(ring, lut, cvt_tables, cbase, R.RB, sub, Q, k, rem, rabs, info, rdir, clen, wrap_fix, tbl, sb, sq, bad);
+                    else emit_chunk16<FASTQ, false, false, RING, UNAL>(ring, lut, cvt_tables, cbase, R.RB, sub, Q, k, rem, rabs, info, rdir, clen, wrap_fix, tbl, sb, sq, bad);
                     // ---- rare: IUPAC codes, one base at a time
                     if (bad & 4u) {
 #pragma unroll
                         for (int i = 0; i < 16; ++i) {
-                            const uint32_t f = emit_fix_base(a, pc, ring, w_ret, w_loaded, cs + i, (R.RB >> (2 * i)) & 3u, (sub >> (2 * i)) & 3u);
+                            const uint32_t f = emit_fix_base<RING>(a, pc, ring, w_ret, w_loaded, cs + i, (R.RB >> (2 * i)) & 3u, (sub >> (2 * i)) & 3u);
                             const uint32_t m = 0xffu << (8 * (i & 3));
                             sb[i >> 2] = (sb[i >> 2] & ~m) | (f << (8 * (i & 3)));
                         }

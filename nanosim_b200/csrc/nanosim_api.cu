@@ -638,9 +638,12 @@ int launch_emit(NsContext* ctx, int kind, uint64_t first_read_id, uint32_t n_pie
         }
     }
     // FASTQ: the quality tables go to shared memory as well
-    void (*kernel)(EmitArgs) = ctx->hcfg.fastq ? emit_kernel<true> : emit_kernel<false>;
-    const size_t smem = (size_t)EMIT_WARPS * EMIT_RING * sizeof(uint4) + 512 + EMIT_WINDOW_SMEM +
-                        (ctx->hcfg.fastq ? (size_t)NS_N_QUAL_STATES * QLUT_SIZE * 4 : 0);
+    // an unaligned batch holds unaligned read bodies only (NS_PIECE_UNALIGNED): the kernel with the longer ring
+    const bool unal = kind == NS_KIND_UNALIGNED;
+    void (*kernel)(EmitArgs) = ctx->hcfg.fastq ? (unal ? emit_kernel<true, EMIT_RING_UNAL> : emit_kernel<true, EMIT_RING>)
+                                               : (unal ? emit_kernel<false, EMIT_RING_UNAL> : emit_kernel<false, EMIT_RING>);
+    const size_t smem = ctx->hcfg.fastq ? (unal ? emit_smem_bytes<true, EMIT_RING_UNAL>() : emit_smem_bytes<true, EMIT_RING>())
+                                        : (unal ? emit_smem_bytes<false, EMIT_RING_UNAL>() : emit_smem_bytes<false, EMIT_RING>());
     CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 1;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, EMIT_WARPS * 32, smem));
