@@ -471,6 +471,20 @@ int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off,
  * NS_EINVAL when the last batch is unaligned reads, the context is in transcriptome mode without a splice map (or with one
  * whose records are not the run's), a lift meets a circular configuration, or the tags' names are not one per refID. */
 int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
+/* transcriptome --transcript_bam: the last aligned batch as mapped BAM records against the TRANSCRIPT records (resident
+ * records 0 .. n-1, n = NsRunConfig.trx_records with intron retention, else every record), built and compressed like
+ * ns_compress_bam_mapped's (DESIGN.md §3 "Transcript-coordinate mapped BAM").  A read on a transcript piece gets the
+ * records of "Mapped BAM": refID its transcript, POS the transcript offset, no aux field but CG.  A read that retains an
+ * intron (an NS_PIECE_GENOME chain) walks its pieces back to back: an exon piece is placed on the transcript through the
+ * splice map (ns_set_splice) and keeps its M and D, an M over a retained intron is an I and a D there vanishes; an exon
+ * piece that does not continue the previous one in transcript offsets starts a supplementary record.  refID is the chain's
+ * transcript (ref_req), flag 16 the read's `reversed`.  A chain whose transcript has no map, or with an exon piece in no
+ * exon of it, gets ns_compress_bam's unmapped record.  With ns_set_aln_tags' tables (one name per transcript record) every
+ * mapped record has NM:I and, when its read has more than one record, SA:Z before CG.  Same name layout, 254-byte name
+ * limit, members slot and ns_fetch_compressed as ns_compress_bam_mapped.  NS_EINVAL outside transcriptome mode, when the
+ * last batch is unaligned reads, with intron retention (trx_records != 0) when the context has no splice map or one whose
+ * transcripts and genome records are not the run's, and when the tags' names are not one per transcript record. */
+int ns_compress_bam_transcript(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes);
 /* Device->host copy of those members; NS_ENOMEM when cap is smaller than ns_compress_records' (or ns_compress_bam's)
  * *nbytes. */
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap);

@@ -25,7 +25,7 @@ NS_STATS_WORDS = NS_STATS_COMP_OFF + 4
 EXPORTS = ["ns_create", "ns_destroy", "ns_last_error", "ns_clone", "ns_set_abundance", "ns_set_expression", "ns_set_reference", "ns_set_model", "ns_configure",
            "ns_simulate", "ns_fetch", "ns_reemit", "ns_batch_info", "ns_device_buffers", "ns_op_stats", "ns_format_records", "ns_format_error_profile", "ns_format_names", "ns_transfer_info", "ns_write_records", "ns_write_error_profile", "ns_read_fasta", "ns_nccl_unique_id", "ns_bcast_nccl", "ns_get_reference", "ns_unpack_bases",
            "ns_compress_records", "ns_fetch_compressed", "ns_compress_error_profile", "ns_fetch_compressed_error_profile", "ns_compress_bam", "ns_apply_variants",
-           "ns_compress_bam_mapped", "ns_set_lift", "ns_set_splice", "ns_set_aln_tags"]
+           "ns_compress_bam_mapped", "ns_set_lift", "ns_set_splice", "ns_set_aln_tags", "ns_compress_bam_transcript"]
 
 
 class NsReference(C.Structure):
@@ -206,6 +206,8 @@ def lib():
     L.ns_compress_bam.restype = C.c_int
     L.ns_compress_bam_mapped.argtypes = [P, P, P, C.POINTER(C.c_uint64)]
     L.ns_compress_bam_mapped.restype = C.c_int
+    L.ns_compress_bam_transcript.argtypes = [P, P, P, C.POINTER(C.c_uint64)]
+    L.ns_compress_bam_transcript.restype = C.c_int
     L.ns_fetch_compressed.argtypes = [P, P, C.c_uint64]
     L.ns_fetch_compressed.restype = C.c_int
     L.ns_compress_error_profile.argtypes = [P, P, P, C.POINTER(C.c_uint64)]

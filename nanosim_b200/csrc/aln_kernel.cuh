@@ -11,6 +11,9 @@
 // ALN_SPLICE (ns_set_splice, DESIGN §3 "Spliced mapped BAM"): transcriptome reads, the walk composed with the transcript's
 // exons (or, for a read that retains an intron, with its chain of genome pieces), so the records are against the genome
 // with an N for every intron the read skips.
+// ALN_TRX (ns_compress_bam_transcript, DESIGN §3 "Transcript-coordinate mapped BAM"): transcriptome reads against the
+// transcripts they came from: a transcript piece takes the plain walk, a read that retains an intron walks its chain of
+// genome pieces composed with its transcript's exons (ns_set_splice), the retained bases as insertions.
 // NM and SA (ns_set_aln_tags, DESIGN §3 "NM and SA tags"): aln_write_tags_kernel is the same write walk counting every
 // record's NM on the way (AlnWrite<kMode, true>::bases); aln_aux_size_kernel and aln_aux_write_kernel then lay out and
 // fill each record's aux fields (HP/XS, NM, SA) for bgzf_deflate_kernel<BgzfRecords<BgzfTaggedLayout>>.
@@ -21,7 +24,9 @@
 #include "haplotype.h"
 
 // which walk an aln kernel instantiation runs
-enum AlnMode : int { ALN_PLAIN = 0, ALN_LIFT = 1, ALN_SPLICE = 2 };
+enum AlnMode : int { ALN_PLAIN = 0, ALN_LIFT = 1, ALN_SPLICE = 2, ALN_TRX = 3 };
+// the walks whose mapped records have a leading aux field (HP:C, XS:A); ALN_TRX records have the plain layout
+__host__ __device__ constexpr bool aln_lead_aux(uint32_t mode) { return mode == ALN_LIFT || mode == ALN_SPLICE; }
 
 // CIGAR operations (SAM/BAM specification §4.2.2: MIDNSHP=X -> 0..8)
 enum : uint32_t { CIG_M = 0, CIG_I = 1, CIG_D = 2, CIG_N = 3, CIG_S = 4, CIG_H = 5 };
@@ -91,7 +96,7 @@ struct BgzfMappedTable {
 template <AlnMode kMode>
 struct BgzfMappedLayoutOf {
     using Table = BgzfMappedTable;
-    static constexpr uint32_t hp = kMode != ALN_PLAIN ? 4 : 0;
+    static constexpr uint32_t hp = aln_lead_aux(kMode) ? 4 : 0;
     static __device__ __forceinline__ uint8_t byte(uint64_t q, const BgzfMappedRec& rc) {
         const BamAln& a = rc.a;
         if (a.flag & 4) return BgzfBamLayout::byte(q, rc.rd);
@@ -105,7 +110,7 @@ struct BgzfMappedLayoutOf {
             case 1: w = a.ref_id; break;
             case 2: w = a.pos; break;
             case 3: w = (nl + 1) | (BAM_MAPQ << 8) | ((uint32_t)a.bin << 16); break;       // l_read_name, mapq, bin
-            case 4: w = nc | ((uint32_t)(kMode != ALN_PLAIN ? a.flag & BAM_FLAG_BITS : a.flag) << 16); break;   // n_cigar_op, flag
+            case 4: w = nc | ((uint32_t)(aln_lead_aux(kMode) ? a.flag & BAM_FLAG_BITS : a.flag) << 16); break;   // n_cigar_op, flag
             case 5: w = ls; break;                                                          // l_seq
             case 8: w = 0; break;                                                           // tlen
             default: w = 0xffffffffu;                                                       // next_refID, next_pos
@@ -348,8 +353,78 @@ __device__ __forceinline__ void splice_put(SpliceWalk& w, uint32_t kind, uint32_
     }
 }
 
+// ALN_TRX: where the walk of a read that retains an intron stands: offset t in piece k (of len bases) of its chain, the
+// segments src[0], src[2], ... (n_src of them) back to back.  off is the transcript offset of piece k's first base in
+// chain order (TRX_RETAINED: the piece lies in a retained intron), end one past the transcript offset of the last exon
+// piece entered (~0u: none yet).  Before each M or D: at, the transcript offset of its first base.
+constexpr uint32_t TRX_RETAINED = ~0u;
+struct TrxWalk {
+    const NsPieceMeta* src;
+    const uint32_t* ops;
+    const SpliceExon* exon;         // the transcript's exons in transcript order (n_exon)
+    uint32_t n_src, n_exon, genome_first;
+    uint32_t k, t, len, off, end, at;
+    bool minus;                     // the transcript's strand
+};
+
+// The transcript offset of the first base in transcript order of the genome bases [pos, pos + len) of genome record
+// chrom, when they lie in one exon of the transcript: the exons' starts ascend in transcript order on the plus strand and
+// descend on the minus strand (ns_set_splice checks that), so a binary search finds the one that starts last at or
+// before pos.  false when no exon holds them.
+__device__ __forceinline__ bool trx_offset(const TrxWalk& w, uint32_t chrom, uint32_t pos, uint32_t len, uint32_t& off) {
+    uint32_t lo = 0, hi = w.n_exon;                 // ends at the first exon starting after pos (plus), at or before it (minus)
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if ((w.exon[mid].start <= pos) != w.minus) lo = mid + 1; else hi = mid;
+    }
+    if (w.minus ? lo == w.n_exon : lo == 0) return false;
+    const SpliceExon e = w.exon[w.minus ? lo : lo - 1];
+    if (e.chrom != chrom || (uint64_t)pos + len > (uint64_t)e.start + e.len) return false;
+    off = e.cum + (w.minus ? e.start + e.len - (pos + len) : pos - e.start);
+    return true;
+}
+
+// Into piece k of the chain: an exon piece that does not start where the last one entered ended (in transcript offsets)
+// ends the alignment (ALN_CUT)
+template <class Fn>
+__device__ __forceinline__ void trx_enter(TrxWalk& w, uint32_t k, Fn& fn) {
+    const NsPieceMeta& pc = w.src[2 * k];
+    w.k = k;
+    w.t = 0;
+    w.len = pc.ref_len;
+    if (pc.kind & NS_PIECE_RETAINED) {
+        w.off = TRX_RETAINED;
+        return;
+    }
+    trx_offset(w, pc.chrom - w.genome_first, pc.pos, pc.ref_len, w.off);      // aln_read_chain checked that it finds one
+    if (w.end != ~0u && w.off != w.end) fn(ALN_CUT, 0u, ALN_SRC_COPY);
+    w.end = w.off + w.len;
+}
+
+// A read op (M, I or D over the chain's pieces back to back) composed with the transcript: I stays I; M and D over an exon
+// piece stay M and D; over a retained intron an M becomes I and a D vanishes
+template <class Fn>
+__device__ __forceinline__ void trx_put(TrxWalk& w, uint32_t kind, uint32_t len, uint32_t src, Fn& fn) {
+    if (kind == CIG_I) {
+        fn(CIG_I, len, src);
+        return;
+    }
+    while (len) {
+        while (w.t >= w.len && w.k + 1 < w.n_src) trx_enter(w, w.k + 1, fn);
+        const uint32_t n = w.t < w.len ? min(len, w.len - w.t) : len;     // past the chain's last base (no chain gets here)
+        if (w.off != TRX_RETAINED) {
+            w.at = w.off + w.t;
+            fn(kind, n, src);
+        } else if (kind == CIG_M) {
+            fn(CIG_I, n, src);
+        }
+        w.t += n;
+        len -= n;
+    }
+}
+
 template <AlnMode kMode>
-using AlnWalk = std::conditional_t<kMode == ALN_SPLICE, SpliceWalk, LiftWalk>;
+using AlnWalk = std::conditional_t<kMode == ALN_SPLICE, SpliceWalk, std::conditional_t<kMode == ALN_TRX, TrxWalk, LiftWalk>>;
 
 struct AlnArgs {
     const NsReadMeta* reads;
@@ -370,7 +445,7 @@ struct AlnArgs {
     uint32_t* cigar;
     uint64_t* rec_size;
     AlnLift lift;                   // ALN_LIFT only
-    AlnSplice splice;               // ALN_SPLICE only
+    AlnSplice splice;               // ALN_SPLICE; ALN_TRX (the chains' transcripts; n_trx = 0: no map)
 };
 
 // fn(kind, len) over a segment's script: CIGAR kinds M I D (HT as I: it only stands at a read's edges), a LIT group followed
@@ -379,6 +454,7 @@ struct AlnArgs {
 // none), an M or D across one split there
 // ALN_LIFT: every op goes through lift_put on walk w instead (no circular record: cut is ~0)
 // ALN_SPLICE: the scripts of w's n_src pieces back to back (sc, n_ops unused), every op through splice_put
+// ALN_TRX (a chain only): the same, every op through trx_put
 template <AlnMode kMode, class Walk, class Fn>
 __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint32_t n_ops, uint64_t cut, uint64_t period, Walk& w,
                                            Fn fn) {
@@ -391,6 +467,9 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
             return;
         } else if constexpr (kMode == ALN_SPLICE) {
             splice_put(w, kind, len, src, fn);
+            return;
+        } else if constexpr (kMode == ALN_TRX) {
+            trx_put(w, kind, len, src, fn);
             return;
         }
         if (kind != CIG_I) {
@@ -407,9 +486,9 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
         fn(kind, len, src);
     };
     uint32_t n_src = 1;
-    if constexpr (kMode == ALN_SPLICE) n_src = w.n_src;
+    if constexpr (kMode == ALN_SPLICE || kMode == ALN_TRX) n_src = w.n_src;
     for (uint32_t p = 0; p < n_src; ++p) {
-        if constexpr (kMode == ALN_SPLICE) {
+        if constexpr (kMode == ALN_SPLICE || kMode == ALN_TRX) {
             sc = w.ops + w.src[2 * p].op_off;
             n_ops = w.src[2 * p].n_ops;
         }
@@ -437,9 +516,9 @@ __device__ __forceinline__ void aln_script(const uint32_t* __restrict__ sc, uint
 // each, sink.begin(q0, rf0) at its first M, sink.op(kind, len) for its merged ops, sink.end(q1, rf1) after its last M
 // (read offsets in the forward read, reference offsets in the segment).  Ops before the first M and after the last one
 // are outside the alignment: their I is clip, their D (or N) moves the start or is dropped.  Two walks per part: the first
-// finds the part's first and last M, the second emits what lies between them.  ALN_LIFT, ALN_SPLICE: every walk starts from
-// `start`, the first one counts the parts (n_parts = 1 on entry), and sink.place(w) follows sink.begin with the walk as it
-// stands at the first M (its position there).
+// finds the part's first and last M, the second emits what lies between them.  ALN_LIFT, ALN_SPLICE, ALN_TRX: every walk
+// starts from `start`, the first one counts the parts (n_parts = 1 on entry), and sink.place(w) follows sink.begin with the
+// walk as it stands at the first M (its position there).
 template <AlnMode kMode, class Sink>
 __device__ __forceinline__ void aln_segment(const uint32_t* sc, uint32_t n_ops, uint64_t cut, uint64_t period, uint32_t n_parts,
                                             uint32_t q_start, const AlnWalk<kMode>& start, Sink& sink) {
@@ -524,14 +603,50 @@ __device__ __forceinline__ void aln_read_spliced(const AlnArgs& a, const NsReadM
     aln_segment<ALN_SPLICE>(nullptr, 0, ~0ull, 0, 1, pc.out_rel, w, sink);
 }
 
+// ALN_TRX: read r laid out on the genome (NS_PIECE_GENOME: it retains an intron) walks its chain of pieces back to back,
+// its exon pieces composed with its transcript's exons, from the first piece.  No alignment when the transcript (ref_req)
+// has no map or one of its exon pieces lies in none of the map's exons.
+template <class Sink>
+__device__ __forceinline__ void aln_read_chain(const AlnArgs& a, const NsReadMeta& r, Sink& sink) {
+    const NsPieceMeta pc = a.pieces[r.piece_first];
+    if (pc.ref_req >= a.splice.n_trx) return;
+    const uint64_t e0 = a.splice.first[pc.ref_req], e1 = a.splice.first[pc.ref_req + 1];
+    if (e0 == e1) return;
+    TrxWalk w{};
+    w.src = a.pieces + r.piece_first;
+    w.ops = a.ops;
+    w.exon = a.splice.exon + e0;
+    w.n_src = (r.n_pieces + 1u) / 2u;
+    w.n_exon = (uint32_t)(e1 - e0);
+    w.genome_first = a.splice.genome_first;
+    w.minus = a.splice.minus[pc.ref_req] != 0;
+    for (uint32_t k = 0; k < w.n_src; ++k) {
+        const NsPieceMeta& p = w.src[2 * k];
+        uint32_t off;
+        if (!(p.kind & NS_PIECE_RETAINED) && !trx_offset(w, p.chrom - w.genome_first, p.pos, p.ref_len, off)) return;
+    }
+    w.end = ~0u;
+    auto none = [](uint32_t, uint32_t, uint32_t) {};
+    trx_enter(w, 0, none);
+    sink.segment(pc, 0);
+    aln_segment<ALN_TRX>(nullptr, 0, ~0ull, 0, 1, pc.out_rel, w, sink);
+}
+
 // every alignment of read r, in the order of its segments: sink.segment(piece, record length) before each segment's.
 // ALN_LIFT: the walk of a segment starts in the lift segment holding its first haplotype base, the last of its record's
-// segments that starts at or before it (binary search).
+// segments that starts at or before it (binary search).  ALN_TRX: a chain (aln_read_chain), else the plain walk.
 template <AlnMode kMode, class Sink>
 __device__ __forceinline__ void aln_read(const AlnArgs& a, const NsReadMeta& r, Sink& sink) {
     if constexpr (kMode == ALN_SPLICE) {
         aln_read_spliced(a, r, sink);
     } else {
+        if constexpr (kMode == ALN_TRX) {
+            if (r.n_pieces && (a.pieces[r.piece_first].kind & NS_PIECE_GENOME)) {
+                aln_read_chain(a, r, sink);
+                return;
+            }
+        }
+        constexpr AlnMode kSeg = kMode == ALN_TRX ? ALN_PLAIN : kMode;
         for (uint32_t k = 0; k < r.n_pieces; ++k) {
             const NsPieceMeta pc = a.pieces[r.piece_first + k];
             if (NS_PIECE_KIND(pc.kind) != NS_PIECE_SEGMENT) continue;
@@ -556,7 +671,7 @@ __device__ __forceinline__ void aln_read(const AlnArgs& a, const NsReadMeta& r, 
                 n_parts = 2 + (uint32_t)((pc.ref_len - 1 - cut) / clen);
             }
             sink.segment(pc, clen);
-            aln_segment<kMode>(a.ops + pc.op_off, pc.n_ops, cut, clen, n_parts, pc.out_rel, w, sink);
+            aln_segment<kSeg>(a.ops + pc.op_off, pc.n_ops, cut, clen, n_parts, pc.out_rel, w, sink);
         }
     }
 }
@@ -626,10 +741,12 @@ __device__ __forceinline__ bool aln_ref_plain(const AlnTagArgs& g, uint32_t rec,
 // ALN_LIFT: refID is the haplotype's source record and POS the lifted one; a part inside an <INV> is a record on the other
 // strand, its CIGAR words (written in haplotype order) reversed in place and its stored bases mirrored.  ALN_SPLICE: refID
 // is the genome record and POS the leftmost genome base; a minus-strand transcript's part is a record on the other strand
-// as an <INV> part is, and the strand goes into the XS field.
+// as an <INV> part is, and the strand goes into the XS field.  ALN_TRX: a transcript piece's records are the plain ones; a
+// chain's refID is its transcript (ref_req) and POS the transcript offset of its first M.
 // kTags: every record's NM into tg.nm: its I and D lengths and the M bases whose 4-bit code differs from the reference
 // byte's, or either is N (DESIGN §3 "NM and SA tags").  An M of a COPY (MIS) op over blocks without an exception matches
-// (differs) base for base; any other M compares the read's bases with the reference bytes.
+// (differs) base for base; any other M, and every M of an ALN_TRX chain (the read was copied from the genome, the record is
+// against the transcript), compares the read's bases with the reference bytes.
 template <AlnMode kMode, bool kTags = false>
 struct AlnWrite {
     uint32_t i, L, nl, prim, rev;
@@ -645,11 +762,18 @@ struct AlnWrite {
     const uint8_t* sq = nullptr;    // the read's bases
     uint32_t* nm_out = nullptr;     // its records' NM
     uint32_t nm = 0, piece_rec = 0; // NM of the alignment so far; the segment's resident record
+    bool chain = false;             // ALN_TRX: the read is a chain
     __device__ void segment(const NsPieceMeta& pc, uint64_t len) {
         chrom = pc.chrom;
         pos = pc.pos;
         clen = len;
         piece_rec = pc.chrom;
+        if constexpr (kMode == ALN_TRX) {
+            if (pc.kind & NS_PIECE_GENOME) {
+                chain = true;
+                chrom = piece_rec = pc.ref_req;
+            }
+        }
     }
     __device__ void begin(uint32_t q, uint32_t rf) {
         q0 = q;
@@ -661,7 +785,7 @@ struct AlnWrite {
     template <class Walk>
     __device__ void place(const Walk& w) {
         at = w.at;
-        inv = w.inv;
+        if constexpr (kMode != ALN_TRX) inv = w.inv;
         if constexpr (kMode == ALN_SPLICE) chrom = w.chrom;
     }
     // an op of the alignment, its first base at read offset q and segment reference offset rf, the walk as it stands
@@ -674,9 +798,13 @@ struct AlnWrite {
             bool comp = false;                                  // the bases run backwards there, complemented
             const uint8_t* paired = nullptr;                    // the REF bytes of an ALT
             bool inv_u = false;                                 // inside an <INV>: a U/u byte stands for the haploid's U
-            if constexpr (kMode == ALN_PLAIN) {
+            bool exact = false;                                 // compared byte by byte whatever the M's source
+            if constexpr (kMode == ALN_PLAIN || (kMode == ALN_TRX && !std::is_same_v<Walk, TrxWalk>)) {
                 const uint64_t x = (uint64_t)pos + rf;
                 off = (uint32_t)(x < clen ? x : x % clen);      // behind a circular record's origin only
+            } else if constexpr (kMode == ALN_TRX) {            // a chain's exon piece: the transcript's bases
+                off = wk.at;
+                exact = true;
             } else if constexpr (kMode == ALN_LIFT) {
                 // haplotype h's segments alternate stretch, variant, ..., stretch from lift.first[h] = 2 var_off[h] + h, so
                 // segment s is a variant when s - h is odd, and then it is variant (s - h - 1) / 2 in NsVariants order (the
@@ -692,7 +820,7 @@ struct AlnWrite {
                 comp = wk.inv;
                 off = wk.inv ? wk.start + wk.len - wk.t - len : wk.start + wk.t;
             }
-            if (!paired && src != ALN_SRC_LIT && aln_ref_plain(tg, rc, off, len)) {
+            if (!paired && !exact && src != ALN_SRC_LIT && aln_ref_plain(tg, rc, off, len)) {
                 if (src == ALN_SRC_MIS) nm += len;
                 return;
             }
@@ -720,7 +848,7 @@ struct AlnWrite {
         b.span = rf1 - rf0;
         b.n_cig = w - w0;
         uint64_t p;
-        if constexpr (kMode != ALN_PLAIN) {
+        if constexpr (kMode == ALN_LIFT || kMode == ALN_SPLICE) {
             b.ref_id = kMode == ALN_LIFT ? lift.hap_chrom[chrom] : chrom;
             p = inv ? at - b.span : at;
             if (inv) {
@@ -731,6 +859,8 @@ struct AlnWrite {
                     cig[y] = c;
                 }
             }
+        } else if (kMode == ALN_TRX && chain) {
+            p = at;
         } else {
             p = ((uint64_t)pos + rf0) % clen;                   // a part behind a circular record's origin starts past it
         }
@@ -741,7 +871,7 @@ struct AlnWrite {
         if constexpr (kMode == ALN_SPLICE) b.flag |= (uint16_t)((uint32_t)inv << BAM_HP_SHIFT);
         b.cig_off = cig_off + w0;
         rec[n_aln] = b;
-        size[n_aln] = bam_mapped_size(nl, b, kMode != ALN_PLAIN ? 4 : 0);
+        size[n_aln] = bam_mapped_size(nl, b, aln_lead_aux(kMode) ? 4 : 0);
         if constexpr (kTags) nm_out[n_aln] = nm;
         ++n_aln;
     }
@@ -792,7 +922,7 @@ __global__ void aln_write_tags_kernel(AlnArgs a, AlnTagArgs tg) {
 
 // ---------------------------------------------------------------------------------------------------------------------
 // aux fields with NM and SA, one thread per read over its records (DESIGN §3 "NM and SA tags"): a mapped record's are
-// HP:C (lift) or XS:A (splice), NM:I, and SA:Z when the read has more than one record, with one entry
+// HP:C (lift) or XS:A (splice) when aln_lead_aux, NM:I, and SA:Z when the read has more than one record, with one entry
 // "rname,pos,strand,CIGAR,60,NM;" for each of its other records in record order.  CG:B,I follows in BgzfTaggedLayout.
 // ---------------------------------------------------------------------------------------------------------------------
 struct AlnAuxArgs {
@@ -857,7 +987,7 @@ __global__ void aln_aux_size_kernel(AlnAuxArgs x) {
         x.aux_len[r0] = 0;
         return;
     }
-    const uint32_t hp = x.mode != ALN_PLAIN ? 4 : 0;
+    const uint32_t hp = aln_lead_aux(x.mode) ? 4 : 0;
     uint64_t all = 0;                                           // every record's SA entry
     if (k > 1)
         for (uint64_t j = 0; j < k; ++j) all += x.aux_len[r0 + j] = aln_sa_len(x, x.aln[r0 + j], x.nm[r0 + j]);
@@ -876,7 +1006,7 @@ __global__ void aln_aux_write_kernel(AlnAuxArgs x) {
     for (uint64_t j = 0; j < k; ++j) {
         const BamAln b = x.aln[r0 + j];
         uint8_t* p = x.aux + x.aux_off[r0 + j];
-        if (x.mode != ALN_PLAIN) {
+        if (aln_lead_aux(x.mode)) {
             const uint32_t v = b.flag >> BAM_HP_SHIFT;
             p[0] = x.mode == ALN_LIFT ? 'H' : 'X';
             p[1] = x.mode == ALN_LIFT ? 'P' : 'S';

@@ -1922,31 +1922,13 @@ static int compress_records(NsContext* ctx, const char* fname, const char* names
     return end_members(ctx, fname, ctx->h_totals.as<uint64_t>()[NS_T_Z_TEXT], src, ctx->z_out, nbytes);
 }
 
-}  // extern "C++"
-
-int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
-    return compress_records<BgzfTextLayout>(ctx, "ns_compress_records", names, name_off, nbytes);
-}
-
-int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
-    return compress_records<BgzfBamLayout>(ctx, "ns_compress_bam", names, name_off, nbytes);
-}
-
-int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
-    static const char* fname = "ns_compress_bam_mapped";
-    if (int rc = check_compress(ctx, fname, names, name_off, nbytes, "alignment")) return rc;
+// ns_compress_bam_mapped and ns_compress_bam_transcript after their checks: the last aligned batch's records by the walk
+// `mode` as BGZF members in z_out.  n_ids: the records' refIDs, for which NM and SA (ns_set_aln_tags) need one name each.
+static int compress_aln(NsContext* ctx, const char* fname, AlnMode mode, uint64_t n_ids, const char* names, const uint64_t* name_off,
+                        uint64_t* nbytes) {
     const Tables& tab = *ctx->tables;
-    // the walk: spliced onto the genome in transcriptome mode, lifted onto the haploid records after ns_set_lift, else plain
-    const AlnMode mode = ctx->hcfg.mode == 2 ? ALN_SPLICE : tab.have_lift ? ALN_LIFT : ALN_PLAIN;
-    if (mode == ALN_SPLICE && !tab.have_splice)
-        return fail(ctx, NS_EINVAL, "%s: transcriptome reads are written as mapped records only with a splice map (ns_set_splice)", fname);
-    if (mode == ALN_SPLICE && ctx->hcfg.trx_records && (tab.splice_n_trx != ctx->hcfg.trx_records || tab.splice_genome_first != ctx->hcfg.trx_records))
-        return fail(ctx, NS_EINVAL, "%s: the splice map's transcripts and genome records are not the run's (trx_records %u)", fname,
-                    ctx->hcfg.trx_records);
-    if (mode == ALN_LIFT && ctx->hcfg.circular) return fail(ctx, NS_EINVAL, "%s: lifted records need linear haplotype records", fname);
     // NM and SA (ns_set_aln_tags): the header's names must be the records' refIDs
     const bool tags = tab.have_aln_tags;
-    const uint64_t n_ids = mode == ALN_SPLICE ? tab.splice_n_genome : mode == ALN_LIFT ? tab.h_haploid_off.size() - 1 : tab.dref.n_chrom;
     if (tags && tab.tag_n_sn != n_ids)
         return fail(ctx, NS_EINVAL, "%s: ns_set_aln_tags gave %u reference names for %llu reference records", fname, tab.tag_n_sn,
                     (unsigned long long)n_ids);
@@ -1975,13 +1957,16 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
     auto run = [&](auto walk) -> int {
         constexpr AlnMode kMode = decltype(walk)::value;
         using Layout = std::conditional_t<kMode == ALN_LIFT, BgzfLiftedLayout,
-                                          std::conditional_t<kMode == ALN_SPLICE, BgzfSplicedLayout, BgzfMappedLayout>>;
+                                          std::conditional_t<kMode == ALN_SPLICE, BgzfSplicedLayout, BgzfMappedLayout>>;   // ALN_TRX: plain
         if constexpr (kMode == ALN_LIFT)
             aa.lift = AlnLift{tab.lift_seg.as<HapLift>(), tab.lift_kind.as<uint8_t>(), tab.lift_first.as<uint64_t>(),
                               tab.lift_chrom.as<uint32_t>(), tab.lift_hp.as<uint8_t>()};
-        if constexpr (kMode == ALN_SPLICE)
-            aa.splice = AlnSplice{tab.splice_exon.as<SpliceExon>(), tab.splice_first.as<uint64_t>(), tab.splice_minus.as<uint8_t>(),
-                                  tab.splice_n_trx, tab.splice_genome_first};
+        // ALN_TRX: only the chains of intron retention read the map; without it the walk sees none (n_trx 0)
+        if constexpr (kMode == ALN_SPLICE || kMode == ALN_TRX) {
+            if (kMode == ALN_SPLICE || ctx->hcfg.trx_records)
+                aa.splice = AlnSplice{tab.splice_exon.as<SpliceExon>(), tab.splice_first.as<uint64_t>(), tab.splice_minus.as<uint8_t>(),
+                                      tab.splice_n_trx, tab.splice_genome_first};
+        }
         CK(launch(ctx, aln_count_kernel<kMode>, grid, 256, 0, aa));
         if (int rc = scan_total(ctx, aa.n_rec, rec_first, n, NS_T_M_RECORDS)) return rc;
         if (int rc = scan_total(ctx, aa.n_cig, rec_first + n, n, NS_T_M_CIGAR_WORDS)) return rc;
@@ -2044,9 +2029,53 @@ int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* na
         src.n_recs = (uint32_t)n_rec;
         return end_members(ctx, fname, h[NS_T_Z_TEXT], src, ctx->z_out, nbytes);
     };
+    // ALN_TRX last: the other walks keep their order of instantiation, on which ptxas' register allocation of the
+    // deflate instantiations depends
     if (mode == ALN_SPLICE) return run(std::integral_constant<AlnMode, ALN_SPLICE>{});
     if (mode == ALN_LIFT) return run(std::integral_constant<AlnMode, ALN_LIFT>{});
-    return run(std::integral_constant<AlnMode, ALN_PLAIN>{});
+    if (mode == ALN_PLAIN) return run(std::integral_constant<AlnMode, ALN_PLAIN>{});
+    return run(std::integral_constant<AlnMode, ALN_TRX>{});
+}
+
+}  // extern "C++"
+
+int ns_compress_records(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    return compress_records<BgzfTextLayout>(ctx, "ns_compress_records", names, name_off, nbytes);
+}
+
+int ns_compress_bam(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    return compress_records<BgzfBamLayout>(ctx, "ns_compress_bam", names, name_off, nbytes);
+}
+
+int ns_compress_bam_mapped(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    static const char* fname = "ns_compress_bam_mapped";
+    if (int rc = check_compress(ctx, fname, names, name_off, nbytes, "alignment")) return rc;
+    const Tables& tab = *ctx->tables;
+    // the walk: spliced onto the genome in transcriptome mode, lifted onto the haploid records after ns_set_lift, else plain
+    const AlnMode mode = ctx->hcfg.mode == 2 ? ALN_SPLICE : tab.have_lift ? ALN_LIFT : ALN_PLAIN;
+    if (mode == ALN_SPLICE && !tab.have_splice)
+        return fail(ctx, NS_EINVAL, "%s: transcriptome reads are written as mapped records only with a splice map (ns_set_splice)", fname);
+    if (mode == ALN_SPLICE && ctx->hcfg.trx_records && (tab.splice_n_trx != ctx->hcfg.trx_records || tab.splice_genome_first != ctx->hcfg.trx_records))
+        return fail(ctx, NS_EINVAL, "%s: the splice map's transcripts and genome records are not the run's (trx_records %u)", fname,
+                    ctx->hcfg.trx_records);
+    if (mode == ALN_LIFT && ctx->hcfg.circular) return fail(ctx, NS_EINVAL, "%s: lifted records need linear haplotype records", fname);
+    const uint64_t n_ids = mode == ALN_SPLICE ? tab.splice_n_genome : mode == ALN_LIFT ? tab.h_haploid_off.size() - 1 : tab.dref.n_chrom;
+    return compress_aln(ctx, fname, mode, n_ids, names, name_off, nbytes);
+}
+
+int ns_compress_bam_transcript(NsContext* ctx, const char* names, const uint64_t* name_off, uint64_t* nbytes) {
+    static const char* fname = "ns_compress_bam_transcript";
+    if (int rc = check_compress(ctx, fname, names, name_off, nbytes, "alignment")) return rc;
+    const Tables& tab = *ctx->tables;
+    if (ctx->hcfg.mode != 2) return fail(ctx, NS_EINVAL, "%s: transcript-coordinate records need a transcriptome context", fname);
+    // with intron retention the reads laid out on the genome are composed with the splice map, which must be the run's
+    const uint32_t n_trx = ctx->hcfg.trx_records;
+    if (n_trx && !tab.have_splice)
+        return fail(ctx, NS_EINVAL, "%s: reads that retain an intron are written as mapped records only with a splice map (ns_set_splice)",
+                    fname);
+    if (n_trx && (tab.splice_n_trx != n_trx || tab.splice_genome_first != n_trx))
+        return fail(ctx, NS_EINVAL, "%s: the splice map's transcripts and genome records are not the run's (trx_records %u)", fname, n_trx);
+    return compress_aln(ctx, fname, ALN_TRX, n_trx ? n_trx : tab.dref.n_chrom, names, name_off, nbytes);
 }
 
 int ns_fetch_compressed(NsContext* ctx, uint8_t* out, uint64_t cap) {

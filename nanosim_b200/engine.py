@@ -113,7 +113,8 @@ class Engine:
 
     def set_splice(self, m):
         """transcriptome --spliced_bam: keeps the transcripts' exons on the genome records (a splice.SpliceMap; ns_set_splice),
-        so that compress_bam_mapped() writes the reads' spliced alignments to the genome.  Call before clone().  Returns the
+        so that compress_bam_mapped() writes the reads' spliced alignments to the genome (and compress_bam_transcript()
+        places the reads that retain an intron on their transcripts).  Call before clone().  Returns the
         device bytes the map keeps."""
         n = C.c_uint64()
         arrs = [np.ascontiguousarray(x, dtype=d) for x, d in ((m.exon_off, np.uint64), (m.exon_chrom, np.uint32), (m.exon_start, np.uint32),
@@ -328,8 +329,17 @@ class Engine:
         self._z_bytes = self._compress("compress_bam_mapped", names)
         return self._z_bytes
 
+    def compress_bam_transcript(self, names):
+        """The last aligned batch of a transcriptome run as mapped BAM records against the transcripts, the true alignment of
+        every read (``names`` as for compress_bam), as BGZF members built on the device and kept there
+        (ns_compress_bam_transcript); they replace those of the last compress_records() / compress_bam().  With intron
+        retention set_splice() must come first: the reads that retain an intron are composed with it.  Returns their size
+        in bytes; neither the BAM header nor the end-of-file block."""
+        self._z_bytes = self._compress("compress_bam_transcript", names)
+        return self._z_bytes
+
     def fetch_compressed(self, out=None):
-        """The members of the last compress_records(), compress_bam() or compress_bam_mapped() -> uint8 array (into ``out`` when given: a
+        """The members of the last compress_records(), compress_bam(), compress_bam_mapped() or compress_bam_transcript() -> uint8 array (into ``out`` when given: a
         uint8 array, pinned memory recommended, at least that large)."""
         if out is None:
             out = np.empty(self._z_bytes, dtype=np.uint8)

@@ -56,14 +56,15 @@ class BatchPipeline:
     names as ``batch.names``.  compress_profile (compressed mode, aligned batches): the error profile is formatted and
     compressed on the device as well (ns_compress_error_profile); its members arrive as ``batch.gz_err``.  bam
     (compressed mode): the records are unaligned BAM records (ns_compress_bam) instead of FASTA/FASTQ text.  mapped_bam (with
-    bam): aligned batches are written as mapped BAM records (ns_compress_bam_mapped), unaligned ones stay unmapped."""
+    bam): aligned batches are written as mapped BAM records (ns_compress_bam_mapped), unaligned ones stay unmapped;
+    transcript_bam (with mapped_bam): against the transcripts (ns_compress_bam_transcript)."""
 
     def __init__(self, engine, depth=2, fetch=True, want_ops=False, want_pieces=True, compress=None, compress_profile=False,
-                 bam=False, mapped_bam=False):
+                 bam=False, mapped_bam=False, transcript_bam=False):
         self.engines = [engine] + [engine.clone() for _ in range(max(1, depth) - 1)]
         self.depth = len(self.engines)
         self.fetch, self.want_ops, self.want_pieces, self.compress = fetch, want_ops, want_pieces, compress
-        self.compress_profile, self.bam, self.mapped_bam = compress_profile, bam, mapped_bam
+        self.compress_profile, self.bam, self.mapped_bam, self.transcript_bam = compress_profile, bam, mapped_bam, transcript_bam
         self.bufs = [_HostBuffers(engine.fastq) for _ in self.engines]
         self.hint = {"seq": 0, "qual": 0, "reads": 0, "pieces": 0, "ops": 0, "gz": 0, "gz_err": 0}     # largest batch seen by any slot (pinned allocs are slow)
 
@@ -117,7 +118,12 @@ class BatchPipeline:
         b.names = self.compress(b, job)
         if self.bam:
             mapped = self.mapped_bam and kind == L.NS_KIND_ALIGNED
-            nz = eng.compress_bam_mapped(b.names) if mapped else eng.compress_bam(b.names)
+            if not mapped:
+                nz = eng.compress_bam(b.names)
+            elif self.transcript_bam:
+                nz = eng.compress_bam_transcript(b.names)
+            else:
+                nz = eng.compress_bam_mapped(b.names)
         else:
             nz = eng.compress_records(b.names)
         if nz > self.hint["gz"]:

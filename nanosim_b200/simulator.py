@@ -148,7 +148,7 @@ class _RemoteReference(PackedReference):
 
 def read_profile(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                  polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                 device=0, seed=0, ir_files=None, ref_on_host=True, vcf=None, lift=False, spliced=False):
+                 device=0, seed=0, ir_files=None, ref_on_host=True, vcf=None, lift=False, spliced=False, transcript=False):
     """read_profile (:244-591).  Under torchrun (WORLD_SIZE > 1) only rank 0 reads the reference files; the other ranks get
     names and offsets through torch.distributed and the bases through ONE NCCL broadcast into their HBM (ns_bcast_nccl).
     ref_on_host: those ranks also copy the bases back to the host, which only the plain error profile's formatter reads.
@@ -157,14 +157,16 @@ def read_profile(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=
     and with ref_on_host copies them back to the host.  lift (``--lift_mapped_bam``): every rank also keeps the lift of the
     haplotypes onto the haploid records (ns_set_lift), so that mapped BAM records are against those.  spliced
     (transcriptome ``--spliced_bam``): rank 0 also builds the transcripts' map onto the genome records (prof.splice) and
-    their header list (prof.spliced_refs) and hands both to the other ranks."""
+    their header list (prof.spliced_refs) and hands both to the other ranks.  transcript (transcriptome ``--transcript_bam``)
+    with intron retention: rank 0 builds the same map (prof.splice), which places the reads that retain an intron on their
+    transcripts."""
     rank, world = _dist_world()
     if world > 1:
         return _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun,
                                          polya, exp, model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host, vcf,
-                                         lift, spliced)
+                                         lift, spliced, transcript)
     prof = _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
-                               chimeric, homopolymer, fastq, device, seed, ir_files, vcf, spliced)
+                               chimeric, homopolymer, fastq, device, seed, ir_files, vcf, spliced, transcript)
     if prof.haplotypes is not None:
         _apply_variants(prof, prof.haplotypes, ref_on_host, lift)
     return prof
@@ -191,12 +193,12 @@ def _apply_variants(prof, tables, ref_on_host, lift=False):
 
 def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp,
                               model_ir, chimeric, homopolymer, fastq, device, seed, ir_files, ref_on_host=True, vcf=None, lift=False,
-                              spliced=False):
+                              spliced=False, transcript=False):
     dist = _dist_init()
     box = [None]
     if rank == 0:
         prof = _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t, dna_type, abun, polya, exp, model_ir,
-                                   chimeric, homopolymer, fastq, device, seed, ir_files, vcf, spliced)
+                                   chimeric, homopolymer, fastq, device, seed, ir_files, vcf, spliced, transcript)
         r = prof.ref
         box[0] = {"names": r.names, "raw": r.raw_names, "offsets": r.offsets, "haplotypes": prof.haplotypes,
                   "meta": (r.species, r.chrom_species, r.chrom_circular, r.chrom_keys) if mode == "metagenome" else None,
@@ -251,7 +253,7 @@ def _read_profile_distributed(rank, world, ref_g, number_list, model_prefix, per
 
 def _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness, ref_t=None, dna_type=None, abun=None,
                         polya=None, exp=None, model_ir=False, chimeric=False, homopolymer=False, fastq=False,
-                        device=0, seed=0, ir_files=None, vcf=None, spliced=False):
+                        device=0, seed=0, ir_files=None, vcf=None, spliced=False, transcript=False):
     prof = Profile()
     prof.ir = None
     prof.n_trx = 0
@@ -309,6 +311,8 @@ def _read_profile_local(ref_g, number_list, model_prefix, per, mode, strandness,
                 prof.polya_flags = np.concatenate([prof.polya_flags, np.zeros(len(genome.names), dtype=np.uint8)])
         if spliced:
             _splice_profile(prof, ref_g, _gff3_path(model_prefix, ir_files), st if model_ir else None, genome if model_ir else None)
+        elif transcript and model_ir:
+            _splice_map(prof, st, genome, _gff3_path(model_prefix, ir_files), "those of their reads that retain an intron are written unmapped")
     else:
         prof.ref = PackedReference.from_fasta(ref_g)
     if mode != "transcriptome":
@@ -359,7 +363,6 @@ def _splice_profile(prof, ref_g, gff3, st=None, genome=None):
     are those it read, and the genome is resident behind the transcripts; without it only the genome's record names and
     lengths are kept (its bases never reach the device) and the GFF3 is read here."""
     from .intron_retention import TranscriptStructures
-    from .splice import build_splice_map
     n_trx = prof.n_trx or len(prof.ref.names)
     if genome is None:
         g = PackedReference.from_fasta(ref_g)
@@ -372,10 +375,18 @@ def _splice_profile(prof, ref_g, gff3, st=None, genome=None):
     if st is None:
         _log("Read in GFF3 annotation file")
         st = TranscriptStructures.from_gff3(gff3, prof.ref.names[:n_trx], genome.raw_names)
+    _splice_map(prof, st, genome, gff3, "their reads are written unmapped")
+
+
+def _splice_map(prof, st, genome, gff3, unmapped):
+    """The map of the transcript records (the first ones of prof.ref) onto the genome records by the structures st
+    (prof.splice); the start-up log counts the expressed transcripts without one and says which of their reads
+    (``unmapped``) that leaves unmapped."""
+    from .splice import build_splice_map
+    n_trx = prof.n_trx or len(prof.ref.names)
     prof.splice = build_splice_map(st, prof.ref.lengths[:n_trx], genome.lengths, n_trx if prof.n_trx else None)
     expressed = np.unique(np.asarray(prof.expr_chrom, dtype=np.int64))
-    _log("%d expressed transcripts have no usable exon structure in %s: their reads are written unmapped"
-         % (int((~prof.splice.has_map()[expressed]).sum()), gff3))
+    _log("%d expressed transcripts have no usable exon structure in %s: %s" % (int((~prof.splice.has_map()[expressed]).sum()), gff3, unmapped))
 
 
 def _shard(n, rank, world):
@@ -388,10 +399,11 @@ def _shard(n, rank, world):
 def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min_l, num_threads, fastq,
                median_l=None, sd_l=None, model_ir=False, uracil=False, polya=None, chimeric=False,
                batch_reads=65536, error_profile=True, rank=0, world=1, gzip=False, gzip_error_profile=False, bam=False,
-               mapped_refs=None):
+               mapped_refs=None, transcript_bam=False):
     """gzip: write the reads as BGZF (``.gz``), compressed on the GPU; bam: write them as unaligned BAM (``.bam``, one
     unmapped record per read), encoded and compressed on the GPU.  mapped_refs (with bam; bam_refs' list): the aligned
-    reads are written as mapped records, their true alignments to those records (``--mapped_bam``).  The error profile stays plain text unless
+    reads are written as mapped records, their true alignments to those records (``--mapped_bam``); transcript_bam
+    (transcriptome ``--transcript_bam``): to the transcript records, mapped_refs listing those.  The error profile stays plain text unless
     gzip_error_profile (needs gzip or bam): then it is formatted and compressed on the GPU too,
     ``<out>_aligned_error_profile.gz``, whose first member is the header line.  Under torchrun (world > 1) the per-rank
     files carry neither the headers nor the end-of-file block: merge_rank_files writes them."""
@@ -411,7 +423,7 @@ def simulation(prof, mode, out, dna_type, per, kmer_bias, basecaller, max_l, min
     gz_err = (gzip or bam) and gzip_error_profile and want_err
     files = output_files(fastq, gzip, gz_err, bam, mapped_refs)
     pipe = BatchPipeline(eng, depth=2, fetch=True, want_ops=want_err and not gz_err, compress_profile=gz_err, bam=bam,
-                         mapped_bam=mapped_refs is not None)
+                         mapped_bam=mapped_refs is not None, transcript_bam=transcript_bam)
     totals = {"reads": 0, "bases": 0, "bytes": 0}
     try:
         _simulation_body(prof, pipe, out, per, fastq, meta, trx, files, want_err, world, rank, batch_reads, fmt_threads, totals)
@@ -553,8 +565,13 @@ LIFT_HELP = ('With --vcf and --mapped_bam: write the true alignments in <out>_al
              'an aligner or a VCF names them) instead of the haplotype records: variants become CIGAR operations, <INV> and '
              '<DUP> split alignments, and every record has HP:C:1 or HP:C:2 for its haplotype. Read names and the error '
              'profile stay in haplotype coordinates (Default = False)')
-ALN_TAGS_HELP = ('With --mapped_bam (genome, metagenome; lifted or not) or --spliced_bam (transcriptome): give every mapped '
-                 'record of <out>_aligned_reads.bam NM:I (edit distance to the reference bases, as samtools calmd counts it) '
+TRANSCRIPT_BAM_HELP = ('With --bam: write <out>_aligned_reads.bam as mapped records, the true alignment of every aligned read '
+                       'to the -rt transcript it was simulated from, built on the GPU. Bases of a retained intron are '
+                       'insertions; with intron retention (the default) the exons of the GFF3 place those reads on the '
+                       'transcript. Cannot be combined with --spliced_bam. Read names, the error profile and '
+                       '<out>_unaligned_reads.bam are unchanged (Default = False)')
+ALN_TAGS_HELP = ('With --mapped_bam (genome, metagenome; lifted or not) or --spliced_bam / --transcript_bam (transcriptome): '
+                 'give every mapped record of <out>_aligned_reads.bam NM:I (edit distance to the reference bases, as samtools calmd counts it) '
                  'and, for a read with more than one record, SA:Z listing its other records, computed on the GPU. '
                  'Nothing else in the output changes (Default = False)')
 
@@ -707,6 +724,7 @@ def build_parser():
     t.add_argument('--bam', help=BAM_HELP, action='store_true', default=False)
     t.add_argument('--mapped_bam', help=argparse.SUPPRESS, action='store_true', default=False)     # a usage error here
     t.add_argument('--spliced_bam', help=SPLICED_BAM_HELP, action='store_true', default=False)
+    t.add_argument('--transcript_bam', help=TRANSCRIPT_BAM_HELP, action='store_true', default=False)
     t.add_argument('--aln_tags', help=ALN_TAGS_HELP, action='store_true', default=False)
     return parser, g, mg, t
 
@@ -749,8 +767,8 @@ def main_transcriptome(args, parser_t):
         parser_t.print_help(sys.stderr)
         sys.exit(1)
     gff3 = _gff3_path(args.model_prefix, {"gff3": args.ir_gff3})
-    if args.spliced_bam and not os.path.exists(gff3):
-        sys.stderr.write("\n--spliced_bam: the GFF3 annotation %s does not exist!\n" % gff3)
+    if (args.spliced_bam or (args.transcript_bam and model_ir)) and not os.path.exists(gff3):
+        sys.stderr.write("\n%s: the GFF3 annotation %s does not exist!\n" % ("--spliced_bam" if args.spliced_bam else "--transcript_bam", gff3))
         parser_t.print_help(sys.stderr)
         sys.exit(1)
     rank = int(os.environ.get("RANK", "0"))
@@ -765,11 +783,16 @@ def main_transcriptome(args, parser_t):
                         ref_t=args.ref_t, dna_type="linear", model_ir=model_ir, polya=args.polya, exp=args.exp,
                         homopolymer=args.homopolymer, fastq=args.fastq, device=device, seed=args.seed or 0,
                         ir_files={"markov": args.ir_markov_model, "gff3": args.ir_gff3}, ref_on_host=_plain_error_profile(args),
-                        spliced=args.spliced_bam)
+                        spliced=args.spliced_bam, transcript=args.transcript_bam)
     mapped_refs = None
     if args.spliced_bam:
         prof.engine.set_splice(prof.splice)
         mapped_refs = prof.spliced_refs
+        _set_aln_tags(args, prof, mapped_refs)
+    elif args.transcript_bam:
+        mapped_refs = _transcript_refs(prof)
+        if prof.ir is not None:
+            prof.engine.set_splice(prof.splice)
         _set_aln_tags(args, prof, mapped_refs)
     if args.coverage is not None:
         number[0] = coverage_to_reads(prof, prof.tables.cm, args.coverage)
@@ -778,7 +801,8 @@ def main_transcriptome(args, parser_t):
     simulation(prof, "transcriptome", args.output, "transcriptome", args.perfect, args.KmerBias if args.homopolymer else None,
                args.basecaller, max_len, min_len, max(args.num_threads, 1), args.fastq, None, None, model_ir, args.uracil,
                args.polya, batch_reads=args.batch_reads, error_profile=not args.no_error_profile, rank=rank, world=world,
-               gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam, mapped_refs=mapped_refs)
+               gzip=args.gzip, gzip_error_profile=args.gzip_error_profile, bam=args.bam, mapped_refs=mapped_refs,
+               transcript_bam=args.transcript_bam)
     if world > 1:
         import torch.distributed as dist
         if not dist.is_initialized():
@@ -872,6 +896,18 @@ def coverage_to_reads(prof, cm, coverage):
     return int(ref_len / mean * coverage)
 
 
+def _transcript_refs(prof):
+    """--transcript_bam: bam_refs of the transcript records (the first prof.n_trx of the resident reference with intron
+    retention, which puts the genome behind them, else all of them); a repeated name is a usage error."""
+    ref = prof.ref
+    n = prof.n_trx or len(ref.names)
+    try:
+        return bam_refs(_RemoteReference(ref.names[:n], np.asarray(ref.offsets)[:n + 1], ref.raw_names[:n]))
+    except ValueError as e:
+        sys.stderr.write("\n--transcript_bam: %s!\n" % e)
+        sys.exit(1)
+
+
 def _mapped_refs(args, prof, circular):
     """--mapped_bam: bam_refs of the resident reference (of the haploid one with --lift_mapped_bam), None without the flag;
     a repeated name is a usage error."""
@@ -898,19 +934,24 @@ def main(argv=None):
     elif args.gzip_error_profile and not (args.gzip or args.bam):
         usage = "--gzip_error_profile needs --gzip or --bam"
     elif args.mapped_bam and args.mode == "transcriptome":
-        usage = "--mapped_bam is not available in transcriptome mode: reads that retain an intron lie on the genome"
+        usage = ("--mapped_bam is not available in transcriptome mode: reads that retain an intron lie on the genome (--spliced_bam "
+                 "writes the alignments to the genome, --transcript_bam to the transcripts)")
     elif getattr(args, "spliced_bam", False) and not args.bam:
         usage = "--spliced_bam needs --bam"
     elif getattr(args, "spliced_bam", False) and not args.ref_g:
         usage = "--spliced_bam needs -rg: its records are against the genome"
+    elif getattr(args, "transcript_bam", False) and not args.bam:
+        usage = "--transcript_bam needs --bam"
+    elif getattr(args, "transcript_bam", False) and args.spliced_bam:
+        usage = "--transcript_bam and --spliced_bam both write <out>_aligned_reads.bam: give one of them (two runs with one --seed write the same reads)"
     elif args.mapped_bam and not args.bam:
         usage = "--mapped_bam needs --bam"
     elif getattr(args, "lift_mapped_bam", False) and not args.vcf:
         usage = "--lift_mapped_bam needs --vcf"
     elif getattr(args, "lift_mapped_bam", False) and not args.mapped_bam:
         usage = "--lift_mapped_bam needs --mapped_bam"
-    elif args.aln_tags and args.mode == "transcriptome" and not args.spliced_bam:
-        usage = "--aln_tags needs --spliced_bam in transcriptome mode"
+    elif args.aln_tags and args.mode == "transcriptome" and not (args.spliced_bam or args.transcript_bam):
+        usage = "--aln_tags needs --spliced_bam in transcriptome mode, or --transcript_bam"
     elif args.aln_tags and args.mode != "transcriptome" and not args.mapped_bam:
         usage = "--aln_tags needs --mapped_bam"
     if usage:
